@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
 """
-bench.py — headline benchmark of the B200 wavefront path tracer.
+bench.py — headline benchmark of the H100 wavefront path tracer.
 
 Metric (BASELINE.json): Mrays/s at 1920x1080, 8 bounces, 1 sample per pixel, where
   rays = sum_b N_ext[b] + sum_b N_shadow[b]   (rays actually submitted to BVH traversal, SURVEY 8d)
 A "step" is one frame: Reset + Integrate with sample_idx = 0, so every step traces identical rays.
 
-  python bench.py --gpus N --steps K --warmup W [--scene CornellBox] [--impl reference]
+  python bench.py --gpus N --steps K --warmup W [--scene CornellBox] [--impl reference] [--dump-outputs DIR]
 
 One process per GPU (torchrun for N > 1): the image is partitioned by scanline (row y -> rank y % N,
 weak in nothing: total work fixed => "strong" scaling), each rank runs the whole wavefront on its rows,
@@ -17,6 +17,8 @@ The JSON line carries: value (HBM-resident, device-timed, max over ranks), e2e (
 host buffers: camera upload + frame + resolve + device->host image), roofline (dominant kernel, algorithmic
 bytes / CUDA-event time vs MEASURED_PEAKS.json), cpu_baseline (the reference's own kernels compiled for the
 CPU, oracle/_ref, or the oracle port), clocks sampled during the timed region, gpu_launches.
+--dump-outputs DIR writes the accumulated radiance of the last timed step (what rt_integrate leaves for the caller, float32,
+the rows of this rank) and its per-bounce ray counts as DIR/*.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -87,7 +89,7 @@ def algorithmic_bytes(st, mb, n_pix):
 
 class ClockSampler(threading.Thread):
     """SM clock, power and throttle reasons sampled through NVML every ~2 ms DURING the timed region
-    (same quantities as the nvidia-smi line of B200_PROFILING.md; nvidia-smi itself is too slow for a ~40 ms region)."""
+    (the quantities of `nvidia-smi --query-gpu=clocks.sm,power.draw,clocks_event_reasons.active`, which is too slow for a ~40 ms region)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -143,7 +145,7 @@ def measured_peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s)"
 
 
 def issue_roofline(name, world, ktimes, steps, sm_mhz, n_sms, peak_hbm, alg_of):
@@ -199,7 +201,7 @@ def issue_roofline(name, world, ktimes, steps, sm_mhz, n_sms, peak_hbm, alg_of):
                     "traffic": d["traffic_bytes_per_launch"]})
     else:
         out.update({"bound": None, "achieved": None, "peak": None, "unit": None, "frac": None, "traffic": None,
-                    "note": f"no committed ncu counters for workload {name} in profiles/traffic.json"})
+                    "note": f"no ncu counters for workload {name} in profiles/traffic.json"})
     out["algorithmic"] = {"achieved_GBs": d["algorithmic_GBs"], "note": "SURVEY 8(d) byte model (48 B per BVH node visit / triangle test); "
                           "secondary figure, not a bound: node and triangle fetches are L1/L2 hits"}
     return out
@@ -307,6 +309,8 @@ def main():
     ap.add_argument("--no-overlap", action="store_true", help="RT_OPT_OVERLAP=0: shadow pass on the render stream (no concurrency with the next traversal)")
     ap.add_argument("--no-smem-bvh", action="store_true", help="RT_OPT_SMEM_BVH=0: fetch BVH records through L1 even for small scenes")
     ap.add_argument("--copies", type=int, default=183, help="Synthetic10M: number of ShaderBalls copies (183 = 10 026 570 triangles)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the radiance of the last timed step and its per-bounce ray counts to DIR/<name>.npy")
     args = ap.parse_args()
     workload = WORKLOADS[args.scene]
     if args.impl == "reference":
@@ -332,6 +336,23 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
 
     import types
+
+    def dump_outputs(ctx, mb):
+        """The arrays a caller of the timed path receives after its last step: the accumulated radiance (this rank's rows,
+        float32 RGBA; when the whole frame is above 48 MB, every k-th pixel of the rows, k fixed by the frame size so that all
+        ranks together stay under it, as an (n, 4) array) and the live-ray counts per bounce (float64).  The inputs are fixed
+        by the workload, so runs are comparable."""
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        sfx = "" if world == 1 else f"_rank{rank}"
+        rad = ctx.read_radiance()
+        rows = rad[rank::world] if world > 1 else rad
+        k = -(-rad.nbytes // (48 << 20))
+        if k > 1:
+            rows = rows.reshape(-1, 4)[::k]
+        np.save(os.path.join(args.dump_outputs, f"radiance{sfx}.npy"), np.ascontiguousarray(rows, dtype=np.float32))
+        st = ctx.frame_stats()
+        for k in ("n_ext", "n_shadow"):
+            np.save(os.path.join(args.dump_outputs, f"{k}{sfx}.npy"), st[k][: mb + 1].astype(np.float64))
 
     def device_run(workload, n_steps):
         """Scene upload, one counter frame, warm-up, n_steps device-timed frames (CUDA events on the context's stream, barrier +
@@ -423,6 +444,8 @@ def main():
                 sampler.err = repr(e)
         barrier()
         sampler.stop_flag = True
+        if args.dump_outputs and workload == WORKLOADS[args.scene]:
+            dump_outputs(ctx, mb)
         ms_total = torch.tensor([ev0.elapsed_time(ev1)], dtype=torch.float64, device=slab.device)
         if world > 1:
             dist.all_reduce(ms_total, op=dist.ReduceOp.MAX)
@@ -531,7 +554,7 @@ def main():
                 ctx.resolve_gathered(gather.recv_ptr, gather.recv_stride_bytes, host_np)
         if world > 1 and not parallel and R.fused is not None:
             dist.barrier()                             # the peers may not push the next frame into the buffer rank 0 is still presenting
-    e2e_steps = max(3, min(args.steps, 20))
+    e2e_steps = args.steps
 
     def time_e2e(parallel):
         for _ in range(3):
@@ -633,7 +656,7 @@ def main():
         sclk = S.sampler.summary()
         if rank == 0:
             s_peak, _ = measured_peak_hbm()
-            s_mhz = float(sclk.get("sm_mhz") or sclk.get("sm_max_mhz") or 1965.0)
+            s_mhz = float(sclk.get("sm_mhz") or sclk.get("sm_max_mhz") or 1980.0)
             _, sw, sh, smb = WORKLOADS[sec_name]
             secondary = {"metric": "Mrays/sec @1920x1080x8-bounce", "value": S.value, "unit": "Mrays/s", "n_gpus": world, "steps": args.secondary_steps,
                          "ms_per_step": S.ms_per_step, "config": {"workload": workload_string(sec_name, sw, sh, smb), "triangles": int(len(S.scene["triangles"])),
@@ -647,13 +670,13 @@ def main():
     if rank == 0:
         peak, peak_src = measured_peak_hbm()
         clk = sampler.summary()
-        sm_mhz = float(clk.get("sm_mhz") or clk.get("sm_max_mhz") or 1965.0)
+        sm_mhz = float(clk.get("sm_mhz") or clk.get("sm_max_mhz") or 1980.0)
         roof = issue_roofline(name, world, ktimes, args.steps, sm_mhz, R.n_sms, peak, alg_of)
         roof["peak_source"] = peak_src
         roof["algorithmic_bytes_per_step"] = alg_total
         roof["whole_frame_algorithmic_GBs"] = alg_total / (ms_per_step * 1e-3) / 1e9
         roof["how"] = ("kernel time: CUDA events of THIS run (per-launch, per-phase kernels, shadow pass as its own kernel); instruction and DRAM "
-                       "counters: committed ncu --set full capture of the same workload and kernels (profiles/); issue peak = SMs x 4 x SM clock")
+                       "counters: ncu --set full capture of the same workload and kernels (profiles/traffic.json, when present); issue peak = SMs x 4 x SM clock")
         line = {
             "metric": "Mrays/sec @1920x1080x8-bounce", "value": value, "unit": "Mrays/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
@@ -661,7 +684,7 @@ def main():
             "config": {"workload": workload_string(name, w, h, mb), "triangles": int(len(scene['triangles'])),
                        "schedule": R.schedule, "partition": f"scanline y%{world}",
                        "rays_per_step": rays_per_frame, "primary_hit_fraction": R.primary_hit_fraction,
-                       "l2": "per-step working set (ray/shadow queues + radiance, ~365 MB at 1080p) exceeds the 126 MB L2; no explicit flush"},
+                       "l2": "per-step working set (ray/shadow queues + radiance, ~365 MB at 1080p) exceeds the 50 MB L2; no explicit flush"},
             "e2e": {"value": e2e_value, "unit": "Mrays/s", "ms_per_step": float(e2e_ms[0]), "steps": e2e_steps,
                     "repetitions_ms_per_step": [round(x, 4) for x in e2e_reps], "h2d_bytes_per_step": 64,
                     "d2h_bytes_per_step": w * h * 16,          # the whole image reaches the host every step (N > 1: split over the ranks' links)

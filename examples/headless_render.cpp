@@ -10,7 +10,7 @@
  * The optional last argument spreads the frame over several GPUs of the node behind the same Render / Integrator objects
  * ("all" = every CUDA device; the image is partitioned by scanline inside the library, rt_create_multi).
  *
- * Needs a B200 (there is no CPU fallback: Render's constructor throws without a CUDA device).
+ * Needs an H100 (there is no CPU fallback: Render's constructor throws without a CUDA device).
  */
 #include <cstdio>
 #include <cstdlib>

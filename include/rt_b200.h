@@ -1,5 +1,5 @@
 /*
- * rt_b200.h — C ABI of the B200 (sm_100a) wavefront path-tracing backend.
+ * rt_b200.h — C ABI of the H100 (sm_90a) wavefront path-tracing backend.
  *
  * This shim takes the place of the reference's OpenCL wrapper layer
  *   /root/reference/src/gpu_wrappers/cl_context.hpp:37-99  (CLContext / CLKernel)
@@ -85,8 +85,8 @@ typedef enum RtOption {
     RT_OPT_FRAME_KERNEL = 26,   /* how rt_integrate runs a frame.  1: ONE persistent kernel in which every CTA is an independent
                                    wavefront over its own pixels (queue cursors in shared memory, no global atomics, no launch
                                    boundaries); 0: one kernel per phase (graph replay / PDL chain as configured above);
-                                   2 (default): the one-kernel frame for partitions of up to 7168 pixels per SM (half a 1080p
-                                   frame or less on a B200), per-phase kernels for larger ones.  Results are bit-identical */
+                                   2 (default): the one-kernel frame for partitions of up to 7168 pixels per SM (0.95 M pixels,
+                                   under half a 1080p frame, on an H100's 132 SMs), per-phase kernels for larger ones.  Results are bit-identical */
     RT_OPT_PRESENT = 27,        /* multi-device contexts, rt_resolve: 0 (default) parallel read-back of every device's rows,
                                    1 gather to devices[0] over NVLink, resolve and read back there */
     RT_OPT_FRAME_THREADS = 28,  /* threads per CTA of the one-kernel frame: 0 (default) by partition size, else a multiple of 32 <= 1024 */

@@ -10,7 +10,7 @@
  * glibc's libm also differ from each other by an ulp here and there, and a
  * path tracer is chaotic (one flipped comparison changes a pixel completely).
  * So the transcendental functions are restated ONCE, here, using only IEEE-754
- * +,-,*,/,sqrt on doubles (correctly rounded on both x86-64 and sm_100a when
+ * +,-,*,/,sqrt on doubles (correctly rounded on both x86-64 and sm_90a when
  * FMA contraction is off: gcc -ffp-contract=off, nvcc -fmad=false) and a final
  * round to float.  Results are within 1 ulp (almost always correctly rounded),
  * well inside the OpenCL 1.2 accuracy requirements (sin/cos/acos 4 ulp, tan 5,

@@ -142,6 +142,8 @@ public:
     Buf radiance_, resolved_, tap_hits_, tap_rays_;
     Buf diffuse_albedo_, depth_, normal_, velocity_;
     std::uint32_t SampleCount() const { return *(std::uint32_t*)sample_counter_.p; }
+    // sampler tables given by the caller instead of the compiled-in ones (ranking followed by 256 zeros, as PaddedRankingTile)
+    std::vector<int> own_sobol_, own_scrambling_, own_ranking_;
 
 protected:
     void CreateKernels() override {}   // variants are picked at call time from the option flags
@@ -203,7 +205,9 @@ protected:
         fn(N(), rays_[in].p, ray_counter_[in].p, pixel_indices_[in].p, hits_.p, scene_.triangles.data(),
             scene_.lights.data(), scene_.emissive.data(), scene_.materials.data(), scene_.textures.data(),
             scene_.texture_data.data(), bounce, width_, height_, sample_counter_.p, &scene_.info,
-            (void*)sobol_256spp_256d, (void*)scramblingTile, (void*)PaddedRankingTile(),
+            own_sobol_.empty() ? (void*)sobol_256spp_256d : (void*)own_sobol_.data(),
+            own_scrambling_.empty() ? (void*)scramblingTile : (void*)own_scrambling_.data(),
+            own_ranking_.empty() ? (void*)PaddedRankingTile() : (void*)own_ranking_.data(),
             throughputs_.p, rays_[out].p, ray_counter_[out].p, pixel_indices_[out].p,
             shadow_rays_.p, shadow_ray_counter_.p, shadow_pixel_indices_.p, direct_light_samples_.p, radiance_.p);
         if (bounce < (std::uint32_t)kMaxStatBounces)
@@ -358,6 +362,12 @@ void ref_enable_white_furnace(void* handle, int e) { ((RefHandle*)handle)->integ
 void ref_sampler_tables(const int** sobol, const int** scrambling, const int** ranking)
 {
     *sobol = (const int*)sobol_256spp_256d; *scrambling = (const int*)scramblingTile; *ranking = (const int*)rankingTile;
+}
+void ref_use_sampler_tables(void* handle, const int* sobol, const int* scrambling, const int* ranking)
+{
+    RefCpuIntegrator& it = *((RefHandle*)handle)->integrator;
+    it.own_sobol_.assign(sobol, sobol + 65536); it.own_scrambling_.assign(scrambling, scrambling + 131072);
+    it.own_ranking_.assign(ranking, ranking + 131072); it.own_ranking_.resize(131072 + 256, 0);
 }
 void ref_set_sampler(void* handle, int blue_noise) { ((RefHandle*)handle)->integrator->SetSamplerType(blue_noise ? Integrator::SamplerType::kBlueNoise : Integrator::SamplerType::kRandom); }
 void ref_enable_denoiser(void* handle, int e) { ((RefHandle*)handle)->integrator->EnableDenoiser(e != 0); }

@@ -49,6 +49,7 @@ class RefRenderer:
             getattr(L, name).argtypes = [C.c_void_p]
         L.ref_set_row_sample.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
         L.ref_sampler_tables.argtypes = [C.POINTER(C.POINTER(C.c_int))] * 3
+        L.ref_use_sampler_tables.argtypes = [C.c_void_p] * 4
         L.ref_read.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         self.h = None
         self.width = self.height = 0
@@ -102,6 +103,12 @@ class RefRenderer:
         ps = [C.POINTER(C.c_int)() for _ in range(3)]
         self.lib.ref_sampler_tables(*[C.byref(p) for p in ps])
         return tuple(np.ctypeslib.as_array(p, shape=(n,)).astype(np.int32) for p, n in zip(ps, (65536, 131072, 131072)))
+
+    def use_sampler_tables(self, tables):
+        """The blue-noise sampler reads these (sobol[65536], scrambling[131072], ranking[131072]) instead of its own; after begin()."""
+        t = [np.ascontiguousarray(a, dtype=np.int32) for a in tables]
+        self.lib.ref_use_sampler_tables(self.h, *[a.ctypes.data_as(C.c_void_p) for a in t])
+
     def enable_denoiser(self, e): self.lib.ref_enable_denoiser(self.h, int(e))
     def set_aov(self, a): self.lib.ref_set_aov(self.h, int(a))
     def set_row_sample(self, first, step): self.lib.ref_set_row_sample(self.h, first, step)

@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""Turn the ncu reports of profiles/run_ncu.sh (gpurun_out/prof_<workload>[_src|_frame|_frame8]_<tag>.ncu-rep) into the committed
+"""Turn the ncu reports of profiles/run_ncu.sh (<output directory>/prof_<workload>[_src|_frame|_frame8]_<tag>.ncu-rep) into the committed
 evidence: profiles/<tag>_<workload>_summary.txt (per-launch metrics + hottest source lines) and profiles/traffic.json — the
 per-frame instruction and DRAM counters of every kernel class that bench.py's roofline divides by its own CUDA-event times.
-usage: profiles/make_summaries.py <tag> [gpurun_out]"""
+usage: profiles/make_summaries.py <tag> [output directory of run_ncu.sh, default ncu_out]"""
 import csv
 import glob
 import json
@@ -12,7 +12,7 @@ import subprocess
 import sys
 
 tag = sys.argv[1]
-src = sys.argv[2] if len(sys.argv) > 2 else "gpurun_out"
+src = sys.argv[2] if len(sys.argv) > 2 else "ncu_out"
 HERE = os.path.dirname(os.path.abspath(__file__))
 CLASSES = {"k_trace_closest": "trace_closest", "k_shadow_accumulate": "shadow_accumulate", "k_shade_queues": "shade_queues",
            "k_trace_both": "trace_both", "k_frame": "frame"}

@@ -1,7 +1,7 @@
 /*
  * rt_device.cuh — device-side building blocks of the wavefront path tracer:
  * RNG, primary-ray generation, environment lookup, material unpacking, Lambert/GGX
- * evaluation and sampling, light sampling.  Written for sm_100a, compiled with
+ * evaluation and sampling, light sampling.  Written for sm_90a, compiled with
  * -fmad=false: every float operation is a separately rounded IEEE binary32 op in the
  * order written, transcendental functions come from include/rt_math.h, so results are
  * bit-identical to the reference semantics pinned by oracle/ (see DESIGN.md "Arithmetic
@@ -208,8 +208,7 @@ __device__ __forceinline__ f3 unpack_rgb8(uint32_t d)
 }
 
 // kernels/common/material.h:251-264 (OpenCL branch), utils.h:123-190
-// (inlined on purpose: as a called function it costs the hot path more (call ABI: registers, stack) than its size saves —
-// measured on B200, profiles/r02_code_size_ab.txt)
+// (inlined on purpose: as a called function it costs the hot path more (call ABI: registers, stack) than its size saves)
 __device__ __forceinline__ Material unpack_material(const DevScene& sc, uint32_t mtl_index, f2 uv)
 {
     const uint32_t* pm = sc.materials + (size_t)mtl_index * 5;

@@ -1,8 +1,8 @@
 /*
- * rt_kernels.cu — the sm_100a kernels of the wavefront path tracer and the C ABI
+ * rt_kernels.cu — the sm_90a kernels of the wavefront path tracer and the C ABI
  * (include/rt_b200.h) that launches them.  One translation unit so that the shading
  * code inlines into both the stepwise kernels (one per reference kernel) and the fused
- * ones.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false (see
+ * ones.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (see
  * __graft_entry__.build()).  There is no CPU fallback anywhere in this file.
  *
  * Data layout in HBM (all SoA streams of float4, indexed by compacted ray slot):
@@ -40,7 +40,7 @@
 using namespace rt;
 
 // minimum resident CTAs per SM requested from ptxas for the hot kernels (register budget = 65536 / (256 * N)):
-// tuned on B200, see DESIGN.md section 6
+// 5 x 256 threads at <= 48 registers and 4 x 256 at <= 64 fill the 64 K-register file of an SM (the same on H100), see DESIGN.md section 4
 #ifndef RT_MINB_TRACE
 #define RT_MINB_TRACE 5
 #endif
@@ -915,7 +915,7 @@ cudaError_t launch_chain(rt_ctx* c, void (*kernel)(KArgs...), int grid, size_t s
 //   mode 1  the whole structure (interior records + triangle records) when it fits 40 KB (5 resident CTAs x 40 KB stay under
 //           the 227 KB of an SM): CornellBox;
 //   mode 2  only the top of the tree — the first top_k interior records in breadth-first order (RT_OPT_TOP_SMEM records,
-//           default 0 = off, see DESIGN.md for the measurements) — when the structure does not fit;
+//           default 0 = off, DESIGN.md section 4 says why) — when the structure does not fit;
 //   mode 0  nothing staged: literal traversal (RT_OPT_TRAVERSAL 0), RT_OPT_SMEM_BVH off.
 struct Stage { int mode; size_t bytes; uint32_t top_k; };
 Stage bvh_stage(const rt_ctx* c)
@@ -1560,25 +1560,22 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
     return RT_OK;
 }
 
-// Which schedule rt_integrate runs, and the CTA shape of the one-kernel frame.  Measured on B200 (profiles/r02_frame_kernel_ab.txt,
-// ms per frame of a 1/world partition of the 1080p frame, per-phase kernels vs k_frame at its best CTA size):
-//   CornellBox   world 1: 2.141 / 2.181   2: 1.157 / 1.134   4: 0.657 / 0.611   8: 0.419 / 0.350
-//   ShaderBalls  world 1: 3.985 / 4.041   2: 2.485 / 2.452   4: 1.768 / 1.571   8: 1.406 / 1.106
-//   Dragon 4K    world 1: 24.74 / 26.59                                         8: 4.273 / 4.102
-// With a whole frame per GPU the per-phase kernels win by 2-7 % (specialised register budgets — 5 CTAs/SM of 48 registers for
-// traversal — and one kind of code per SM at a time); from half a 1080p frame down the launch boundaries and kernel tails of
-// 20+ dependent launches cost more and the one-kernel frame wins (1.2-1.3x on a 1/8 partition).  RT_OPT_FRAME_KERNEL = 2
-// switches at 7168 pixels per SM (1.06 M pixels on 148 SMs).
+// Which schedule rt_integrate runs, and the CTA shape of the one-kernel frame.  With a whole 1080p frame per GPU the per-phase
+// kernels are at least as fast (specialised register budgets — 5 CTAs/SM of 48 registers for traversal — and one kind of code per
+// SM at a time; on one H100 80GB HBM3: a tie within 1.5 % on CornellBox, 1 % ahead on ShaderBalls, DESIGN.md section 4); from
+// half a 1080p frame down the
+// launch boundaries and kernel tails of 20+ dependent launches cost more and the one-kernel frame wins.  RT_OPT_FRAME_KERNEL = 2
+// switches at 7168 pixels per SM (0.95 M pixels on 132 SMs).
 static bool frame_kernel_selected(const rt_ctx* c)
 {
     if (c->frame_kernel == 2) return (size_t)c->n_local <= (size_t)c->num_sms * 7168u;
     return c->frame_kernel == 1;
 }
 
-// CTA size of k_frame (same measurements).  One 1024-thread CTA per SM keeps all 32 warps of an SM in the same phase — one kind
+// CTA size of k_frame (measured during development on partitions of 1-8 GPUs, not re-measured on H100).  One 1024-thread CTA per SM keeps all 32 warps of an SM in the same phase — one kind
 // of code in the instruction caches — and is the best shape when the BVH lives in shared memory (CornellBox, every partition
 // size) or every warp still has several items per phase; scenes traversed through L1/L2 on small partitions (<= 4096 pixels
-// per SM) prefer 4 CTAs of 256 threads per SM whose phases interleave (ShaderBalls, 1/8 partition: 1.106 vs 1.252 ms).
+// per SM) prefer 4 CTAs of 256 threads per SM whose phases interleave.
 static int frame_kernel_threads(const rt_ctx* c)
 {
     if (c->frame_threads) return c->frame_threads;

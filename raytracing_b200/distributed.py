@@ -2,7 +2,7 @@
 Multi-GPU plumbing (one process per GPU, torch.distributed): the image is partitioned by scanline — row y
 belongs to rank y % world — every rank renders its rows with the scene replicated, and ONE gather of the
 radiance slabs to rank 0 ends the frame (BASELINE.json north_star; SURVEY 8e).  No other collective exists
-on the data path.  Backend "nccl" on the GPUs (NVLink 5 / NVSwitch), "gloo" in the CPU tests.
+on the data path.  Backend "nccl" on the GPUs (NVLink / NVSwitch), "gloo" in the CPU tests.
 
 A rank's slab is local_rows x width float4, local row r = image row rank + r * world.  Ranks can own one row
 less than rank 0 when world does not divide the height, so slabs are padded to rows_max for the gather.

@@ -55,7 +55,7 @@ void CUDAPathTraceIntegrator::SetResolveTarget(float* host_rgba, bool page_lock)
     resolve_target_locked_ = host_rgba && page_lock && rt_host_register(host_rgba, (std::uint64_t)width_ * height_ * 16) == RT_OK;
 }
 
-// Kernel variants are compiled ahead of time for sm_100a (there is no runtime compilation / hot reload,
+// Kernel variants are compiled ahead of time for sm_90a (there is no runtime compilation / hot reload,
 // cl_context.cpp:173-210); "creating the kernels" pushes the current option set to the context.
 void CUDAPathTraceIntegrator::CreateKernels()
 {

@@ -1,5 +1,5 @@
 /*
- * CUDAPathTraceIntegrator — the B200 backend behind the reference's Integrator interface, the
+ * CUDAPathTraceIntegrator — the H100 backend behind the reference's Integrator interface, the
  * counterpart of CLPathTraceIntegrator (/root/reference/src/integrator/cl_pt_integrator.hpp:31-125).
  * It owns an opaque rt_ctx and forwards every virtual step to the C ABI (include/rt_b200.h), which
  * takes the place of CLContext/CLKernel.  Errors come back as status codes and are re-thrown as

@@ -1,13 +1,13 @@
 /*
  * reference_api.hpp — the reference-facing C++ interface of the backend, in one header.
  *
- * The B200 backend is a drop-in behind the reference's own abstractions, so the host side mirrors three of them with
+ * The H100 backend is a drop-in behind the reference's own abstractions, so the host side mirrors three of them with
  * the same names, members and call contracts (paths relative to /root/reference/src):
  *   AccelerationStructure   acceleration_structure.hpp:31-38   BuildCPU reorders the triangles into leaf order
  *   Integrator              integrator/integrator.hpp:34-100, integrator.cpp:27-77
  *                           public interface + the 15 protected virtual steps + the fixed wavefront schedule Integrate()
  *   Scene                   scene/scene.hpp:34-67, scene/scene.cpp:46-361   OBJ/MTL -> the seven arrays the integrator uploads
- * A backend plugs in by deriving from Integrator (cuda_pt_integrator.hpp is the B200 one, next to the reference's
+ * A backend plugs in by deriving from Integrator (cuda_pt_integrator.hpp is the H100 one, next to the reference's
  * OpenCL and OpenGL backends); Bvh (bvh.hpp) derives from AccelerationStructure; Render (render.hpp) wires them up.
  */
 #pragma once

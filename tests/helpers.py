@@ -1,5 +1,8 @@
 """Shared helpers for the parity tests."""
 import glob
+import hashlib
+import json
+import lzma
 import os
 
 import numpy as np
@@ -35,7 +38,7 @@ def load_golden(path):
 
 def bits(a):
     """Bit pattern of a float32 array for exact comparisons.  NaNs are canonicalised first: the payload/sign of a NaN
-    produced by an invalid operation is not specified by IEEE 754 (x86 gives 0xFFC00000, sm_100a 0x7FFFFFFF)."""
+    produced by an invalid operation is not specified by IEEE 754 (x86 gives 0xFFC00000, sm_90a 0x7FFFFFFF)."""
     u = np.ascontiguousarray(a, dtype="<f4").copy().view("<u4")
     u[(u & 0x7FFFFFFF) > 0x7F800000] = 0x7FC00000
     return u
@@ -76,3 +79,40 @@ def fuzz_configs(n=12, seed=77):
     out.append(("CornellBox", 65, 33, 3, {"position": (0.0, -1.0, 1.0), "yaw": 1.5707963267948966, "pitch": 1.5707963267948966}, False))
     out.append(("ShaderBalls", 64, 48, 4, {"position": (0.0, 0.0, 3.0), "yaw": 0.0, "pitch": 3.14159265}, False))
     return out
+
+
+STAT_KEYS = ("n_ext", "n_miss", "n_hit", "n_shadow", "n_cont", "n_unoccluded")
+_ref_records = {}
+
+
+def digest(a):
+    """64 bits of the sha256 of an array's bytes: enough to tell two outputs apart, small enough to store per case."""
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()[:16]
+
+
+def frame_record(stats, mb, radiance, hits=None, keys=STAT_KEYS):
+    """What a parity test compares of one rendered sample: per-bounce counters, the bits of the radiance and (optionally) the
+    primary hits, the last two as digests."""
+    rec = {"stats": {k: [int(x) for x in stats[k][: mb + 1]] for k in keys}, "radiance": digest(bits(radiance[..., :3]))}
+    if hits is not None:
+        rec["hits"] = digest(np.ascontiguousarray(hits["primitive_id"], dtype="<u4"))
+    return rec
+
+
+def ref_records(name):
+    """{case: record} of what the reference's own code (oracle/_ref) produced for the cases of a test, as stored in
+    tests/golden/ref/<name> by tests/golden/make_ref_records.py."""
+    if name not in _ref_records:
+        with lzma.open(os.path.join(GOLDEN, "ref", name), "rt") as f:
+            _ref_records[name] = json.load(f)
+    return _ref_records[name]
+
+
+def assert_frames(key, records):
+    """records (one per sample) equal what the reference produced for the case `key`, field by field."""
+    want = ref_records("frames.json.xz")[key]
+    assert len(records) == len(want), key
+    for i, (got, ref) in enumerate(zip(records, want)):
+        assert set(got) == set(ref), (key, i)
+        for field in sorted(ref):
+            assert got[field] == ref[field], (key, "sample %d" % i, field)

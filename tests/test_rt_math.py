@@ -132,7 +132,7 @@ def test_rt_math_exact_building_blocks(host):
 @pytest.mark.gpu
 @pytest.mark.parametrize("fn", sorted(FN))
 def test_device_rt_math_equals_host_rt_math(host, fn):
-    """sm_100a (-fmad=false) and x86-64 (-ffp-contract=off) evaluate include/rt_math.h to the same bits."""
+    """sm_90a (-fmad=false) and x86-64 (-ffp-contract=off) evaluate include/rt_math.h to the same bits."""
     from raytracing_b200 import capi
     rng = np.random.default_rng(4321 + FN[fn])
     a, b = arguments(fn, rng)

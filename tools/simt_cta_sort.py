@@ -16,7 +16,7 @@ M = C.CDLL(lib_path)
 M.simt_model.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_int, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p]
 name = sys.argv[1] if len(sys.argv) > 1 else "CornellBox"
 w, h, mb = 960, 540, 4
-n_cta = int(sys.argv[2]) if len(sys.argv) > 2 else 148
+n_cta = int(sys.argv[2]) if len(sys.argv) > 2 else 132
 sc = scene_io.load_scene(name); o = Oracle(sc); cam = default_camera(w, h)
 nodes = np.ascontiguousarray(sc["nodes"]); tris = np.ascontiguousarray(sc["triangles"])
 costs = np.array([75.0, 24.0, 48.0, 66.0, 78.0, 90.0])
