@@ -546,7 +546,7 @@ typedef struct OrcScene
     RtSceneInfo info;
 } OrcScene;
 
-#define ORC_MAX_BOUNCES 64
+#define ORC_MAX_BOUNCES 256     /* per-bounce counters for bounces 0..RT_MAX_BOUNCES */
 typedef struct OrcStats
 {
     uint32_t n_ext[ORC_MAX_BOUNCES], n_miss[ORC_MAX_BOUNCES], n_hit[ORC_MAX_BOUNCES];

@@ -14,7 +14,7 @@ from .refbind import (CAMERA_DT, HIT_DT, LIGHT_DT, MATERIAL_DT, NODE_DT, RAY_DT,
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "liboracle.so")
-MAX_BOUNCES = 64
+MAX_BOUNCES = 256        # entries of the per-bounce counters: bounces 0..255, as the CUDA path (RT_MAX_BOUNCES)
 
 
 class OrcScene(C.Structure):

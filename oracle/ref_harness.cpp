@@ -85,7 +85,7 @@ struct SceneArrays
     SceneInfo info = {};
 };
 
-const int kMaxStatBounces = 64;
+const int kMaxStatBounces = 256;     // bounces 0..255, as the CUDA path (RT_MAX_BOUNCES)
 struct Stats
 {
     std::uint32_t n_ext[kMaxStatBounces], n_miss[kMaxStatBounces], n_hit[kMaxStatBounces];
@@ -377,7 +377,7 @@ void ref_request_reset(void* handle) { ((RefHandle*)handle)->integrator->Request
 void ref_integrate(void* handle) { ((RefHandle*)handle)->integrator->Integrate(); }
 
 // which: 0 radiance(float4/pixel) 1 resolved image(float4/pixel) 2 primary hits (Hit/ray) 3 primary rays (Ray/ray)
-//        4 stats (6 x 64 uint32) 5 sample count (1 uint32) 6 albedo(float4) 7 depth(float) 8 normal(float4) 9 velocity(float2)
+//        4 stats (6 x 256 uint32) 5 sample count (1 uint32) 6 albedo(float4) 7 depth(float) 8 normal(float4) 9 velocity(float2)
 int ref_read(void* handle, int which, void* dst)
 {
     RefHandle* h = (RefHandle*)handle;

@@ -126,7 +126,7 @@ class RefRenderer:
     def primary_rays(self): return self._read(3, RAY_DT, self.width * self.height)
 
     def stats(self) -> dict:
-        s = self._read(4, "<u4", 6 * 64).reshape(6, 64)
+        s = self._read(4, "<u4", 6 * 256).reshape(6, 256)
         return {k: s[i] for i, k in enumerate(("n_ext", "n_miss", "n_hit", "n_shadow", "n_cont", "n_unoccluded"))}
 
     def sample_count(self): return int(self._read(5, "<u4", 1)[0])

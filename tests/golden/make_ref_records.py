@@ -36,14 +36,17 @@ from tests import test_oracle_vs_ref as T  # noqa: E402
 from tests.helpers import bits, digest, frame_record, fuzz_configs, scene, synthetic_sampler_tables  # noqa: E402
 
 
-def ref_samples(sc, cam, w, h, mb, n, wf=False, with_hits=True, keys=None, tables=None):
+def ref_samples(sc, cam, w, h, mb, n, wf=False, with_hits=True, keys=None, tables=None, keep=None):
+    """Records of n accumulated samples of the reference's Integrate(), or of the samples (0-based) listed in `keep`."""
     r = refbind.RefRenderer().open_arrays(sc)
     r.begin(w, h); r.set_camera(cam); r.set_max_bounces(mb); r.enable_white_furnace(wf)
     if tables is not None:
         r.use_sampler_tables(tables); r.set_blue_noise(True)
     out = []
-    for _ in range(n):
+    for sample in range(n):
         r.integrate()
+        if keep is not None and sample not in keep:
+            continue
         kw = {"keys": keys} if keys else {}
         out.append(frame_record(r.stats(), mb, r.radiance(), r.primary_hits() if with_hits else None, **kw))
     r.close()
@@ -78,6 +81,14 @@ def oracle_vs_ref_frames():
         F["degenerate/" + case] = ref_samples(scene(name), default_camera(w, h, **kw), w, h, mb, 2)
     for i, (name, w, h, mb, kw, wf) in enumerate(fuzz_configs()):
         F["fuzzed/%d" % i] = ref_samples(scene(name), default_camera(w, h, **kw), w, h, mb, 2, wf)
+    from tests.scenes_extra import closed_cornell
+    for w, h, mb, sampler in T.LONG_PATH_CASES:
+        F["long_path/closed_cornell_%dx%d_b%d_%s" % (w, h, mb, sampler)] = ref_samples(closed_cornell(), default_camera(w, h), w, h, mb, 2,
+                                                                                      tables=T.sampler_tables(sampler))
+    for name, w, h, mb, sampler in T.LATE_SAMPLE_CASES:
+        F["late_sample/%s_%dx%d_b%d_%s" % (name, w, h, mb, sampler)] = ref_samples(scene(name), default_camera(w, h), w, h, mb,
+                                                                                  T.LATE_SAMPLE_COUNT, tables=T.sampler_tables(sampler),
+                                                                                  keep=T.LATE_SAMPLE_KEEP)
     return F
 
 

@@ -55,6 +55,28 @@ def single_leaf_scene(n_tris=1):
     return sc
 
 
+def closed_cornell():
+    """CornellBox with its open side (the plane y = -1 of the default camera) closed by a quad of the back wall's material,
+    facing into the box.  Primary rays leave through its back face (culled, trace_bvh.cl:37); every later ray stays inside, so
+    paths only end when a sampled direction has pdf 0.  With no Russian roulette in the reference, their throughput decays
+    through the subnormal range over a few hundred bounces.  The default light is directional: its shadow rays are always
+    occluded, so the shadow-ray count of a bounce is the number of hits whose light sample is still non-zero."""
+    from raytracing_b200 import hostapi
+    sc = dict(scene("CornellBox"))
+    tris = sc["triangles"]
+    quad = tris[[4, 5]].copy()                                       # back wall (y = +1), material of the back wall
+    quad["v1"]["position"][:, :3] = [(1.0, -1.0, 0.0), (-1.0, -1.0, 2.0)]
+    quad["v2"]["position"][:, :3] = [(-1.0, -1.0, 0.0), (1.0, -1.0, 2.0)]
+    quad["v3"]["position"][:, :3] = [(-1.0, -1.0, 2.0), (1.0, -1.0, 0.0)]
+    for v in ("v1", "v2", "v3"):
+        quad[v]["normal"][:, :3] = (0.0, 1.0, 0.0)
+    ordered, nodes, _ = hostapi.build_bvh(np.concatenate([tris, quad]))
+    sc["triangles"], sc["nodes"] = ordered, nodes
+    emissive_mtl = tris["mtlIndex"][sc["emissive"]]                 # the ceiling light's triangles, now in leaf order
+    sc["emissive"] = np.flatnonzero(np.isin(ordered["mtlIndex"], emissive_mtl)).astype("<u4")
+    return sc
+
+
 def many_lights_scene(name="CornellBox"):
     """The fixture with five analytic lights — two directional, three point lights inside the box (light.h:30-65: uniform
     pick, 1/d^2 fall-off, shadow rays that stop at the light)."""

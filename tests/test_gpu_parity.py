@@ -22,6 +22,22 @@ pytestmark = pytest.mark.gpu
 
 INVALID = 0xFFFFFFFF
 
+# The ways rt_integrate can run a frame: the options set on a fresh context before reset().  The default
+# (RT_OPT_FRAME_KERNEL = 2) picks `frame` for every image these tests render below 0.95 M pixels, so each schedule is named
+# explicitly.  "stepwise" is not an rt_integrate schedule: Context.integrate_stepwise, one call per reference virtual.
+SCHEDULES = {
+    "frame": ((capi.OPT_FRAME_KERNEL, 1),),                            # k_frame, automatic CTA shape
+    "phase_graph": ((capi.OPT_FRAME_KERNEL, 0),),                      # the 1080p default: one CUDA graph, PDL, shadow pass
+                                                                       # merged into k_trace_both
+    "phase_direct": ((capi.OPT_FRAME_KERNEL, 0), (capi.OPT_GRAPH, 0)), # the same kernels launched one by one
+    "counted": ((capi.OPT_COUNT_TRAVERSAL, 1),),                       # k_trace_closest<true,0> / k_shadow_accumulate<true,0>,
+                                                                       # BVH not staged
+    "timed": ((capi.OPT_KERNEL_TIMING, 1),),                           # unmerged per-phase kernels between CUDA events, no graph,
+                                                                       # no PDL
+}
+BASIC = ("frame", "phase_graph", "stepwise")
+EVERY = ("frame", "phase_graph", "phase_direct", "counted", "timed", "stepwise")
+
 
 def make_ctx(name, w, h, **kw):
     ctx = capi.Context(w, h, **kw)
@@ -30,25 +46,75 @@ def make_ctx(name, w, h, **kw):
     return ctx
 
 
-def check_stats(st, ost, mb):
+def schedule_ctx(schedule, sc, cam, w, h, options=(), rank=0, world=1):
+    """A context that runs `schedule`, with the extra (key, value) options set after it; not reset yet."""
+    c = capi.Context(w, h, rank=rank, world=world)
+    c.upload_scene(sc); c.set_camera(cam)
+    for k, v in SCHEDULES.get(schedule, ()) + tuple(options):
+        c.set_option(k, v)
+    return c
+
+
+def run_frame(c, schedule, mb):
+    c.integrate_stepwise(mb) if schedule == "stepwise" else c.integrate(mb)
+
+
+def check_stats(st, ost, mb, where=()):
     for k in ("n_ext", "n_miss", "n_shadow", "n_cont", "n_unoccluded", "n_emissive_hits"):
-        assert np.array_equal(st[k][: mb + 1], ost[k][: mb + 1]), k
+        assert np.array_equal(st[k][: mb + 1], ost[k][: mb + 1]), (k,) + tuple(where)
+
+
+def check_frame(c, ost, oacc, mb, where):
+    """Per-bounce counters and the accumulated radiance's bits of context c equal the oracle's."""
+    check_stats(c.frame_stats(), ost, mb, where)
+    assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(oacc[..., :3])), tuple(where)
+
+
+def schedules_match_oracle(sc, cam, w, h, mb, schedules, samples=2, wf=False, tables=None, options=(), where=()):
+    """Renders every sample once with the oracle and compares each schedule's context with it after every sample.  Returns the
+    contexts ({schedule: context}, to be destroyed by the caller) and the oracle's last accumulated radiance."""
+    ctxs = {}
+    for s in schedules:
+        c = schedule_ctx(s, sc, cam, w, h, options)
+        c.set_option(capi.OPT_WHITE_FURNACE, int(wf))
+        if tables is not None:
+            c.upload_sampler_tables(*tables); c.set_option(capi.OPT_SAMPLER, 1)
+        c.reset()
+        ctxs[s] = c
+    o = Oracle(sc)
+    oacc = np.zeros((h, w, 4), dtype="<f4")
+    try:
+        o.set_sampler_tables(tables)
+        for sample in range(samples):
+            oacc, _, ost = o.render(cam, w, h, mb, sample_idx=sample, white_furnace=wf, radiance=oacc)
+            for s, c in ctxs.items():
+                run_frame(c, s, mb)
+                check_frame(c, ost, oacc, mb, tuple(where) + (s, "sample %d" % sample))
+    except BaseException:
+        destroy(ctxs)
+        raise
+    finally:
+        o.set_sampler_tables(None)
+    return ctxs, oacc
+
+
+def destroy(ctxs):
+    for c in ctxs.values():
+        c.destroy()
 
 
 @pytest.mark.parametrize("path", golden_files(), ids=lambda p: p.split("golden_")[-1].replace(".npz.xz", ""))
-@pytest.mark.parametrize("fused", [False, True], ids=["stepwise", "fused"])
-def test_matches_reference_golden(path, fused):
-    """CUDA vs outputs of the reference's own kernels (committed fixtures)."""
+@pytest.mark.parametrize("schedule", BASIC)
+def test_matches_reference_golden(path, schedule):
+    """CUDA vs outputs of the reference's own kernels (committed fixtures); the stepwise arm also checks the primary hits
+    and rays."""
     g = load_golden(path)
     w, h, mb = int(g["width"]), int(g["height"]), int(g["max_bounces"])
-    ctx = capi.Context(w, h)
-    ctx.upload_scene(scene(g["scene_name"]))
-    ctx.set_camera(g["camera"])
-    ctx.set_option(capi.OPT_WHITE_FURNACE, int(g["white_furnace"]))
+    ctx = schedule_ctx(schedule, scene(g["scene_name"]), g["camera"], w, h, ((capi.OPT_WHITE_FURNACE, int(g["white_furnace"])),))
     ctx.reset()
     for _ in range(int(g["sample_count"]) - 1):               # progressive fixtures: the earlier samples
-        ctx.integrate(mb) if fused else ctx.integrate_stepwise(mb)
-    if fused:
+        run_frame(ctx, schedule, mb)
+    if schedule != "stepwise":
         ctx.integrate(mb)
     else:
         ctx.generate_rays()
@@ -72,12 +138,12 @@ def test_matches_reference_golden(path, fused):
     rad = ctx.read_radiance()
     st = ctx.frame_stats()
     for k in ("n_ext", "n_miss", "n_shadow", "n_cont", "n_unoccluded"):
-        assert np.array_equal(st[k][: mb + 1], g[k]), k
-    assert np.array_equal(bits(rad[..., :3]), bits(g["radiance_rgb"]))
+        assert np.array_equal(st[k][: mb + 1], g[k]), (k, schedule)
+    assert np.array_equal(bits(rad[..., :3]), bits(g["radiance_rgb"])), schedule
     assert ctx.sample_count() == int(g["sample_count"])
     if "resolved" in g:
         res = ctx.resolve()
-        assert np.array_equal(bits(res), bits(g["resolved"]))
+        assert np.array_equal(bits(res), bits(g["resolved"])), schedule
     ctx.destroy()
 
 
@@ -89,57 +155,38 @@ def test_matches_reference_golden(path, fused):
 ])
 @pytest.mark.parametrize("traversal", [0, 1], ids=["literal", "fast"])
 def test_fused_and_stepwise_match_oracle(name, w, h, mb, traversal):
-    """CUDA (both schedules, both traversal kernels) vs the CPU oracle, live, two accumulated samples."""
-    sc = scene(name)
-    cam = default_camera(w, h)
-    o = Oracle(sc)
-    oacc = np.zeros((h, w, 4), dtype="<f4")
-    ctxs = {}
-    for mode in ("fused", "stepwise"):
-        c = make_ctx(name, w, h)
-        c.set_option(capi.OPT_TRAVERSAL, traversal)
-        c.reset()
-        ctxs[mode] = c
-    for sample in range(2):
-        oacc, ohits, ost = o.render(cam, w, h, mb, sample_idx=sample, radiance=oacc)
-        ctxs["fused"].integrate(mb)
-        ctxs["stepwise"].integrate_stepwise(mb)
-        for mode, c in ctxs.items():
-            check_stats(c.frame_stats(), ost, mb)
-            assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(oacc[..., :3])), (mode, sample)
-    for c in ctxs.values():
-        c.destroy()
+    """CUDA (the one-kernel frame, the per-phase graph and the stepwise calls; both traversal kernels) vs the CPU oracle, live,
+    two accumulated samples."""
+    ctxs, _ = schedules_match_oracle(scene(name), default_camera(w, h), w, h, mb, BASIC, options=((capi.OPT_TRAVERSAL, traversal),),
+                                     where=(name,))
+    destroy(ctxs)
 
 
 def test_traversal_work_counters_match_oracle():
-    """RT_OPT_COUNT_TRAVERSAL: nodes visited / triangles tested in reference order (the algorithmic-bytes inputs)."""
+    """RT_OPT_COUNT_TRAVERSAL: nodes visited / triangles tested in reference order (the algorithmic-bytes inputs), and the
+    frame those counting kernels render."""
     name, w, h, mb = "ShaderBalls", 320, 180, 4
     cam = default_camera(w, h)
-    _, _, ost = Oracle(scene(name)).render(cam, w, h, mb)
+    orad, _, ost = Oracle(scene(name)).render(cam, w, h, mb)
     c = make_ctx(name, w, h)
     c.set_option(capi.OPT_COUNT_TRAVERSAL, 1)
     c.reset(); c.integrate(mb)
     st = c.frame_stats()
     for k in ("nodes_ext", "tris_ext", "nodes_shadow", "tris_shadow"):
         assert np.array_equal(st[k][: mb + 1], ost[k][: mb + 1]), k
+    check_frame(c, ost, orad, mb, ("counted",))
     c.destroy()
 
 
 def test_white_furnace_and_empty_tail():
     """White furnace (energy aid, SURVEY 4) + more bounces than any path survives (empty queues must be harmless)."""
     name, w, h, mb = "CornellBox", 128, 96, 40
-    cam = default_camera(w, h)
-    orad, _, ost = Oracle(scene(name)).render(cam, w, h, mb, white_furnace=True)
-    c = make_ctx(name, w, h)
-    c.set_option(capi.OPT_WHITE_FURNACE, 1)
-    c.reset(); c.integrate(mb)
-    rad = c.read_radiance()
-    assert np.array_equal(bits(rad[..., :3]), bits(orad[..., :3]))
-    assert np.isfinite(rad).all()
-    # pixels whose paths never picked up the analytic light see only the 0.5-grey sky: never more than 0.5 (+rounding)
-    st = c.frame_stats()
-    assert st["n_ext"][mb] == 0 or st["n_ext"][mb] < st["n_ext"][0]
-    c.destroy()
+    ctxs, _ = schedules_match_oracle(scene(name), default_camera(w, h), w, h, mb, BASIC, samples=1, wf=True, where=(name,))
+    for c in ctxs.values():
+        assert np.isfinite(c.read_radiance()).all()
+        st = c.frame_stats()
+        assert st["n_ext"][mb] == 0 or st["n_ext"][mb] < st["n_ext"][0]
+    destroy(ctxs)
 
 
 @pytest.mark.parametrize("world", [2, 3])
@@ -307,7 +354,7 @@ def test_aovs_denoiser_and_views_match_oracle():
         c.set_option(capi.OPT_AOV, view)
         assert np.array_equal(bits(c.resolve()), bits(o.resolve(view, den, al, de, no, ve, 3, denoiser=True))), view
     c.destroy()
-    # fused schedule + AOV view without the denoiser
+    # rt_integrate (the one-kernel frame at this size) + AOV view without the denoiser
     c = make_ctx(name, w, h)
     c.set_option(capi.OPT_AOV, 3)
     c.reset(); c.integrate(mb)
@@ -331,18 +378,11 @@ def test_resolve_async_matches_blocking_resolve():
 
 
 def test_textured_materials_match_oracle():
-    """Texture sampling path of the shader (per-hit unpack instead of the precomputed material record)."""
+    """Texture sampling path of the shader (per-hit unpack instead of the precomputed material record), every schedule."""
     from tests.scenes_extra import textured_cornell
-    sc = textured_cornell()
     w, h, mb = 200, 150, 5
-    cam = default_camera(w, h)
-    orad, _, ost = Oracle(sc).render(cam, w, h, mb)
-    for stepwise in (False, True):
-        c = capi.Context(w, h); c.upload_scene(sc); c.set_camera(cam); c.reset()
-        c.integrate_stepwise(mb) if stepwise else c.integrate(mb)
-        check_stats(c.frame_stats(), ost, mb)
-        assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(orad[..., :3]))
-        c.destroy()
+    ctxs, _ = schedules_match_oracle(textured_cornell(), default_camera(w, h), w, h, mb, EVERY, samples=1, where=("textured",))
+    destroy(ctxs)
 
 
 @pytest.mark.parametrize("tables", ["synthetic", "reference"])
@@ -352,39 +392,20 @@ def test_textured_materials_match_oracle():
     ("CornellBox", 64, 64, 5, True),
 ])
 def test_blue_noise_sampler_matches_oracle(name, w, h, mb, wf, tables):
-    """SetSamplerType(kBlueNoise): all three schedules vs the oracle (itself pinned to hit_surface.cl -DBLUE_NOISE_SAMPLER
-    in tests/test_oracle_vs_ref.py), three progressive samples, then back to kRandom."""
+    """SetSamplerType(kBlueNoise): every schedule vs the oracle (itself pinned to hit_surface.cl -DBLUE_NOISE_SAMPLER in
+    tests/test_oracle_vs_ref.py), three progressive samples, then back to kRandom on the per-phase graph's context."""
     t = synthetic_sampler_tables() if tables == "synthetic" else reference_sampler_tables()
     if t is None:
         pytest.skip("oracle/_ref/libref.so (the carrier of the reference's tables) is not built here")
     sc = scene(name); cam = default_camera(w, h)
-    o = Oracle(sc)
-    ctxs = {}
-    for mode in ("fused", "stepwise"):
-        c = make_ctx(name, w, h)
-        c.set_option(capi.OPT_WHITE_FURNACE, int(wf))
-        c.upload_sampler_tables(*t)
-        c.set_option(capi.OPT_SAMPLER, 1)
-        c.reset()
-        ctxs[mode] = c
+    ctxs, _ = schedules_match_oracle(sc, cam, w, h, mb, EVERY, samples=3, wf=wf, tables=t, where=(name, tables))
     try:
-        o.set_sampler_tables(t)
-        oacc = np.zeros((h, w, 4), dtype="<f4")
-        for sample in range(3):
-            oacc, _, ost = o.render(cam, w, h, mb, sample_idx=sample, white_furnace=wf, radiance=oacc)
-            for mode, c in ctxs.items():
-                c.integrate_stepwise(mb) if mode == "stepwise" else c.integrate(mb)
-                check_stats(c.frame_stats(), ost, mb)
-                assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(oacc[..., :3])), (mode, sample)
-        o.set_sampler_tables(None)
-        plain, _, _ = o.render(cam, w, h, mb, sample_idx=0, white_furnace=wf)
-        c = ctxs["fused"]
-        c.set_option(capi.OPT_SAMPLER, 0); c.reset(); c.integrate(mb)      # switching back re-captures the frame graph
+        plain, _, _ = Oracle(sc).render(cam, w, h, mb, sample_idx=0, white_furnace=wf)
+        c = ctxs["phase_graph"]
+        c.set_option(capi.OPT_SAMPLER, 0); c.reset(); c.integrate(mb)      # the sampler is a launch argument: the graph is re-captured
         assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(plain[..., :3]))
     finally:
-        o.set_sampler_tables(None)
-        for c in ctxs.values():
-            c.destroy()
+        destroy(ctxs)
 
 
 @pytest.mark.parametrize("n_tris", [1, 2])
@@ -393,14 +414,10 @@ def test_root_leaf_bvh_and_tiny_images(n_tris):
     from tests.scenes_extra import single_leaf_scene
     sc = single_leaf_scene(n_tris)
     for (w, h) in [(1, 1), (33, 3)]:
-        cam = default_camera(w, h)
-        orad, _, ost = Oracle(sc).render(cam, w, h, 3)
         for traversal in (0, 1):
-            c = capi.Context(w, h); c.upload_scene(sc); c.set_camera(cam); c.set_option(capi.OPT_TRAVERSAL, traversal)
-            c.reset(); c.integrate(3)
-            check_stats(c.frame_stats(), ost, 3)
-            assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(orad[..., :3]))
-            c.destroy()
+            ctxs, orad = schedules_match_oracle(sc, default_camera(w, h), w, h, 3, BASIC, samples=1,
+                                                options=((capi.OPT_TRAVERSAL, traversal),), where=(w, h, traversal))
+            destroy(ctxs)
     w, h = 33, 3
     out = np.zeros((h, w, 4), "<f4")
     for rank in range(4):                       # rank 3 owns zero rows
@@ -446,65 +463,33 @@ def test_shadow_pass_overlap_modes_are_equivalent(name, w, h, mb):
 
 @pytest.mark.parametrize("name,w,h,mb", [("CornellBox", 300, 170, 6), ("ShaderBalls", 256, 144, 5)])
 def test_point_lights_and_thin_lens_match_oracle(name, w, h, mb):
-    """Five analytic lights (point + directional) and a thin-lens camera off the default pose: fused and stepwise vs the
-    oracle (pinned on the same configuration in tests/test_oracle_vs_ref.py)."""
+    """Five analytic lights (point + directional) and a thin-lens camera off the default pose vs the
+    oracle (pinned on the same configuration in tests/test_oracle_vs_ref.py), every schedule."""
     from tests.scenes_extra import many_lights_scene
-    sc = many_lights_scene(name)
     cam = default_camera(w, h, position=(0.15, -1.3, 0.9), aperture=0.04, focus_distance=1.7)
-    o = Oracle(sc)
-    oacc = np.zeros((h, w, 4), dtype="<f4")
-    ctxs = []
-    for stepwise in (False, True):
-        c = capi.Context(w, h); c.upload_scene(sc); c.set_camera(cam); c.reset()
-        ctxs.append((stepwise, c))
-    for sample in range(2):
-        oacc, ohits, ost = o.render(cam, w, h, mb, sample_idx=sample, radiance=oacc)
-        for stepwise, c in ctxs:
-            c.integrate_stepwise(mb) if stepwise else c.integrate(mb)
-            check_stats(c.frame_stats(), ost, mb)
-            assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(oacc[..., :3])), (stepwise, sample)
-    for _, c in ctxs:
-        c.destroy()
+    ctxs, _ = schedules_match_oracle(many_lights_scene(name), cam, w, h, mb, EVERY, where=(name,))
+    destroy(ctxs)
 
 
 @pytest.mark.parametrize("case", ["zero_bounces", "all_miss", "inside_geometry"])
 def test_degenerate_frames_match_oracle(case):
-    """max_bounces = 0; a frame whose every primary ray misses (all later queues empty: persistent kernels with nothing to
-    drain, merged traversal kernels with two empty queues); a camera inside closed geometry."""
+    """max_bounces = 0; a frame whose every primary ray misses (all later queues empty: CTAs of k_frame whose queues run dry
+    after bounce 0; per-phase persistent kernels with nothing to drain, k_trace_both with two empty queues); a camera inside
+    closed geometry.  Every schedule."""
     name, w, h, mb, kw = {"zero_bounces": ("CornellBox", 192, 128, 0, {}),
                           "all_miss": ("ShaderBalls", 160, 96, 4, {"position": (0.0, -30.0, 40.0), "pitch": 0.3}),
                           "inside_geometry": ("ShaderBalls", 160, 96, 4, {"position": (0.0, 0.0, 0.35), "pitch": 1.9})}[case]
-    sc = scene(name); cam = default_camera(w, h, **kw)
-    o = Oracle(sc)
-    oacc = np.zeros((h, w, 4), dtype="<f4")
-    ctxs = []
-    for stepwise in (False, True):
-        c = capi.Context(w, h); c.upload_scene(sc); c.set_camera(cam); c.reset()
-        ctxs.append((stepwise, c))
-    for sample in range(2):
-        oacc, _, ost = o.render(cam, w, h, mb, sample_idx=sample, radiance=oacc)
-        for stepwise, c in ctxs:
-            c.integrate_stepwise(mb) if stepwise else c.integrate(mb)
-            check_stats(c.frame_stats(), ost, mb)
-            assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(oacc[..., :3])), (case, stepwise, sample)
-    for _, c in ctxs:
-        c.destroy()
+    ctxs, _ = schedules_match_oracle(scene(name), default_camera(w, h, **kw), w, h, mb, EVERY, where=(case,))
+    destroy(ctxs)
 
 
 def test_fuzzed_frames_match_oracle():
     """The seeded random configurations of tests/test_oracle_vs_ref.py (scenes, sizes, bounce counts, camera poses and lenses,
-    axis-aligned views): fused schedule vs the oracle, two progressive samples each."""
+    axis-aligned views): the one-kernel frame, the per-phase graph and the stepwise calls vs the oracle, two progressive
+    samples each."""
     for name, w, h, mb, kw, wf in fuzz_configs():
-        sc = scene(name); cam = default_camera(w, h, **kw)
-        o = Oracle(sc)
-        c = capi.Context(w, h); c.upload_scene(sc); c.set_camera(cam); c.set_option(capi.OPT_WHITE_FURNACE, int(wf)); c.reset()
-        oacc = np.zeros((h, w, 4), dtype="<f4")
-        for sample in range(2):
-            oacc, _, ost = o.render(cam, w, h, mb, sample_idx=sample, white_furnace=wf, radiance=oacc)
-            c.integrate(mb)
-            check_stats(c.frame_stats(), ost, mb)
-            assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(oacc[..., :3])), (name, w, h, mb, kw, wf, sample)
-        c.destroy()
+        ctxs, _ = schedules_match_oracle(scene(name), default_camera(w, h, **kw), w, h, mb, BASIC, wf=wf, where=(name, w, h, mb, kw, wf))
+        destroy(ctxs)
 
 
 @pytest.mark.parametrize("name,w,h,mb", [("CornellBox", 333, 127, 8), ("ShaderBalls", 480, 270, 6), ("CornellBox_Dragon", 200, 112, 12), ("CornellBox", 37, 5, 3)])
@@ -640,23 +625,28 @@ def test_multi_device_context_matches_single_device(name, w, h, mb):
 
 
 def test_scene_reupload_and_camera_change_on_one_context():
-    """UploadGPUData twice and SetCameraData between frames on the same context (the frame graph is re-captured when a
-    launch argument changes, and only its per-frame constants are refreshed when the camera moves)."""
+    """UploadGPUData twice and SetCameraData between frames, each schedule on one context throughout.  On the per-phase graph's
+    context the frame graph is re-captured when a launch argument changes (a new scene) and only its per-frame constants are
+    refreshed when the camera moves; the one-kernel frame takes both as launch arguments."""
     w, h, mb = 200, 112, 5
-    c = capi.Context(w, h)
     cams = [default_camera(w, h), default_camera(w, h, position=(0.3, -1.4, 1.2))]
-    for name in ("CornellBox", "ShaderBalls", "CornellBox"):
-        sc = scene(name); o = Oracle(sc)
-        c.upload_scene(sc)
-        for cam in cams:
-            c.set_camera(cam); c.reset()
-            acc = np.zeros((h, w, 4), dtype="<f4")
-            for sample in range(2):
-                c.integrate(mb)
-                acc, _, ost = o.render(cam, w, h, mb, sample_idx=sample, radiance=acc)
-                check_stats(c.frame_stats(), ost, mb)
-                assert np.array_equal(bits(c.read_radiance()[..., :3]), bits(acc[..., :3])), (name, sample)
-    c.destroy()
+    ctxs = {s: schedule_ctx(s, scene("CornellBox"), cams[0], w, h) for s in BASIC}
+    try:
+        for name in ("CornellBox", "ShaderBalls", "CornellBox"):
+            sc = scene(name); o = Oracle(sc)
+            for c in ctxs.values():
+                c.upload_scene(sc)
+            for cam in cams:
+                for c in ctxs.values():
+                    c.set_camera(cam); c.reset()
+                acc = np.zeros((h, w, 4), dtype="<f4")
+                for sample in range(2):
+                    acc, _, ost = o.render(cam, w, h, mb, sample_idx=sample, radiance=acc)
+                    for s, c in ctxs.items():
+                        run_frame(c, s, mb)
+                        check_frame(c, ost, acc, mb, (name, s, "sample %d" % sample))
+    finally:
+        destroy(ctxs)
 
 
 def test_error_behaviour():

@@ -30,6 +30,12 @@ LIGHTS_CASES = [("CornellBox", 150, 90, 5), ("ShaderBalls", 128, 72, 4)]
 DEGENERATE_CASES = {"zero_bounces": ("CornellBox", 96, 64, 0, {}),
                     "all_miss": ("ShaderBalls", 80, 48, 4, {"position": (0.0, -30.0, 40.0), "pitch": 0.3}),
                     "inside_geometry": ("ShaderBalls", 80, 48, 4, {"position": (0.0, 0.0, 0.35), "pitch": 1.9})}
+# the closed box (tests/scenes_extra.closed_cornell): paths that never leave it, throughput decaying through the subnormal range.
+# 60 bounces passes the wrap of the blue-noise dimension (bounce * 5 + type) & 255 at bounce 51; 255 is RT_MAX_BOUNCES.
+LONG_PATH_CASES = [(48, 32, 60, "blue_noise"), (48, 32, 255, "random")]
+# late sample indices: 258 accumulated samples, records of the last four (the blue-noise sample index wraps at 256)
+LATE_SAMPLE_CASES = [("CornellBox", 24, 16, 2, "random"), ("CornellBox", 24, 16, 2, "blue_noise")]
+LATE_SAMPLE_COUNT, LATE_SAMPLE_KEEP = 258, (254, 255, 256, 257)
 LIBM_CASES = [("CornellBox", 160, 90, 8, 0.02), ("ShaderBalls", 160, 90, 8, 0.02), ("CornellBox_Dragon", 160, 90, 16, 0.04)]
 LIBM_SAMPLE = 1024          # pixels of each frame kept in tests/golden/ref/libm_sample.npz (seeded)
 
@@ -46,14 +52,25 @@ def lights_camera(w, h):
     return default_camera(w, h, position=(0.15, -1.3, 0.9), aperture=0.04, focus_distance=1.7)
 
 
-def oracle_samples(sc, cam, w, h, mb, n, wf=False, with_hits=True):
+def oracle_samples(sc, cam, w, h, mb, n, wf=False, with_hits=True, tables=None, keep=None):
+    """Records of n progressively accumulated samples (sample_idx 0, 1, ...), or of the samples listed in `keep`; kBlueNoise
+    with `tables`."""
     o = Oracle(sc)
     acc = np.zeros((h, w, 4), dtype="<f4")
     out = []
-    for sample in range(n):                     # progressive accumulation: sample_idx 0, 1, ...
-        acc, hits, st = o.render(cam, w, h, mb, sample_idx=sample, white_furnace=wf, radiance=acc)
-        out.append(frame_record(st, mb, acc, hits if with_hits else None))
+    try:
+        o.set_sampler_tables(tables)
+        for sample in range(n):
+            acc, hits, st = o.render(cam, w, h, mb, sample_idx=sample, white_furnace=wf, radiance=acc)
+            if keep is None or sample in keep:
+                out.append(frame_record(st, mb, acc, hits if with_hits else None))
+    finally:
+        o.set_sampler_tables(None)
     return out, st
+
+
+def sampler_tables(sampler):
+    return synthetic_sampler_tables() if sampler == "blue_noise" else None
 
 
 @pytest.mark.parametrize("name,w,h,mb,wf", BIT_EXACT_CASES)
@@ -147,6 +164,26 @@ def test_fuzzed_frames_bit_exact_vs_reference_kernels(cfg):
     name, w, h, mb, kw, wf = cfg
     recs, _ = oracle_samples(scene(name), default_camera(w, h, **kw), w, h, mb, 2, wf)
     assert_frames("fuzzed/%d" % fuzz_configs().index(cfg), recs)
+
+
+@pytest.mark.parametrize("w,h,mb,sampler", LONG_PATH_CASES)
+def test_long_paths_bit_exact_vs_reference_kernels(w, h, mb, sampler):
+    """Paths of up to 256 segments inside the closed box (no Russian roulette in the reference): the blue-noise dimension
+    wraps at bounce 51, the throughput underflows through the subnormals and the shadow-ray test dot(light_sample,
+    light_sample) > 0 (hit_surface.cl:127) then turns on whether subnormals are kept.  Two progressive samples."""
+    from tests.scenes_extra import closed_cornell
+    recs, st = oracle_samples(closed_cornell(), default_camera(w, h), w, h, mb, 2, tables=sampler_tables(sampler))
+    assert_frames("long_path/closed_cornell_%dx%d_b%d_%s" % (w, h, mb, sampler), recs)
+    assert st["n_ext"][mb] == w * h                 # nothing escapes the box
+    assert st["n_shadow"][mb] < st["n_shadow"][10] // 4
+
+
+@pytest.mark.parametrize("name,w,h,mb,sampler", LATE_SAMPLE_CASES)
+def test_late_sample_indices_bit_exact_vs_reference_kernels(name, w, h, mb, sampler):
+    """Sample indices 254..257 of one accumulation (the blue-noise sampler wraps the index with & 255, kRandom hashes it)."""
+    recs, _ = oracle_samples(scene(name), default_camera(w, h), w, h, mb, LATE_SAMPLE_COUNT, tables=sampler_tables(sampler),
+                             keep=LATE_SAMPLE_KEEP)
+    assert_frames("late_sample/%s_%dx%d_b%d_%s" % (name, w, h, mb, sampler), recs)
 
 
 @pytest.mark.parametrize("name,w,h,mb,limit", LIBM_CASES)
