@@ -146,7 +146,6 @@ struct DevScene
     uint32_t wnodes_f4, wtris_f4;  // sizes of the two arrays in float4 (for the TMA staging of small scenes)
     uint32_t top_n;                // interior records [0, top_n) are the top of the tree in breadth-first order
     uint32_t top_k;                // of those, the records a kernel staged into shared memory (set per launch; 0 = none)
-    uint32_t stack_off;            // RT_SMEM_STACK experiment: byte offset of the traversal stacks in dynamic shared memory
     int root_ref;
 };
 

@@ -1,5 +1,6 @@
 /*
- * rt_frame_kernel.cuh — the one-kernel frame (k_frame): every CTA an independent wavefront over its own pixels.
+ * rt_frame_kernel.cuh — the one-kernel frame (k_frame): every CTA an independent wavefront over its own pixels, its phases built from
+ * the warp work items that the per-phase kernels use (rt_kernels.cu).
  * Part of the single translation unit rt_kernels.cu (included there, inside its anonymous namespace).
  */
 #pragma once
@@ -36,13 +37,11 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
     __shared__ uint64_t s_mbar;
     __shared__ CtaFrame s;
     p.dyn = &dyn;                                  // per-frame constants (sample index, camera) arrive as a kernel parameter
-    if (SMEM == 1) tma_stage_bvh(s_bvh, sc, &s_mbar);
-    if (SMEM == 2) tma_stage_top(s_bvh, sc.wnodes, sc.top_k, &s_mbar);
+    stage_bvh<SMEM>(s_bvh, sc, &s_mbar);
     const int lane = threadIdx.x & 31;
     const uint32_t base = blockIdx.x * slots_per_cta;          // this CTA's region of every queue: slots [base, base + slots_per_cta)
     // (queue pointers are re-read from the kernel parameters where they are used: nothing but `base` stays live across the
     // traversal and shading loops)
-#define FQ(plane, i) (q.plane)[base + (i)]
     if (threadIdx.x == 0)
     {
         const uint32_t n_groups = (p.n_local + 31u) / 32u;
@@ -53,7 +52,6 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
         if (blockIdx.x == 0) ctr->n_primary = p.n_local;
     }
     __syncthreads();
-    const uint32_t sample_idx = p.dyn->sample_idx;
     uint32_t nv = 0, nt = 0;     // (not counted here: RT_OPT_COUNT_TRAVERSAL uses the per-phase kernels)
 
     for (uint32_t b = 0; b <= max_bounces + 1u; ++b)
@@ -69,81 +67,23 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
             {   // state of the NEXT phases that nobody reads during this one
                 s.cur_shade = 0; s.ext_n[(b + 1u) & 1] = 0; s.shadow_n[in] = 0; s.emit[in] = 0ull; s.ended_n[in] = 0;
             }
-            for (;;)
+            for (uint32_t at; (at = warp_grab(&s.cur_trace)) < total;)
             {
-                uint32_t at = 0;
-                if (lane == 0) at = atomicAdd(&s.cur_trace, 32u);
-                at = __shfl_sync(0xffffffffu, at, 0);
-                if (at >= total) break;
                 if (at < ext_span)
                 {
                     const uint32_t i = at + lane;
-                    bool live = i < n_ext, hit = false;
-                    float bu = 0.0f, bv = 0.0f, bt = 0.0f;
-                    uint32_t prim = RT_INVALID_ID;
+                    bool live = i < n_ext;
                     float4 a, bb;
                     if (b == 0)
-                    {   // RayGeneration (raygeneration.cl:65-139) fused into the first traversal pass; slot i <-> local pixel li
+                    {   // primary rays generated in the first traversal pass; slot i <-> local pixel li
                         const uint32_t li = (blockIdx.x + (i >> 5) * gridDim.x) * 32u + (uint32_t)lane;
                         live = li < p.n_local;
-                        if (live)
-                        {
-                            const uint32_t px = li % p.width, py = (li / p.width) * p.world + p.rank;
-                            f3 o, d;
-                            generate_primary_ray(p.dyn->raygen, py * p.width + px, px, py, sample_idx, o, d);
-                            a = make_float4(o.x, o.y, o.z, __uint_as_float(pack_pixel(px, py)));
-                            bb = make_float4(d.x, d.y, d.z, RT_MAX_RENDER_DIST);
-                            FQ(A[0], i) = a; FQ(B[0], i) = bb; FQ(C[0], i) = make_float4(1.0f, 1.0f, 1.0f, 0.0f);
-                            if (aov.enabled)
-                            {   // raygeneration.cl:129-133
-                                aov.albedo[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                                aov.depth[li] = RT_MAX_RENDER_DIST;
-                                aov.normal[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                                aov.velocity[li] = make_float2(0.0f, 0.0f);
-                            }
-                        }
+                        if (live) primary_ray(p, q, aov, base + i, li, a, bb);
                     }
-                    else if (live) { a = FQ(A[in], i); bb = FQ(B[in], i); }
-                    if (live)
-                    {
-                        if (SMEM == 1) prim = trace_fast<false, false, 1, true>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(bb), 0.0f, bb.w, bu, bv, bt, nv, nt);
-                        else if (SMEM == 2) prim = trace_fast<false, false, 2, true>(sc, s_bvh, sc.wtris, mk3(a), mk3(bb), 0.0f, bb.w, bu, bv, bt, nv, nt);
-                        else prim = trace<false, false>(sc, mode, mk3(a), mk3(bb), 0.0f, bb.w, bu, bv, bt, nv, nt);
-                        hit = prim != RT_INVALID_ID;
-                    }
-                    const unsigned hmask = __ballot_sync(0xffffffffu, hit);
-                    const unsigned mmask = __ballot_sync(0xffffffffu, live && !hit);
-                    unsigned long long slot = 0ull;
-                    if (lane == 0)
-                        slot = atomicAdd(&s.hm[in], (unsigned long long)__popc(hmask) | ((unsigned long long)__popc(mmask) << 32));
-                    slot = __shfl_sync(0xffffffffu, slot, 0);
-                    const unsigned lt_mask = (1u << lane) - 1u;
-                    if (hit) FQ(hitq, (uint32_t)slot + __popc(hmask & lt_mask)) = make_float4(bu, bv, __uint_as_float(prim), __uint_as_float(i));
-                    else if (live) FQ(missq, (uint32_t)(slot >> 32) + __popc(mmask & lt_mask)) = i;
+                    else if (live) { a = q.A[in][base + i]; bb = q.B[in][base + i]; }
+                    closest_group<false, SMEM, true>(sc, mode, s_bvh, q, base, i, live, a, bb, &s.hm[in], nv, nt);
                 }
-                else
-                {   // IntersectShadowRays + AccumulateDirectSamples of bounce b-1
-                    const uint32_t i = at - ext_span + lane;
-                    bool un = false;
-                    if (i < n_sh)
-                    {
-                        const float4 a = FQ(sA, i), bb = FQ(sB, i);
-                        float bu, bv, bt;
-                        if (SMEM == 1) un = trace_fast<true, false, 1, true>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(bb), 0.0f, bb.w, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-                        else if (SMEM == 2) un = trace_fast<true, false, 2, true>(sc, s_bvh, sc.wtris, mk3(a), mk3(bb), 0.0f, bb.w, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-                        else un = trace<true, false>(sc, mode, mk3(a), mk3(bb), 0.0f, bb.w, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-                        if (un)
-                        {
-                            const float4 c = FQ(sC, i);
-                            const uint32_t li = local_index(p, __float_as_uint(a.w));
-                            float4 r = radiance[li];
-                            r.x += c.x; r.y += c.y; r.z += c.z;
-                            radiance[li] = r;
-                        }
-                    }
-                    const unsigned umask = __ballot_sync(0xffffffffu, un);
-                    if (lane == 0 && umask) atomicAdd(&s.n_unoccluded, (uint32_t)__popc(umask));
-                }
+                else shadow_group<false, SMEM, true>(p, sc, mode, s_bvh, q, base, at - ext_span + lane, n_sh, radiance, &s.n_unoccluded, nv, nt);
             }
             __syncthreads();
             if (p.gather && b > 0)
@@ -158,7 +98,7 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                     const uint32_t n_alive = s.ext_n[in];
                     for (uint32_t k = threadIdx.x; k < n_alive; k += blockDim.x)
                     {
-                        const uint32_t li = local_index(p, __float_as_uint(FQ(A[in], k).w));
+                        const uint32_t li = local_index(p, __float_as_uint(q.A[in][base + k].w));
                         p.gather[li] = radiance[li];
                     }
                 }
@@ -180,88 +120,30 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
             const uint32_t hit_span = (n_hit + 31u) & ~31u;            // warps never mix hits and misses
             const uint32_t total = hit_span + n_miss;
             if (threadIdx.x == 0) { s.cur_trace = 0; s.hm[out] = 0ull; }
-            for (;;)
+            for (uint32_t at; (at = warp_grab(&s.cur_shade)) < total;)
             {
-                uint32_t at = 0;
-                if (lane == 0) at = atomicAdd(&s.cur_shade, 32u);
-                at = __shfl_sync(0xffffffffu, at, 0);
-                if (at >= total) break;
                 if (at < hit_span)
                 {
                     const uint32_t k = at + lane;
                     const bool hit = k < n_hit;
-                    uint32_t pixel = 0;
-                    ShadeOut so;
-                    so.emissive = so.spawn_next = so.spawn_shadow = false;
-                    if (hit)
-                    {
-                        const float4 h = FQ(hitq, k);
-                        const uint32_t i = __float_as_uint(h.w);
-                        const float4 a = FQ(A[in], i), bb = FQ(B[in], i), c = FQ(C[in], i);
-                        pixel = __float_as_uint(a.w);
-                        shade_hit(sc, p, aov, b, pixel, mk3(a), mk3(bb), mk3(c), __float_as_uint(h.z), h.x, h.y, so);
-                        if (so.emissive)
-                        {
-                            const uint32_t li = local_index(p, pixel);
-                            float4 r = radiance[li];
-                            r.x += so.emission_add.x; r.y += so.emission_add.y; r.z += so.emission_add.z;
-                            radiance[li] = r;
-                        }
-                    }
-                    const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
-                    const unsigned smask = __ballot_sync(0xffffffffu, ss), nmask = __ballot_sync(0xffffffffu, sn);
-                    const unsigned emask = __ballot_sync(0xffffffffu, hit && so.emissive);
-                    unsigned long long slot = 0ull;
-                    if ((smask | nmask | emask) != 0u)
-                    {
-                        if (lane == 0)
-                        {
-                            slot = atomicAdd(&s.emit[in], (unsigned long long)__popc(smask) | ((unsigned long long)__popc(nmask) << 32));
-                            if (emask) atomicAdd(&s.n_emissive, (uint32_t)__popc(emask));
-                        }
-                        slot = __shfl_sync(0xffffffffu, slot, 0);
-                    }
-                    const unsigned lt_mask = (1u << lane) - 1u;
+                    float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                    if (hit) h = q.hitq[base + k];
+                    uint32_t pixel;
+                    const bool ends = shade_hit_group(p, sc, aov, q, base, b, hit, h, __float_as_uint(h.w), radiance, &s.emit[in], &s.n_emissive, pixel);
                     if (p.gather)
                     {   // paths that end at this hit (no continuation ray): final once their shadow ray is accumulated in T(b+1)
-                        const unsigned dmask = __ballot_sync(0xffffffffu, hit && !so.spawn_next);
+                        const unsigned dmask = __ballot_sync(0xffffffffu, ends);
                         if (dmask)
                         {
                             uint32_t at0 = 0;
                             if (lane == 0) at0 = atomicAdd(&s.ended_n[in], (uint32_t)__popc(dmask));
                             at0 = __shfl_sync(0xffffffffu, at0, 0);
-                            if (hit && !so.spawn_next)
-                            {
-                                uint32_t* list = in ? (uint32_t*)q.hits + base : q.shadow_flags + base;
-                                list[at0 + __popc(dmask & lt_mask)] = local_index(p, pixel);
-                            }
+                            uint32_t* list = in ? (uint32_t*)q.hits + base : q.shadow_flags + base;
+                            if (ends) list[at0 + __popc(dmask & ((1u << lane) - 1u))] = local_index(p, pixel);
                         }
                     }
-                    if (ss)
-                    {
-                        const uint32_t si = (uint32_t)slot + __popc(smask & lt_mask);
-                        FQ(sA, si) = make_float4(so.s_origin.x, so.s_origin.y, so.s_origin.z, __uint_as_float(pixel));
-                        FQ(sB, si) = make_float4(so.s_dir.x, so.s_dir.y, so.s_dir.z, so.s_tmax);
-                        FQ(sC, si) = make_float4(so.s_sample.x, so.s_sample.y, so.s_sample.z, 0.0f);
-                    }
-                    if (sn)
-                    {
-                        const uint32_t ni = (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
-                        FQ(A[out], ni) = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
-                        FQ(B[out], ni) = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
-                        FQ(C[out], ni) = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, 0.0f);
-                    }
                 }
-                else
-                {
-                    const uint32_t k = at - hit_span + lane;
-                    if (k < n_miss)
-                    {
-                        const uint32_t i = FQ(missq, k);
-                        const float4 a = FQ(A[in], i), bb = FQ(B[in], i), c = FQ(C[in], i);
-                        shade_miss(sc, p, radiance, __float_as_uint(a.w), mk3(bb), mk3(c));
-                    }
-                }
+                else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, in, base + q.missq[base + at - hit_span + lane], radiance);
             }
             __syncthreads();
             if (threadIdx.x == 0)
@@ -276,4 +158,3 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
         }
     }
 }
-#undef FQ

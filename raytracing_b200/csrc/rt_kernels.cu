@@ -1,8 +1,9 @@
 /*
  * rt_kernels.cu — the sm_90a kernels of the wavefront path tracer and the C ABI
  * (include/rt_b200.h) that launches them.  One translation unit so that the shading
- * code inlines into both the stepwise kernels (one per reference kernel) and the fused
- * ones.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (see
+ * code and the warp work items (closest hit, shadow rays, shading of 32 queue entries)
+ * inline into the stepwise kernels (one per reference kernel), the per-phase kernels
+ * and the one-kernel frame (rt_frame_kernel.cuh) alike.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (see
  * __graft_entry__.build()).  There is no CPU fallback anywhere in this file.
  *
  * Data layout in HBM (all SoA streams of float4, indexed by compacted ray slot):
@@ -27,10 +28,12 @@
  */
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "rt_b200.h"
@@ -67,15 +70,13 @@ struct ShadeOut
     f3 n_origin, n_dir, n_throughput;
 };
 
-// kernels/cl/miss.cl:41-77: radiance += sky * throughput
-__device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams& p, float4* radiance, uint32_t pxy, f3 dir, f3 throughput)
+// kernels/cl/miss.cl:41-77: radiance += sky * throughput, for the ray in slot `slot` of ray queue `in`
+__device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams& p, const Queues& q, int in, uint32_t slot, float4* radiance)
 {
-    f3 sky = p.white_furnace ? splat(0.5f) : sample_sky(sc, dir);
-    f3 add = sky * throughput;
-    uint32_t li = local_index(p, pxy);
-    float4 r = radiance[li];
-    r.x += add.x; r.y += add.y; r.z += add.z;
-    radiance[li] = r;
+    const float4 a = q.A[in][slot], b = q.B[in][slot], c = q.C[in][slot];
+    f3 sky = p.white_furnace ? splat(0.5f) : sample_sky(sc, mk3(b));
+    uint32_t li = local_index(p, __float_as_uint(a.w));
+    float4 r = add_radiance(radiance, li, sky * mk3(c));
     if (p.gather) p.gather[li] = r;        // the path ends here: its pixel is final (its last shadow ray was accumulated a phase ago)
 }
 
@@ -163,26 +164,21 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
     }
 }
 
-// ------------------------------------------------------------------------------------ kernels
-__global__ void __launch_bounds__(256) k_reset(float4* radiance, uint32_t n)
-{
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) radiance[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-}
+// ------------------------------------------------------------------------------------ warp work items
+// The bodies shared by the per-phase kernels and the one-kernel frame (rt_frame_kernel.cuh); the closest-hit, shadow and shading
+// items each handle one group of 32 queue entries.  Entry i of a queue lives in slot base + i: base is 0 for the per-phase
+// kernels and the CTA's region of every queue for k_frame.  The slot and statistics counters are global memory (DevCounters)
+// for the per-phase kernels and shared memory (CtaFrame) for k_frame.
 
-// raygeneration.cl:65-139.  One thread per LOCAL pixel; slot i of queue 0 = local pixel i.
-__global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCounters* ctr, AovParams aov)
+// RayGeneration (raygeneration.cl:65-139): the primary ray (a, b) of local pixel li, stored in slot `slot` of ray queue 0
+__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, uint32_t slot, uint32_t li, float4& a, float4& b)
 {
-    uint32_t li = blockIdx.x * blockDim.x + threadIdx.x;
-    if (li == 0) ctr->n_primary = p.n_local;
-    if (li >= p.n_local) return;
-    uint32_t px = li % p.width, py = (li / p.width) * p.world + p.rank;
-    uint32_t pixel = py * p.width + px;
+    const uint32_t px = li % p.width, py = (li / p.width) * p.world + p.rank;
     f3 o, d;
-    generate_primary_ray(p.dyn->raygen, pixel, px, py, p.dyn->sample_idx, o, d);
-    q.A[0][li] = make_float4(o.x, o.y, o.z, __uint_as_float(pack_pixel(px, py)));
-    q.B[0][li] = make_float4(d.x, d.y, d.z, RT_MAX_RENDER_DIST);
-    q.C[0][li] = make_float4(1.0f, 1.0f, 1.0f, 0.0f);
+    generate_primary_ray(p.dyn->raygen, py * p.width + px, px, py, p.dyn->sample_idx, o, d);
+    a = make_float4(o.x, o.y, o.z, __uint_as_float(pack_pixel(px, py)));
+    b = make_float4(d.x, d.y, d.z, RT_MAX_RENDER_DIST);
+    q.A[0][slot] = a; q.B[0][slot] = b; q.C[0][slot] = make_float4(1.0f, 1.0f, 1.0f, 0.0f);
     if (aov.enabled)
     {   // raygeneration.cl:129-133
         aov.albedo[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -190,6 +186,115 @@ __global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCoun
         aov.normal[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         aov.velocity[li] = make_float2(0.0f, 0.0f);
     }
+}
+
+// Closest hit of the ray (a, b) of entry i (live lanes) and hit/miss stream compaction: __ballot + __popc give every lane its
+// slot, ONE 64-bit atomic per warp on `hm` reserves the slots of both queues (hits in the low word, misses in the high).
+template <bool COUNT, int SMEM, bool PIN>
+__device__ __forceinline__ void closest_group(const DevScene& sc, int mode, const float4* s_bvh, const Queues& q, uint32_t base, uint32_t i, bool live,
+                                              float4 a, float4 b, unsigned long long* hm, uint32_t& nv, uint32_t& nt)
+{
+    const int lane = threadIdx.x & 31;
+    bool hit = false;
+    float bu = 0.0f, bv = 0.0f, bt = 0.0f;
+    uint32_t prim = RT_INVALID_ID;
+    if (live)
+    {
+        prim = trace_staged<false, COUNT, SMEM, PIN>(sc, mode, s_bvh, a, b, bu, bv, bt, nv, nt);
+        hit = prim != RT_INVALID_ID;
+    }
+    const unsigned hmask = __ballot_sync(0xffffffffu, hit);
+    const unsigned mmask = __ballot_sync(0xffffffffu, live && !hit);
+    unsigned long long slot = 0ull;
+    if (lane == 0) slot = atomicAdd(hm, (unsigned long long)__popc(hmask) | ((unsigned long long)__popc(mmask) << 32));
+    slot = __shfl_sync(0xffffffffu, slot, 0);
+    const unsigned lt_mask = (1u << lane) - 1u;
+    if (hit) q.hitq[base + (uint32_t)slot + __popc(hmask & lt_mask)] = make_float4(bu, bv, __uint_as_float(prim), __uint_as_float(i));
+    else if (live) q.missq[base + (uint32_t)(slot >> 32) + __popc(mmask & lt_mask)] = i;
+}
+
+// IntersectShadowRays + AccumulateDirectSamples (accumulate_direct_samples.cl:27-53) of shadow-queue entry i < n: any-hit trace,
+// the light sample of an unoccluded ray added to its pixel, the unoccluded rays counted on `n_unoccluded`
+template <bool COUNT, int SMEM, bool PIN>
+__device__ __forceinline__ void shadow_group(const FrameParams& p, const DevScene& sc, int mode, const float4* s_bvh, const Queues& q, uint32_t base,
+                                             uint32_t i, uint32_t n, float4* radiance, uint32_t* n_unoccluded, uint32_t& nv, uint32_t& nt)
+{
+    bool un = false;
+    if (i < n)
+    {
+        const float4 a = q.sA[base + i], b = q.sB[base + i];
+        float bu, bv, bt;
+        un = trace_staged<true, COUNT, SMEM, PIN>(sc, mode, s_bvh, a, b, bu, bv, bt, nv, nt) == RT_INVALID_ID;
+        if (un) add_radiance(radiance, local_index(p, __float_as_uint(a.w)), mk3(q.sC[base + i]));
+    }
+    warp_count(n_unoccluded, un);
+}
+
+// ShadeSurfaceHits (hit_surface.cl) of the hit h = (bc.x, bc.y, primitive_id bits, -) of the ray in entry i (hit lanes): shading,
+// emission into the radiance, and compaction of the two output streams — ONE 64-bit atomic per warp on `emit` reserves the slots
+// of both queues (shadow rays in the low word, continuation rays in the high).  Returns whether the lane's path ends at this hit
+// (no continuation ray); `pixel` is the packed pixel of the ray.
+__device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevScene& sc, const AovParams& aov, const Queues& q, uint32_t base, uint32_t bounce,
+                                                bool hit, float4 h, uint32_t i, float4* radiance, unsigned long long* emit, uint32_t* n_emissive, uint32_t& pixel)
+{
+    const int in = bounce & 1, out = (bounce + 1) & 1;
+    ShadeOut so;
+    so.emissive = so.spawn_next = so.spawn_shadow = false;
+    pixel = 0;
+    if (hit)
+    {
+        const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
+        pixel = __float_as_uint(a.w);
+        shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), __float_as_uint(h.z), h.x, h.y, so);
+        if (so.emissive) add_radiance(radiance, local_index(p, pixel), so.emission_add);
+    }
+    const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
+    const unsigned smask = __ballot_sync(0xffffffffu, ss), nmask = __ballot_sync(0xffffffffu, sn);
+    const unsigned emask = __ballot_sync(0xffffffffu, hit && so.emissive);
+    const int lane = threadIdx.x & 31;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    unsigned long long slot = 0ull;
+    if ((smask | nmask | emask) != 0u)
+    {
+        if (lane == 0)
+        {
+            slot = atomicAdd(emit, (unsigned long long)__popc(smask) | ((unsigned long long)__popc(nmask) << 32));
+            if (emask) atomicAdd(n_emissive, (uint32_t)__popc(emask));
+        }
+        slot = __shfl_sync(0xffffffffu, slot, 0);
+    }
+    if (ss)
+    {
+        const uint32_t si = base + (uint32_t)slot + __popc(smask & lt_mask);
+        q.sA[si] = make_float4(so.s_origin.x, so.s_origin.y, so.s_origin.z, __uint_as_float(pixel));
+        q.sB[si] = make_float4(so.s_dir.x, so.s_dir.y, so.s_dir.z, so.s_tmax);
+        q.sC[si] = make_float4(so.s_sample.x, so.s_sample.y, so.s_sample.z, 0.0f);
+    }
+    if (sn)
+    {
+        const uint32_t ni = base + (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
+        q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
+        q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
+        q.C[out][ni] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, 0.0f);
+    }
+    return hit && !so.spawn_next;
+}
+
+// ------------------------------------------------------------------------------------ kernels
+__global__ void __launch_bounds__(256) k_reset(float4* radiance, uint32_t n)
+{
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) radiance[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
+// One thread per LOCAL pixel; slot i of queue 0 = local pixel i.
+__global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCounters* ctr, AovParams aov)
+{
+    uint32_t li = blockIdx.x * blockDim.x + threadIdx.x;
+    if (li == 0) ctr->n_primary = p.n_local;
+    if (li >= p.n_local) return;
+    float4 a, b;
+    primary_ray(p, q, aov, li, li, a, b);
 }
 
 // IntersectRays (stepwise): closest hit of every live ray of bounce b -> hits[]
@@ -215,60 +320,13 @@ __global__ void __launch_bounds__(256) k_shade_miss(FrameParams p, DevScene sc, 
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t n = *in_count_ptr(ctr, bounce);
-    int in = bounce & 1;
     bool miss = false;
     if (i < n)
     {
-        float4 h = q.hits[i];
-        miss = __float_as_uint(h.z) == RT_INVALID_ID;
-        if (miss)
-        {
-            float4 a = q.A[in][i], b = q.B[in][i], c = q.C[in][i];
-            shade_miss(sc, p, radiance, __float_as_uint(a.w), mk3(b), mk3(c));
-        }
+        miss = __float_as_uint(q.hits[i].z) == RT_INVALID_ID;
+        if (miss) shade_miss(sc, p, q, bounce & 1, i, radiance);
     }
     warp_count(&ctr->hm[bounce].miss, miss);
-}
-
-__device__ __forceinline__ void emit_rays(const FrameParams& p, Queues& q, DevCounters* ctr, float4* radiance, uint32_t bounce,
-                                          uint32_t pixel, bool hit, const ShadeOut& so)
-{
-    int out = (bounce + 1) & 1;
-    if (hit && so.emissive)
-    {
-        uint32_t li = local_index(p, pixel);
-        float4 r = radiance[li];
-        r.x += so.emission_add.x; r.y += so.emission_add.y; r.z += so.emission_add.z;
-        radiance[li] = r;
-    }
-    warp_count(&ctr->n_emissive[bounce], hit && so.emissive);
-    // hit/miss stream compaction of the two output streams: __ballot + __popc give every lane its slot, ONE 64-bit
-    // atomic per warp reserves the slots of both queues (shadow count in the low word, continuation count in the high)
-    const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
-    const unsigned smask = __ballot_sync(0xffffffffu, ss), nmask = __ballot_sync(0xffffffffu, sn);
-    const int lane = threadIdx.x & 31;
-    const unsigned lt_mask = (1u << lane) - 1u;
-    unsigned long long slot = 0ull;
-    if ((smask | nmask) != 0u)
-    {
-        if (lane == 0)
-            slot = atomicAdd((unsigned long long*)&ctr->emit[bounce], (unsigned long long)__popc(smask) | ((unsigned long long)__popc(nmask) << 32));
-        slot = __shfl_sync(0xffffffffu, slot, 0);
-    }
-    if (ss)
-    {
-        uint32_t si = (uint32_t)slot + __popc(smask & lt_mask);
-        q.sA[si] = make_float4(so.s_origin.x, so.s_origin.y, so.s_origin.z, __uint_as_float(pixel));
-        q.sB[si] = make_float4(so.s_dir.x, so.s_dir.y, so.s_dir.z, so.s_tmax);
-        q.sC[si] = make_float4(so.s_sample.x, so.s_sample.y, so.s_sample.z, 0.0f);
-    }
-    if (sn)
-    {
-        uint32_t ni = (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
-        q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
-        q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
-        q.C[out][ni] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, 0.0f);
-    }
 }
 
 // ShadeSurfaceHits (stepwise)
@@ -276,24 +334,15 @@ __global__ void __launch_bounds__(256) k_shade_hits(FrameParams p, DevScene sc, 
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t n = *in_count_ptr(ctr, bounce);
-    int in = bounce & 1;
     bool hit = false;
-    uint32_t pixel = 0;
-    ShadeOut so;
-    so.emissive = so.spawn_next = so.spawn_shadow = false;
+    float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     if (i < n)
     {
-        float4 h = q.hits[i];
-        uint32_t prim = __float_as_uint(h.z);
-        hit = prim != RT_INVALID_ID;
-        if (hit)
-        {
-            float4 a = q.A[in][i], b = q.B[in][i], c = q.C[in][i];
-            pixel = __float_as_uint(a.w);
-            shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), prim, h.x, h.y, so);
-        }
+        h = q.hits[i];
+        hit = __float_as_uint(h.z) != RT_INVALID_ID;
     }
-    emit_rays(p, q, ctr, radiance, bounce, pixel, hit, so);
+    uint32_t pixel;
+    shade_hit_group(p, sc, aov, q, 0, bounce, hit, h, i, radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
 }
 
 // IntersectShadowRays (stepwise): any-hit -> flags (0 = occluded, INVALID_ID = unoccluded)
@@ -321,57 +370,44 @@ __global__ void __launch_bounds__(256) k_accumulate(FrameParams p, Queues q, Dev
     if (i < n)
     {
         un = q.shadow_flags[i] == RT_INVALID_ID;
-        if (un)
-        {
-            float4 a = q.sA[i], c = q.sC[i];
-            uint32_t pixel = __float_as_uint(a.w);
-            uint32_t li = local_index(p, pixel);
-            float4 r = radiance[li];
-            r.x += c.x; r.y += c.y; r.z += c.z;
-            radiance[li] = r;
-        }
+        if (un) add_radiance(radiance, local_index(p, __float_as_uint(q.sA[i].w)), mk3(q.sC[i]));
     }
     warp_count(&ctr->n_unoccluded[bounce], un);
 }
 
-// Fused IntersectShadowRays + AccumulateDirectSamples: persistent warps drain the bounce's shadow-ray queue through a
-// global atomic cursor (work_shadow[bounce]), 32 consecutive rays per grab.
+// ---- queue-split schedule (default): hit/miss stream compaction between traversal and shading --------------
+// Traversal and shading are separate persistent kernels: the traversal kernel stays small in registers
+// (more resident warps to hide the dependent node fetches), and it compacts its results into a HIT queue and a
+// MISS queue with one warp-aggregated atomic each (__ballot + __popc), so that the shading kernel runs full
+// warps of hits (Lambert/GGX + NEE) and full warps of misses (environment lookup) instead of warps that
+// mix the two and idle through each other's code.  Every kernel drains its queues through a global atomic
+// cursor (warp_grab).
+template <bool COUNT, int SMEM>
+__device__ __forceinline__ void closest_phase(const DevScene& sc, int mode, const Queues& q, DevCounters* ctr, uint32_t bounce, const float4* s_bvh)
+{
+    const uint32_t n = *in_count_ptr(ctr, bounce);
+    const int in = bounce & 1;
+    uint32_t nv = 0, nt = 0;
+    for (uint32_t at; (at = warp_grab(&ctr->work_ext[bounce])) < n;)
+    {
+        const uint32_t i = at + (threadIdx.x & 31);
+        const bool live = i < n;
+        float4 a, b;
+        if (live) { a = q.A[in][i]; b = q.B[in][i]; }
+        closest_group<COUNT, SMEM, false>(sc, mode, s_bvh, q, 0, i, live, a, b, (unsigned long long*)&ctr->hm[bounce], nv, nt);
+    }
+    if (COUNT) { warp_sum64(&ctr->nodes_ext[bounce], nv); warp_sum64(&ctr->tris_ext[bounce], nt); }
+}
+
+// Fused IntersectShadowRays + AccumulateDirectSamples over the bounce's shadow-ray queue
 template <bool COUNT, int SMEM>
 __device__ __forceinline__ void shadow_phase(const FrameParams& p, const DevScene& sc, int mode, const Queues& q, DevCounters* ctr, float4* radiance,
                                              uint32_t bounce, const float4* s_bvh)
 {
     const uint32_t n = ctr->emit[bounce].shadow;
-    const int lane = threadIdx.x & 31;
     uint32_t nv = 0, nt = 0;
-    for (;;)
-    {
-        uint32_t base = 0;
-        if (lane == 0) base = atomicAdd(&ctr->work_shadow[bounce], 32u);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= n) break;
-      {
-        uint32_t i = base + lane;
-        bool un = false;
-        if (i < n)
-        {
-            float4 a = q.sA[i], b = q.sB[i];
-            float bu, bv, bt;
-            if (SMEM == 1) un = trace_fast<true, false, 1>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-            else if (SMEM == 2) un = trace_fast<true, false, 2>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-            else un = trace<true, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-            if (un)
-            {
-                float4 c = q.sC[i];
-                uint32_t pixel = __float_as_uint(a.w);
-                uint32_t li = local_index(p, pixel);
-                float4 r = radiance[li];
-                r.x += c.x; r.y += c.y; r.z += c.z;
-                radiance[li] = r;
-            }
-        }
-        warp_count(&ctr->n_unoccluded[bounce], un);
-      }
-    }
+    for (uint32_t at; (at = warp_grab(&ctr->work_shadow[bounce])) < n;)
+        shadow_group<COUNT, SMEM, false>(p, sc, mode, s_bvh, q, 0, at + (threadIdx.x & 31), n, radiance, &ctr->n_unoccluded[bounce], nv, nt);
     if (COUNT) { warp_sum64(&ctr->nodes_shadow[bounce], nv); warp_sum64(&ctr->tris_shadow[bounce], nt); }
 }
 
@@ -380,70 +416,9 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_shadow_accumulate(FrameP
 {
     extern __shared__ __align__(128) float4 s_bvh[];
     __shared__ uint64_t s_mbar;
-    if (SMEM == 1) tma_stage_bvh(s_bvh, sc, &s_mbar);
-    if (SMEM == 2) tma_stage_top(s_bvh, sc.wnodes, sc.top_k, &s_mbar);
+    stage_bvh<SMEM>(s_bvh, sc, &s_mbar);
     pdl_wait(); pdl_launch_dependents();
     shadow_phase<COUNT, SMEM>(p, sc, mode, q, ctr, radiance, bounce, s_bvh);
-}
-
-// ---- queue-split schedule (default): hit/miss stream compaction between traversal and shading --------------
-// Traversal and shading are separate persistent kernels: the traversal kernel stays small in registers
-// (more resident warps to hide the dependent node fetches), and it compacts its results into a HIT queue and a
-// MISS queue with one warp-aggregated atomic each (__ballot + __popc), so that the shading kernel runs full
-// warps of hits (Lambert/GGX + NEE) and full warps of misses (environment lookup) instead of warps that
-// mix the two and idle through each other's code.  Both kernels drain their queues through a global atomic
-// cursor, 32 entries per grab.
-template <bool COUNT, int SMEM>
-__device__ __forceinline__ void closest_phase(const FrameParams& p, const DevScene& sc, int mode, const Queues& q, DevCounters* ctr, uint32_t bounce,
-                                              const float4* s_bvh)
-{
-    const uint32_t n = *in_count_ptr(ctr, bounce);
-    const int in = bounce & 1;
-    const int lane = threadIdx.x & 31;
-    const unsigned lt_mask = (1u << lane) - 1u;
-    uint32_t nv = 0, nt = 0;
-    // 32 rays per cursor grab.  Measured alternatives that were slower: 64 rays per grab (-4 %), and issuing the next
-    // round's grab before the current round's work to hide the atomic's latency (-5 %): both make a warp own more
-    // work at a time, and the coarser tail costs more than the hidden latency saves.
-    for (;;)
-    {
-        uint32_t base = 0;
-        if (lane == 0) base = atomicAdd(&ctr->work_ext[bounce], 32u);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= n) break;
-        {
-            uint32_t i = base + lane;
-            bool live = i < n, hit = false;
-            float bu = 0.0f, bv = 0.0f, bt = 0.0f;
-            uint32_t prim = RT_INVALID_ID;
-            if (live)
-            {
-                float4 a = q.A[in][i], b = q.B[in][i];
-                if (SMEM == 1) prim = trace_fast<false, false, 1>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-                else if (SMEM == 2) prim = trace_fast<false, false, 2>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-                else prim = trace<false, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-                hit = prim != RT_INVALID_ID;
-            }
-            const unsigned hmask = __ballot_sync(0xffffffffu, hit);
-            const unsigned mmask = __ballot_sync(0xffffffffu, live && !hit);
-            unsigned long long slot = 0ull;
-            if (lane == 0)
-                slot = atomicAdd((unsigned long long*)&ctr->hm[bounce], (unsigned long long)__popc(hmask) | ((unsigned long long)__popc(mmask) << 32));
-            slot = __shfl_sync(0xffffffffu, slot, 0);
-#ifdef RT_HITQ_CARRY
-            if (hit)
-            {
-                const uint32_t k = (uint32_t)slot + __popc(hmask & lt_mask);
-                q.hitq[k] = make_float4(bu, bv, __uint_as_float(prim), __uint_as_float(i));
-                q.hA[k] = q.A[in][i]; q.hB[k] = q.B[in][i]; q.hC[k] = q.C[in][i];
-            }
-#else
-            if (hit) q.hitq[(uint32_t)slot + __popc(hmask & lt_mask)] = make_float4(bu, bv, __uint_as_float(prim), __uint_as_float(i));
-#endif
-            else if (live) q.missq[(uint32_t)(slot >> 32) + __popc(mmask & lt_mask)] = i;
-        }
-    }
-    if (COUNT) { warp_sum64(&ctr->nodes_ext[bounce], nv); warp_sum64(&ctr->tris_ext[bounce], nt); }
 }
 
 template <bool COUNT, int SMEM>
@@ -451,10 +426,9 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_closest(FrameParam
 {
     extern __shared__ __align__(128) float4 s_bvh[];
     __shared__ uint64_t s_mbar;
-    if (SMEM == 1) tma_stage_bvh(s_bvh, sc, &s_mbar);
-    if (SMEM == 2) tma_stage_top(s_bvh, sc.wnodes, sc.top_k, &s_mbar);
+    stage_bvh<SMEM>(s_bvh, sc, &s_mbar);
     pdl_wait(); pdl_launch_dependents();
-    closest_phase<COUNT, SMEM>(p, sc, mode, q, ctr, bounce, s_bvh);
+    closest_phase<COUNT, SMEM>(sc, mode, q, ctr, bounce, s_bvh);
 }
 
 // Closest-hit traversal of bounce b and the shadow pass of bounce b-1 in ONE persistent kernel (RT_OPT_OVERLAP = 2, the
@@ -467,13 +441,11 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_both(FrameParams p
 {
     extern __shared__ __align__(128) float4 s_bvh[];
     __shared__ uint64_t s_mbar;
-    if (SMEM == 1) tma_stage_bvh(s_bvh, sc, &s_mbar);
-    if (SMEM == 2) tma_stage_top(s_bvh, sc.wnodes, sc.top_k, &s_mbar);
+    stage_bvh<SMEM>(s_bvh, sc, &s_mbar);
     pdl_wait(); pdl_launch_dependents();
-    closest_phase<false, SMEM>(p, sc, mode, q, ctr, bounce, s_bvh);
+    closest_phase<false, SMEM>(sc, mode, q, ctr, bounce, s_bvh);
     shadow_phase<false, SMEM>(p, sc, mode, q, ctr, radiance, shadow_bounce, s_bvh);
 }
-
 
 // ShadeSurfaceHits over the hit queue, then ShadeMissedRays over the miss queue (independent pixels).
 __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce, AovParams aov)
@@ -481,46 +453,19 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
     pdl_wait(); pdl_launch_dependents();
     const uint32_t n_hit = ctr->hm[bounce].hit, n_miss = ctr->hm[bounce].miss;
     const uint32_t hit_span = (n_hit + 31u) & ~31u;            // warps never mix hits and misses
-    const uint32_t total = hit_span + n_miss;
-    const int in = bounce & 1;
     const int lane = threadIdx.x & 31;
-    for (;;)
+    for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < hit_span + n_miss;)
     {
-        uint32_t base = 0;
-        if (lane == 0) base = atomicAdd(&ctr->work_shade[bounce], 32u);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= total) break;
-        if (base < hit_span)
+        if (at < hit_span)
         {
-            uint32_t k = base + lane;
-            bool hit = k < n_hit;
-            uint32_t pixel = 0;
-            ShadeOut so;
-            so.emissive = so.spawn_next = so.spawn_shadow = false;
-            if (hit)
-            {
-                float4 h = q.hitq[k];
-#ifdef RT_HITQ_CARRY
-                float4 a = q.hA[k], b = q.hB[k], c = q.hC[k];
-#else
-                uint32_t i = __float_as_uint(h.w);
-                float4 a = q.A[in][i], b = q.B[in][i], c = q.C[in][i];
-#endif
-                pixel = __float_as_uint(a.w);
-                shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), __float_as_uint(h.z), h.x, h.y, so);
-            }
-            emit_rays(p, q, ctr, radiance, bounce, pixel, hit, so);
+            const uint32_t k = at + lane;
+            const bool hit = k < n_hit;
+            float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            if (hit) h = q.hitq[k];
+            uint32_t pixel;
+            shade_hit_group(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
         }
-        else
-        {
-            uint32_t k = base - hit_span + lane;
-            if (k < n_miss)
-            {
-                uint32_t i = q.missq[k];
-                float4 a = q.A[in][i], b = q.B[in][i], c = q.C[in][i];
-                shade_miss(sc, p, radiance, __float_as_uint(a.w), mk3(b), mk3(c));
-            }
-        }
+        else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
     }
 }
 
@@ -656,7 +601,6 @@ struct rt_ctx
     // options
     int white_furnace = 0, sampler = 0, aov = 0, denoiser = 0, count_traversal = 0, kernel_timing = 0, traversal = 1, smem_bvh = 1;
     uint32_t top_smem_records = 0;                 // RT_OPT_TOP_SMEM
-    int bvh_depth = 0;
 
     // per-pixel buffers
     Queues q = {};
@@ -704,8 +648,8 @@ struct rt_ctx
     int frame_threads = 0;         // RT_OPT_FRAME_THREADS: threads per CTA of k_frame (0 = by partition size)
     size_t n_alloc = 0;            // entries of every per-pixel queue: n_local + one group of 32 per CTA that can be resident (k_frame's regions)
     int* d_bn = nullptr;           // sobol | scrambling | ranking (rt_upload_sampler_tables)
-    struct Occupancy { const void* kernel; size_t smem; int per_sm; };
-    std::vector<Occupancy> occupancy;   // resident CTAs per SM of each persistent kernel (persistent_grid)
+    struct Occupancy { const void* kernel; int threads; size_t smem; int per_sm; };
+    std::vector<Occupancy> occupancy;   // resident CTAs per SM of each persistent kernel (resident_per_sm)
     void* scratch = nullptr; size_t scratch_bytes = 0;
 
     // scene
@@ -840,6 +784,17 @@ void free_aov_buffers(rt_ctx* c);
 bool aov_wanted(const rt_ctx* c);
 int ensure_aov_buffers(rt_ctx* c);
 
+// the per-pixel buffers: queues, radiance, resolve targets, AOVs
+void free_frame_buffers(rt_ctx* c)
+{
+    auto freep = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
+    for (int i = 0; i < 2; ++i) { freep(c->q.A[i]); freep(c->q.B[i]); freep(c->q.C[i]); }
+    freep(c->q.sA); freep(c->q.sB); freep(c->q.sC); freep(c->q.hits); freep(c->q.shadow_flags);
+    freep(c->q.hitq); freep(c->q.missq);
+    freep(c->radiance); freep(c->resolved); freep(c->resolved2);
+    free_aov_buffers(c);
+}
+
 int alloc_frame_buffers(rt_ctx* c)
 {
     if (c->stream) cudaStreamSynchronize(c->stream);
@@ -847,12 +802,7 @@ int alloc_frame_buffers(rt_ctx* c)
     if (c->copy_stream) cudaStreamSynchronize(c->copy_stream); // a pipelined read-back may still be reading the resolve buffers
     c->shadow_pending = false; c->shadow_deferred = false;     // the frame in flight (if any) is abandoned with its buffers
     ++c->config_gen;
-    auto freep = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
-    for (int i = 0; i < 2; ++i) { freep(c->q.A[i]); freep(c->q.B[i]); freep(c->q.C[i]); }
-    freep(c->q.sA); freep(c->q.sB); freep(c->q.sC); freep(c->q.hits); freep(c->q.shadow_flags);
-    freep(c->q.hitq); freep(c->q.missq);
-    freep(c->radiance); freep(c->resolved); freep(c->resolved2);
-    free_aov_buffers(c);
+    free_frame_buffers(c);
     c->local_rows = (c->height > c->rank) ? (c->height - c->rank + c->world - 1) / c->world : 0;
     c->n_local = c->local_rows * c->width;
     // k_frame gives every resident CTA its own region of each queue, rounded up to whole groups of 32 slots
@@ -865,9 +815,6 @@ int alloc_frame_buffers(rt_ctx* c)
     RT_CUDA(c, cudaMalloc(&c->q.sA, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.sB, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.sC, n * 16));
     RT_CUDA(c, cudaMalloc(&c->q.hits, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.shadow_flags, n * 4));
     RT_CUDA(c, cudaMalloc(&c->q.hitq, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.missq, n * 4));
-#ifdef RT_HITQ_CARRY
-    RT_CUDA(c, cudaMalloc(&c->q.hA, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.hB, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.hC, n * 16));
-#endif
     RT_CUDA(c, cudaMalloc(&c->radiance, n * 16)); RT_CUDA(c, cudaMalloc(&c->resolved, n * 16));
     RT_CUDA(c, cudaMemsetAsync(c->radiance, 0, n * 16, c->stream));
     c->copy_pending[0] = c->copy_pending[1] = false;          // both streams were drained above
@@ -878,16 +825,19 @@ int alloc_frame_buffers(rt_ctx* c)
 // Grid of a persistent kernel: exactly the CTAs that are resident at once (occupancy x SMs) — CTAs of a second wave
 // would only start, find the cursor exhausted and exit — and no more CTAs than there can be work for (a rank of a
 // multi-GPU partition owns few pixels).  Measured: -1.4 % frame time on one GPU, -5 % on a 1/8 partition.
+// resident CTAs per SM of a kernel at a launch shape, looked up once per context
+int resident_per_sm(rt_ctx* c, const void* kernel, int threads, size_t smem)
+{
+    for (auto& e : c->occupancy) if (e.kernel == kernel && e.threads == threads && e.smem == smem) return e.per_sm;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+    c->occupancy.push_back({ kernel, threads, smem, per_sm });
+    return per_sm;
+}
+
 int persistent_grid(rt_ctx* c, const void* kernel, size_t dyn_smem)
 {
-    int per_sm = 0;
-    for (auto& e : c->occupancy) if (e.kernel == kernel && e.smem == dyn_smem) { per_sm = e.per_sm; break; }
-    if (!per_sm)
-    {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, dyn_smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-        c->occupancy.push_back({ kernel, dyn_smem, per_sm });
-    }
-    int g = c->num_sms * per_sm / c->grid_div;
+    int g = c->num_sms * resident_per_sm(c, kernel, 256, dyn_smem) / c->grid_div;
     if (g < c->num_sms) g = c->num_sms;
     int need = (int)((c->n_local + 255u) / 256u);
     if (need < 1) need = 1;
@@ -928,16 +878,20 @@ Stage bvh_stage(const rt_ctx* c)
     if (k >= 8) { st.mode = 2; st.bytes = (size_t)k * 64; st.top_k = k; }
     return st;
 }
-size_t smem_stage_bytes(const rt_ctx* c) { return bvh_stage(c).bytes; }
-DevScene staged_scene(const rt_ctx* c, const Stage& st) { DevScene sc = c->scene; sc.top_k = st.top_k; sc.stack_off = (uint32_t)((st.bytes + 127) & ~(size_t)127); return sc; }
-// kernels that ask for more than 48 KB of dynamic shared memory need the limit raised first
-void set_smem_limit(const void* kernel, size_t bytes) { if (bytes > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes); }
-#ifdef RT_SMEM_STACK
-// experiment: dynamic shared memory of the per-phase traversal kernels = staged BVH + one stack column per thread
-size_t with_stack(const rt_ctx* c, size_t stage) { return ((stage + 127) & ~(size_t)127) + (size_t)c->bvh_depth * 256 * 8; }
-#else
-size_t with_stack(const rt_ctx*, size_t stage) { return stage; }
-#endif
+
+// Launches a staged traversal kernel: calls launch(std::integral_constant<int, SMEM>, the DevScene with this launch's top_k, the
+// dynamic shared-memory bytes) once, for the launch's staging mode, and returns its result.  At most 40 KB are staged, under the
+// 48 KB that every kernel may take without raising its shared-memory limit.
+template <class F>
+auto launch_staged(const rt_ctx* c, F&& launch)
+{
+    const Stage sg = bvh_stage(c);
+    DevScene sc = c->scene;
+    sc.top_k = sg.top_k;
+    if (sg.mode == 1) return launch(std::integral_constant<int, 1>(), sc, sg.bytes);
+    if (sg.mode == 2) return launch(std::integral_constant<int, 2>(), sc, sg.bytes);
+    return launch(std::integral_constant<int, 0>(), sc, sg.bytes);
+}
 
 AovCam aov_cam(const RtCamera& cam);
 
@@ -1050,10 +1004,8 @@ int rt_destroy(rt_ctx* c)
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->shadow_stream) cudaStreamSynchronize(c->shadow_stream);
-    for (int i = 0; i < 2; ++i) { cudaFree(c->q.A[i]); cudaFree(c->q.B[i]); cudaFree(c->q.C[i]); }
-    cudaFree(c->q.sA); cudaFree(c->q.sB); cudaFree(c->q.sC); cudaFree(c->q.hits); cudaFree(c->q.shadow_flags);
-    cudaFree(c->q.hitq); cudaFree(c->q.missq);
-    cudaFree(c->radiance); cudaFree(c->resolved); cudaFree(c->resolved2); cudaFree(c->counters); cudaFree(c->scratch); cudaFree(c->d_dyn); cudaFree(c->d_bn); cudaFree(c->resolved_full[0]); cudaFree(c->resolved_full[1]);
+    free_frame_buffers(c);
+    cudaFree(c->counters); cudaFree(c->scratch); cudaFree(c->d_dyn); cudaFree(c->d_bn); cudaFree(c->resolved_full[0]); cudaFree(c->resolved_full[1]);
     if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
     if (c->graph) cudaGraphDestroy(c->graph);
     if (c->shadow_stream) { cudaStreamSynchronize(c->shadow_stream); cudaStreamDestroy(c->shadow_stream); }
@@ -1061,7 +1013,6 @@ int rt_destroy(rt_ctx* c)
     if (c->ev_shadowed) cudaEventDestroy(c->ev_shadowed);
     for (int i = 0; i < 2; ++i) { if (c->resolve_done[i]) cudaEventDestroy(c->resolve_done[i]); if (c->copy_done[i]) cudaEventDestroy(c->copy_done[i]); }
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
-    free_aov_buffers(c);
     cudaFree(c->own_gather);
     for (void* p : c->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void* p : c->scene_allocs) cudaFree(p);
@@ -1166,8 +1117,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
         if ((rc = upload(wl.tris.data(), wl.tris.size() * 16, (const void**)&ds.wtris))) return rc;
         ds.root_ref = wl.root_ref;
         ds.wnodes_f4 = (uint32_t)wl.nodes.size(); ds.wtris_f4 = (uint32_t)wl.tris.size();
-        ds.top_n = wl.top_n; ds.top_k = 0; ds.stack_off = 0;
-        c->bvh_depth = wl.max_depth;
+        ds.top_n = wl.top_n; ds.top_k = 0;
     }
     c->scene_ready = true;
     ++c->config_gen;
@@ -1424,26 +1374,20 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     {   // this bounce's closest-hit traversal + the previous bounce's shadow pass in one kernel
         c->shadow_deferred = false;
         TimedLaunch t(c, RT_K_TRACE_BOTH);
-        const Stage sg = bvh_stage(c);
-        const DevScene sc = staged_scene(c, sg);
-        const size_t sm = with_stack(c, sg.bytes);
-        set_smem_limit((const void*)k_trace_both<0>, sm); set_smem_limit((const void*)k_trace_both<1>, sm); set_smem_limit((const void*)k_trace_both<2>, sm);
-        if (sg.mode == 1) launch_chain(c, k_trace_both<1>, RT_PGRID(c, k_trace_both<1>, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce, c->shadow_deferred_bounce);
-        else if (sg.mode == 2) launch_chain(c, k_trace_both<2>, RT_PGRID(c, k_trace_both<2>, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce, c->shadow_deferred_bounce);
-        else launch_chain(c, k_trace_both<0>, RT_PGRID(c, k_trace_both<0>, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce, c->shadow_deferred_bounce);
+        launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) {
+            auto* k = k_trace_both<smem.value>;
+            launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce, c->shadow_deferred_bounce);
+        });
         int rc = post_launch(c, "k_trace_both"); if (rc) return rc;
     }
     else
     {
         TimedLaunch t(c, RT_K_TRACE_CLOSEST);
-        const Stage sg = bvh_stage(c);
-        const DevScene sc = staged_scene(c, sg);
-        const size_t sm = with_stack(c, sg.bytes);
-        set_smem_limit((const void*)k_trace_closest<false, 0>, sm); set_smem_limit((const void*)k_trace_closest<false, 1>, sm); set_smem_limit((const void*)k_trace_closest<false, 2>, sm);
         if (c->count_traversal) k_trace_closest<true, 0><<<RT_PGRID(c, (k_trace_closest<true, 0>), 0), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
-        else if (sg.mode == 1) launch_chain(c, k_trace_closest<false, 1>, RT_PGRID(c, (k_trace_closest<false, 1>), sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
-        else if (sg.mode == 2) launch_chain(c, k_trace_closest<false, 2>, RT_PGRID(c, (k_trace_closest<false, 2>), sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
-        else launch_chain(c, k_trace_closest<false, 0>, RT_PGRID(c, (k_trace_closest<false, 0>), sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
+        else launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) {
+            auto* k = k_trace_closest<false, smem.value>;
+            launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
+        });
         int rc = post_launch(c, "k_trace_closest"); if (rc) return rc;
     }
     { int rc = join_shadow(c); if (rc) return rc; }     // the shading pass accumulates into radiance and refills the shadow queue
@@ -1452,17 +1396,24 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     return post_launch(c, "k_shade_queues");
 }
 
+// the second stream of RT_OPT_OVERLAP 1 and its two events
+static int ensure_shadow_stream(rt_ctx* c)
+{
+    if (c->shadow_stream) return RT_OK;
+    RT_CUDA(c, cudaStreamCreateWithFlags(&c->shadow_stream, cudaStreamNonBlocking));
+    RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shaded, cudaEventDisableTiming));
+    RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shadowed, cudaEventDisableTiming));
+    return RT_OK;
+}
+
 static int launch_shadow_pass(rt_ctx* c, uint32_t bounce, cudaStream_t st)
 {
     TimedLaunch t(c, RT_K_SHADOW_ACCUMULATE, st);
-    const Stage sg = bvh_stage(c);
-    const DevScene sc = staged_scene(c, sg);
-    const size_t sm = with_stack(c, sg.bytes);
-    set_smem_limit((const void*)k_shadow_accumulate<false, 0>, sm); set_smem_limit((const void*)k_shadow_accumulate<false, 1>, sm); set_smem_limit((const void*)k_shadow_accumulate<false, 2>, sm);
     if (c->count_traversal) k_shadow_accumulate<true, 0><<<RT_PGRID(c, (k_shadow_accumulate<true, 0>), 0), 256, 0, st>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->radiance, bounce);
-    else if (sg.mode == 1) k_shadow_accumulate<false, 1><<<RT_PGRID(c, (k_shadow_accumulate<false, 1>), sm), 256, sm, st>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce);
-    else if (sg.mode == 2) k_shadow_accumulate<false, 2><<<RT_PGRID(c, (k_shadow_accumulate<false, 2>), sm), 256, sm, st>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce);
-    else k_shadow_accumulate<false, 0><<<RT_PGRID(c, (k_shadow_accumulate<false, 0>), sm), 256, sm, st>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce);
+    else launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) {
+        auto* k = k_shadow_accumulate<false, smem.value>;
+        k<<<RT_PGRID(c, k, sm), 256, sm, st>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce);
+    });
     return post_launch(c, "k_shadow_accumulate");
 }
 
@@ -1480,12 +1431,7 @@ int rt_shadow_accumulate(rt_ctx* c, uint32_t bounce)
     if (c->overlap != 1) return launch_shadow_pass(c, bounce, c->stream);
     // overlap 1: second stream; join_shadow() orders it before the next kernel that needs its results.  Both kernels are
     // persistent, so the second fills the SMs as the first drains.
-    if (!c->shadow_stream)
-    {
-        RT_CUDA(c, cudaStreamCreateWithFlags(&c->shadow_stream, cudaStreamNonBlocking));
-        RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shaded, cudaEventDisableTiming));
-        RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shadowed, cudaEventDisableTiming));
-    }
+    if ((rc = ensure_shadow_stream(c))) return rc;
     cudaStream_t st = c->shadow_stream;
     RT_CUDA(c, cudaEventRecord(c->ev_shaded, c->stream));
     RT_CUDA(c, cudaStreamWaitEvent(st, c->ev_shaded, 0));
@@ -1518,12 +1464,7 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
 {
     drop_graph(c);
     int rc = join_shadow(c); if (rc) return rc;
-    if (c->overlap == 1 && !c->shadow_stream)
-    {   // create the second stream and its events outside the capture
-        RT_CUDA(c, cudaStreamCreateWithFlags(&c->shadow_stream, cudaStreamNonBlocking));
-        RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shaded, cudaEventDisableTiming));
-        RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shadowed, cudaEventDisableTiming));
-    }
+    if (c->overlap == 1 && (rc = ensure_shadow_stream(c))) return rc;      // created outside the capture
     const uint32_t saved_samples = c->sample_count, saved_bounce = c->cur_bounce;
     const uint64_t saved_launches = c->launches;
     const bool saved_started = c->frame_started;
@@ -1604,36 +1545,25 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces)
     if ((rc = join_shadow(c))) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
     RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
-    const Stage sg = bvh_stage(c);
-    const DevScene sc = staged_scene(c, sg);
-    const size_t stage = sg.bytes;
-    const void* kern = sg.mode == 1 ? (const void*)k_frame<1> : (sg.mode == 2 ? (const void*)k_frame<2> : (const void*)k_frame<0>);
     const int threads = frame_kernel_threads(c);
-    int per_sm = 0;
-    for (auto& e : c->occupancy) if (e.kernel == kern && e.smem == stage + ((size_t)threads << 32)) { per_sm = e.per_sm; break; }
-    if (!per_sm)
-    {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, stage) != cudaSuccess || per_sm < 1) per_sm = 1;
-        if (per_sm > 32) per_sm = 32;
-        c->occupancy.push_back({ kern, stage + ((size_t)threads << 32), per_sm });
-    }
-    const uint32_t n_groups = (c->n_local + 31u) / 32u;
-    uint32_t grid = (uint32_t)(c->num_sms * per_sm / c->grid_div);
-    if (grid < (uint32_t)c->num_sms) grid = (uint32_t)c->num_sms;
-    if (grid > n_groups) grid = n_groups;
-    if (grid < 1) grid = 1;
-    const uint32_t slots_per_cta = ((n_groups + grid - 1u) / grid) * 32u;
-    if ((size_t)grid * slots_per_cta > c->n_alloc) RT_FAIL(c, RT_ERR_CUDA, "frame kernel: queue regions exceed the allocation");
     const FrameDyn dyn = frame_dyn(c);
     FrameParams fp = frame_params(c);
     fp.gather = c->gather_slab;
-    {
+    rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
+        auto* k = k_frame<smem.value>;
+        const int per_sm = std::min(resident_per_sm(c, (const void*)k, threads, sm), 32);
+        const uint32_t n_groups = (c->n_local + 31u) / 32u;
+        uint32_t grid = (uint32_t)(c->num_sms * per_sm / c->grid_div);
+        if (grid < (uint32_t)c->num_sms) grid = (uint32_t)c->num_sms;
+        if (grid > n_groups) grid = n_groups;
+        if (grid < 1) grid = 1;
+        const uint32_t slots_per_cta = ((n_groups + grid - 1u) / grid) * 32u;
+        if ((size_t)grid * slots_per_cta > c->n_alloc) RT_FAIL(c, RT_ERR_CUDA, "frame kernel: queue regions exceed the allocation");
         TimedLaunch t(c, RT_K_MISC);
-        if (sg.mode == 1) k_frame<1><<<grid, threads, stage, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
-        else if (sg.mode == 2) k_frame<2><<<grid, threads, stage, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
-        else k_frame<0><<<grid, threads, 0, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
-    }
-    if ((rc = post_launch(c, "k_frame"))) return rc;
+        k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
+        return RT_OK;
+    });
+    if (rc || (rc = post_launch(c, "k_frame"))) return rc;
     c->frame_started = true; c->cur_bounce = max_bounces;
     ++c->sample_count;
     return gather_signal(c, false);
@@ -1669,18 +1599,35 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
     return gather_signal(c, true);
 }
 
+// the resolve kernel of this context's rows into `out`, on its stream
+static int launch_resolve(rt_ctx* c, float4* out)
+{
+    TimedLaunch t(c, RT_K_RESOLVE);
+    const AovParams ap = aov_params(c);
+    k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, out, c->n_local, c->sample_count, c->denoiser, ap.enabled ? c->aov : 0, ap);
+    return post_launch(c, "k_resolve");
+}
+
+// the pipelined read-back's copy stream and its events
+static int ensure_copy_stream(rt_ctx* c)
+{
+    if (c->copy_stream) return RT_OK;
+    RT_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i)
+    {
+        RT_CUDA(c, cudaEventCreateWithFlags(&c->resolve_done[i], cudaEventDisableTiming));
+        RT_CUDA(c, cudaEventCreateWithFlags(&c->copy_done[i], cudaEventDisableTiming));
+    }
+    return RT_OK;
+}
+
 // resolve kernel + device->host copy of this context's rows, enqueued on its stream (no synchronisation)
 static int resolve_enqueue(rt_ctx* c, float* dst)
 {
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     RT_CUDA(c, cudaSetDevice(c->device));
     if (c->copy_pending[0]) RT_CUDA(c, cudaStreamWaitEvent(c->stream, c->copy_done[0], 0));   // rt_resolve_async may still copy out of c->resolved
-    {
-        TimedLaunch t(c, RT_K_RESOLVE);
-        k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, c->resolved, c->n_local, c->sample_count, c->denoiser,
-                                                                  aov_params(c).enabled ? c->aov : 0, aov_params(c));
-        int rc = post_launch(c, "k_resolve"); if (rc) return rc;
-    }
+    { int rc = launch_resolve(c, c->resolved); if (rc) return rc; }
     if (dst && c->local_rows)
         RT_CUDA(c, cudaMemcpy2DAsync(dst + (size_t)c->rank * c->width * 4, (size_t)c->world * c->width * 16, c->resolved,
                                      (size_t)c->width * 16, (size_t)c->width * 16, c->local_rows, cudaMemcpyDeviceToHost, c->stream));
@@ -1736,25 +1683,12 @@ int rt_resolve_async(rt_ctx* c, float* dst)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     if (!dst) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_resolve_async: null destination");
     RT_CUDA(c, cudaSetDevice(c->device));
-    if (!c->copy_stream)
-    {
-        RT_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; ++i)
-        {
-            RT_CUDA(c, cudaEventCreateWithFlags(&c->resolve_done[i], cudaEventDisableTiming));
-            RT_CUDA(c, cudaEventCreateWithFlags(&c->copy_done[i], cudaEventDisableTiming));
-        }
-    }
+    { int rc = ensure_copy_stream(c); if (rc) return rc; }
     if (!c->resolved2) RT_CUDA(c, cudaMalloc(&c->resolved2, (size_t)(c->n_local ? c->n_local : 1) * 16));
     const int k = (int)(c->async_index++ & 1u);
     float4* buf = k ? c->resolved2 : c->resolved;
     if (c->copy_pending[k]) RT_CUDA(c, cudaStreamWaitEvent(c->stream, c->copy_done[k], 0));   // buffer k is being re-used
-    {
-        TimedLaunch t(c, RT_K_RESOLVE);
-        AovParams ap = aov_params(c);
-        k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, buf, c->n_local, c->sample_count, c->denoiser, ap.enabled ? c->aov : 0, ap);
-        int rc = post_launch(c, "k_resolve"); if (rc) return rc;
-    }
+    { int rc = launch_resolve(c, buf); if (rc) return rc; }
     RT_CUDA(c, cudaEventRecord(c->resolve_done[k], c->stream));
     RT_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->resolve_done[k], 0));
     if (c->local_rows)
@@ -1779,15 +1713,7 @@ static int resolve_gathered_impl(rt_ctx* c, const void* slabs, uint64_t stride_b
     int k = 0;
     if (async)
     {
-        if (!c->copy_stream)
-        {
-            RT_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-            for (int i = 0; i < 2; ++i)
-            {
-                RT_CUDA(c, cudaEventCreateWithFlags(&c->resolve_done[i], cudaEventDisableTiming));
-                RT_CUDA(c, cudaEventCreateWithFlags(&c->copy_done[i], cudaEventDisableTiming));
-            }
-        }
+        { int rc = ensure_copy_stream(c); if (rc) return rc; }
         k = (int)(c->async_index++ & 1u);
         if (c->copy_pending[k]) RT_CUDA(c, cudaStreamWaitEvent(c->stream, c->copy_done[k], 0));
     }

@@ -1,5 +1,6 @@
 /*
- * rt_traverse.cuh — BVH staging (TMA bulk copies) and the traversal functions: literal reference-order traversal and the child-box layout traversal.
+ * rt_traverse.cuh — BVH staging (TMA bulk copies) and the traversal functions: literal reference-order traversal, the child-box layout
+ * traversal, and trace_staged, the traversal call of a kernel that staged the BVH.
  * Part of the single translation unit rt_kernels.cu (included there, inside its anonymous namespace).
  */
 #pragma once
@@ -14,10 +15,15 @@
 // is amortised over every ray the CTA traces.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void tma_stage_bvh(float4* dst, const DevScene& sc, uint64_t* mbar)
+// SMEM 1 stages the whole structure (records, then triangles: two bulk copies), SMEM 2 the first sc.top_k interior records —
+// breadth-first, the top of the tree (rt_bvh_layout.h) — with one bulk copy, deeper records and all triangles staying behind
+// L1/L2 (RT_OPT_TOP_SMEM); SMEM 0 stages nothing.
+template <int SMEM>
+__device__ __forceinline__ void stage_bvh(float4* dst, const DevScene& sc, uint64_t* mbar)
 {
+    if (SMEM == 0) return;
     const uint32_t bar = smem_u32(mbar);
-    const uint32_t nodes_bytes = sc.wnodes_f4 * 16u, tris_bytes = sc.wtris_f4 * 16u;
+    const uint32_t nodes_bytes = (SMEM == 1 ? sc.wnodes_f4 : sc.top_k * 4u) * 16u, tris_bytes = SMEM == 1 ? sc.wtris_f4 * 16u : 0u;
     if (threadIdx.x == 0)
     {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1));
@@ -30,33 +36,9 @@ __device__ __forceinline__ void tma_stage_bvh(float4* dst, const DevScene& sc, u
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(nodes_bytes + tris_bytes) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(smem_u32(dst)), "l"(sc.wnodes), "r"(nodes_bytes), "r"(bar) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(smem_u32(dst + sc.wnodes_f4)), "l"(sc.wtris), "r"(tris_bytes), "r"(bar) : "memory");
-    }
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(done) : "r"(bar), "r"(0) : "memory");
-}
-
-// Scenes that do not fit: only the top of the tree — the first `n_records` interior records, breadth-first (rt_bvh_layout.h) — is
-// staged, with one TMA bulk copy per CTA; deeper records and all triangles stay behind L1/L2 (RT_OPT_TOP_SMEM).
-__device__ __forceinline__ void tma_stage_top(float4* dst, const float4* wnodes, uint32_t n_records, uint64_t* mbar)
-{
-    const uint32_t bar = smem_u32(mbar);
-    const uint32_t bytes = n_records * 64u;
-    if (threadIdx.x == 0)
-    {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    __syncthreads();
-    if (threadIdx.x == 0)
-    {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(smem_u32(dst)), "l"(wnodes), "r"(bytes), "r"(bar) : "memory");
+        if (SMEM == 1)
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                         ::"r"(smem_u32(dst + sc.wnodes_f4)), "l"(sc.wtris), "r"(tris_bytes), "r"(bar) : "memory");
     }
     uint32_t done = 0;
     while (!done)
@@ -173,18 +155,9 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
     // (measured, same results): with the records in shared memory the kernel is purely issue-bound and the packed
     // 64-bit stack entry + the sign-bit axis test win (CornellBox frame -2.7 %); with the records behind L1/L2 the two
     // 32-bit arrays (a discarded pop costs one load) and predicate selects are faster (ShaderBalls +1 %, Dragon +3.5 %).
-#ifdef RT_SMEM_STACK
-    // experiment: the traversal stack in shared memory (entry i of thread t at [i * 256 + t]: conflict-free), per-phase kernels only
-    extern __shared__ __align__(128) float4 rt_dyn_smem[];
-    int2* const sstk = (int2*)((char*)rt_dyn_smem + sc.stack_off) + threadIdx.x;
-    constexpr bool SSTK = !PIN;
-#else
-    int2* const sstk = nullptr;
-    constexpr bool SSTK = false;
-#endif
-    int2 stack[(SMEM == 1 && !SSTK) ? 64 : 1];
-    int stack_ref[(SMEM == 1 || SSTK) ? 1 : 64];
-    float stack_t[(SMEM == 1 || SSTK) ? 1 : 64];
+    int2 stack[SMEM == 1 ? 64 : 1];
+    int stack_ref[SMEM == 1 ? 1 : 64];
+    float stack_t[SMEM == 1 ? 1 : 64];
     if (cur < 0)
     {   // single-leaf tree: the root box is tested like any visited node
         float4 r0 = __ldg(sc.nodes_ref), r1 = __ldg(sc.nodes_ref + 1);
@@ -235,8 +208,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
             {
                 if (far_hit)
                 {
-                    if (SSTK) sstk[sp * 256] = make_int2(far_ref, __float_as_int(far_lo));
-                    else if (SMEM == 1) stack[sp] = make_int2(far_ref, __float_as_int(far_lo));
+                    if (SMEM == 1) stack[sp] = make_int2(far_ref, __float_as_int(far_lo));
                     else { stack_ref[sp] = far_ref; stack_t[sp] = far_lo; }
                     ++sp;
                 }
@@ -250,8 +222,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
                 while (sp > 0)
                 {
                     --sp;
-                    if (SSTK) { int2 e = sstk[sp * 256]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
-                    else if (SMEM == 1) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
+                    if (SMEM == 1) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
                     else if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; }
                 }
                 if (!found) return prim;
@@ -302,8 +273,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
         while (sp > 0)
                 {
                     --sp;
-                    if (SSTK) { int2 e = sstk[sp * 256]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
-                    else if (SMEM == 1) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
+                    if (SMEM == 1) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
                     else if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; }
                 }
         if (!found) return prim;
@@ -316,4 +286,15 @@ __device__ __forceinline__ uint32_t trace(const DevScene& sc, int mode, f3 o, f3
 {
     if (mode == 0) return trace_literal<ANY, COUNT>(sc, o, d, t_min, t_max, bu, bv, bt, nv, nt);
     return trace_fast<ANY, COUNT, 0>(sc, sc.wnodes, sc.wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt);
+}
+
+// The traversal call of every persistent kernel, for the kernel's staging mode (stage_bvh): ray (a, b) = (origin, -), (dir, t_max).
+// PIN (trace_fast) is applied to the staged modes only.
+template <bool ANY, bool COUNT, int SMEM, bool PIN>
+__device__ __forceinline__ uint32_t trace_staged(const DevScene& sc, int mode, const float4* s_bvh, float4 a, float4 b,
+                                                 float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
+{
+    if (SMEM == 1) return trace_fast<ANY, COUNT, 1, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    if (SMEM == 2) return trace_fast<ANY, COUNT, 2, PIN>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    return trace<ANY, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
 }
