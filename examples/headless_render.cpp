@@ -1,7 +1,8 @@
 /*
  * examples/headless_render.cpp — the reference's main.cpp (src/main.cpp:30-79) minus the window: load an OBJ scene,
- * add the directional light main.cpp:58 adds, create a Render with the CUDA backend, render N progressive samples and
- * write the resolved image as a binary PFM.
+ * add the directional light main.cpp:58 adds, create a Render with the CUDA backend, render N progressive samples with one
+ * RenderFrame() (SetSamplesPerFrame: one rt_integrate_samples call, the same image as N frames of one sample) and write the
+ * resolved image as a binary PFM.
  *
  *   g++ -std=c++17 -O2 -Iinclude -Iraytracing_b200/host examples/headless_render.cpp \
  *       -Lraytracing_b200 -lrt_host -lrt_b200 -Wl,-rpath,'$ORIGIN/../raytracing_b200' -o examples/headless_render
@@ -37,7 +38,11 @@ int main(int argc, char** argv)
                                                      : new rt_host::Render(width, height, rt_host::Render::RenderBackend::kCUDA, scene, argv[2]));
         rt_host::Render& render = *owner;
         render.SetMaxBounces(8);
-        for (unsigned s = 0; s < samples; ++s) render.RenderFrame();                               // one sample per frame, accumulated
+        if (samples > 0)
+        {
+            render.SetSamplesPerFrame(samples);
+            render.RenderFrame();                                                                  // every sample in one call, accumulated
+        }
         std::FILE* f = std::fopen(argv[6], "wb");
         if (!f) { std::perror(argv[6]); return 1; }
         std::fprintf(f, "PF\n%u %u\n-1.0\n", width, height);

@@ -86,7 +86,10 @@ typedef enum RtOption {
                                    wavefront over its own pixels (queue cursors in shared memory, no global atomics, no launch
                                    boundaries); 0: one kernel per phase (graph replay / PDL chain as configured above);
                                    2 (default): the one-kernel frame for partitions of up to 7168 pixels per SM (0.95 M pixels,
-                                   under half a 1080p frame, on an H100's 132 SMs), per-phase kernels for larger ones.  Results are bit-identical */
+                                   under half a 1080p frame, on an H100's 132 SMs), per-phase kernels for larger ones.  Results are bit-identical.
+                                   rt_integrate_samples: 1 also selects the regenerating frame kernel (one launch per call), which is
+                                   bit-identical but measured slower than n one-kernel frames on scenes traversed through L1 (up to
+                                   29 % on ShaderBalls, DESIGN.md section 4); 0 and 2 run n frames of rt_integrate's schedule */
     RT_OPT_PRESENT = 27,        /* multi-device contexts, rt_resolve: 0 (default) parallel read-back of every device's rows,
                                    1 gather to devices[0] over NVLink, resolve and read back there */
     RT_OPT_FRAME_THREADS = 28,  /* threads per CTA of the one-kernel frame: 0 (default) by partition size, else a multiple of 32 <= 1024 */
@@ -96,8 +99,10 @@ typedef enum RtOption {
 } RtOption;
 
 #define RT_MAX_BOUNCES 255u     /* bounce index range supported per frame (reference GUI: 0..5) */
+#define RT_MAX_REGEN_SAMPLES (1u << 24)   /* n_samples limit of rt_integrate_samples on the regenerating kernel (RT_OPT_FRAME_KERNEL 1) */
 
-/* Per-bounce device counters of the last frame (index = bounce, 0..max_bounces). */
+/* Per-bounce device counters of the last rt_integrate / rt_integrate_samples call (index = bounce, 0..max_bounces); a
+ * multi-sample call returns the element-wise sums over its samples. */
 typedef struct RtFrameStats {
     uint32_t n_ext[RT_MAX_BOUNCES + 1];        /* rays entering closest-hit traversal (ray_counter, trace_bvh.cl:116) */
     uint32_t n_miss[RT_MAX_BOUNCES + 1];
@@ -229,6 +234,22 @@ int rt_shadow_accumulate(rt_ctx* ctx, uint32_t bounce);         /* IntersectShad
 /* GenerateRays + (max_bounces+1) x {extend_shade, shadow_accumulate} + AdvanceSampleCount, i.e. the body of
  * Integrator::Integrate between Reset() and ResolveRadiance(). */
 int rt_integrate(rt_ctx* ctx, uint32_t max_bounces);
+/* n_samples consecutive frames of rt_integrate(ctx, max_bounces) in one call.  The results are bit-identical to calling
+ * rt_integrate n_samples times: the radiance of every pixel, the sample count (n_samples higher), the AOV buffers (the last
+ * sample's values), the resolved image of every view and, once the call completes, the fused-gather slab.  rt_read_frame_stats
+ * returns the per-bounce counters summed over the call's samples.  With a gather target set, the completion flag is signalled
+ * once per call.
+ * With RT_OPT_FRAME_KERNEL = 1 (and neither RT_OPT_KERNEL_TIMING nor RT_OPT_COUNT_TRAVERSAL) the call is ONE launch of the
+ * regenerating frame kernel: when a pixel's path ends, its CTA starts that pixel's next sample in the next traversal round.  It
+ * carries a path's sample offset in 24 bits: n_samples > RT_MAX_REGEN_SAMPLES is RT_ERR_INVALID_ARGUMENT there.
+ * Otherwise, the default included, the frame rt_integrate would run is run n_samples times (measured on H100, the regenerating
+ * kernel is not faster at any partition size; DESIGN.md section 4); the fused gather is pushed by the last frame only.
+ * n_samples == 1 is rt_integrate.  The stepwise taps (rt_read_rays, rt_read_hits) find no rays of a multi-sample call that ran
+ * the one-kernel frame, and the last frame's rays after one that ran the per-phase frames.
+ * Errors, checked before anything is enqueued: RT_ERR_INVALID_ARGUMENT for n_samples == 0, a sample count that would wrap
+ * uint32_t, or max_bounces > RT_MAX_BOUNCES; RT_ERR_UNSUPPORTED for n_samples > 1 with the
+ * temporal denoiser on (it runs once per sample).  Multi-device contexts fan out like rt_integrate. */
+int rt_integrate_samples(rt_ctx* ctx, uint32_t max_bounces, uint32_t n_samples);
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

@@ -28,7 +28,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_reset", "rt_advance_sample_count", "rt_generate_rays", "rt_intersect", "rt_compute_aovs", "rt_shade_miss",
            "rt_clear_outgoing_counter", "rt_clear_shadow_counter", "rt_shade_hits", "rt_intersect_shadow",
            "rt_accumulate_direct", "rt_denoise", "rt_copy_history", "rt_resolve", "rt_resolve_async", "rt_resolve_wait", "rt_resolve_gathered", "rt_resolve_gathered_async", "rt_extend_shade", "rt_shadow_accumulate",
-           "rt_integrate", "rt_sync", "rt_read_hits", "rt_read_rays", "rt_read_radiance", "rt_read_frame_stats",
+           "rt_integrate", "rt_integrate_samples", "rt_sync", "rt_read_hits", "rt_read_rays", "rt_read_radiance", "rt_read_frame_stats",
            "rt_read_sample_count", "rt_read_aovs", "rt_kernel_times", "rt_launch_count", "rt_local_pixel_count",
            "rt_radiance_device_ptr", "rt_stream_handle",
            "rt_create_multi", "rt_device_count", "rt_gather_radiance", "rt_host_register", "rt_host_unregister", "rt_math_eval",
@@ -83,6 +83,7 @@ def load_library():
     for name in ("rt_intersect", "rt_shade_miss", "rt_clear_outgoing_counter", "rt_shade_hits", "rt_extend_shade",
                  "rt_shadow_accumulate", "rt_integrate"):
         getattr(L, name).argtypes = [C.c_void_p, C.c_uint32]
+    L.rt_integrate_samples.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
     L.rt_resolve.argtypes = [C.c_void_p, C.c_void_p]
     L.rt_resolve_async.argtypes = [C.c_void_p, C.c_void_p]
     L.rt_resolve_wait.argtypes = [C.c_void_p]
@@ -229,6 +230,12 @@ class Context:
     def extend_shade(self, bounce): self._ck(self.lib.rt_extend_shade(self.h, bounce))
     def shadow_accumulate(self, bounce): self._ck(self.lib.rt_shadow_accumulate(self.h, bounce))
     def integrate(self, max_bounces): self._ck(self.lib.rt_integrate(self.h, max_bounces))
+
+    def integrate_samples(self, max_bounces, n_samples):
+        """n_samples consecutive frames of integrate(max_bounces) in one call (rt_integrate_samples): the same bits, the frame
+        statistics summed over the samples."""
+        self._ck(self.lib.rt_integrate_samples(self.h, max_bounces, n_samples))
+
     def sync(self): self._ck(self.lib.rt_sync(self.h))
 
     def integrate_stepwise(self, max_bounces):

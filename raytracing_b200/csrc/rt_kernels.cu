@@ -80,9 +80,9 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
     if (p.gather) p.gather[li] = r;        // the path ends here: its pixel is final (its last shadow ray was accumulated a phase ago)
 }
 
-// kernels/cl/hit_surface.cl:30-186
+// kernels/cl/hit_surface.cl:30-186, for the path of sample p.dyn->sample_idx + sample_offset (a later sample of a multi-sample call)
 __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
-                                          f3 ray_origin, f3 ray_dir, f3 hit_throughput, uint32_t prim, float u, float v, ShadeOut& out)
+                                          f3 ray_origin, f3 ray_dir, f3 hit_throughput, uint32_t prim, float u, float v, uint32_t sample_offset, ShadeOut& out)
 {
     f3 incoming = -ray_dir;
     uint32_t px = pxy & 0xFFFFu, py = pxy >> 16;
@@ -118,9 +118,9 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         out.emissive = true;
         out.emission_add = hit_throughput * material.emission;
     }
-    uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx);
+    uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx + sample_offset);
     {   // direct lighting (next-event estimation on analytic lights)
-        float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx, bounce * 5u + SAMPLE_LIGHT)
+        float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx + sample_offset, bounce * 5u + SAMPLE_LIGHT)
                              : sample_random(pixel_seed, bounce, SAMPLE_LIGHT);
         f3 outgoing; float pdf, distance_to_light;
         f3 light_radiance = light_sample(sc, position, s_light, outgoing, distance_to_light, pdf);
@@ -142,7 +142,7 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         f2 s; float s1;
         if (p.bn)
         {
-            const uint32_t sample_idx = p.dyn->sample_idx;
+            const uint32_t sample_idx = p.dyn->sample_idx + sample_offset;
             s.x = sample_blue_noise(p.bn, px, py, sample_idx, bounce * 5u + SAMPLE_U);
             s.y = sample_blue_noise(p.bn, px, py, sample_idx, bounce * 5u + SAMPLE_V);
             s1 = sample_blue_noise(p.bn, px, py, sample_idx, bounce * 5u + SAMPLE_LAYER);
@@ -170,15 +170,17 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
 // kernels and the CTA's region of every queue for k_frame.  The slot and statistics counters are global memory (DevCounters)
 // for the per-phase kernels and shared memory (CtaFrame) for k_frame.
 
-// RayGeneration (raygeneration.cl:65-139): the primary ray (a, b) of local pixel li, stored in slot `slot` of ray queue 0
-__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, uint32_t slot, uint32_t li, float4& a, float4& b)
+// RayGeneration (raygeneration.cl:65-139): the primary ray (a, b) of local pixel li for sample `sample_idx`, stored in slot `slot`
+// of ray queue `in` with `state` in C.w (the path state of the regenerating frame kernel; 0 everywhere else)
+__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, int in, uint32_t slot, uint32_t li,
+                                            uint32_t sample_idx, uint32_t state, float4& a, float4& b)
 {
     const uint32_t px = li % p.width, py = (li / p.width) * p.world + p.rank;
     f3 o, d;
-    generate_primary_ray(p.dyn->raygen, py * p.width + px, px, py, p.dyn->sample_idx, o, d);
+    generate_primary_ray(p.dyn->raygen, py * p.width + px, px, py, sample_idx, o, d);
     a = make_float4(o.x, o.y, o.z, __uint_as_float(pack_pixel(px, py)));
     b = make_float4(d.x, d.y, d.z, RT_MAX_RENDER_DIST);
-    q.A[0][slot] = a; q.B[0][slot] = b; q.C[0][slot] = make_float4(1.0f, 1.0f, 1.0f, 0.0f);
+    q.A[in][slot] = a; q.B[in][slot] = b; q.C[in][slot] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(state));
     if (aov.enabled)
     {   // raygeneration.cl:129-133
         aov.albedo[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -245,7 +247,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
     {
         const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
         pixel = __float_as_uint(a.w);
-        shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), __float_as_uint(h.z), h.x, h.y, so);
+        shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), __float_as_uint(h.z), h.x, h.y, 0u, so);
         if (so.emissive) add_radiance(radiance, local_index(p, pixel), so.emission_add);
     }
     const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
@@ -294,7 +296,7 @@ __global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCoun
     if (li == 0) ctr->n_primary = p.n_local;
     if (li >= p.n_local) return;
     float4 a, b;
-    primary_ray(p, q, aov, li, li, a, b);
+    primary_ray(p, q, aov, 0, li, li, p.dyn->sample_idx, 0u, a, b);
 }
 
 // IntersectRays (stepwise): closest hit of every live ray of bounce b -> hits[]
@@ -570,6 +572,21 @@ __global__ void k_math_eval(int fn, const float* a, const float* b, float* out, 
     out[i] = r;
 }
 
+// rt_integrate_samples on the per-frame path: the statistics of `frames` frames (added up in f by k_frame, or one per-phase frame)
+// added into the call's sums (one CTA).  Every frame has f->n_primary primary rays.
+__global__ void __launch_bounds__(256) k_add_counters(DevCounters* sum, const DevCounters* f, uint32_t frames)
+{
+    for (uint32_t b = threadIdx.x; b <= RT_MAX_BOUNCES; b += blockDim.x)
+    {
+        sum->emit[b].shadow += f->emit[b].shadow; sum->emit[b].next += f->emit[b].next;
+        sum->hm[b].hit += f->hm[b].hit; sum->hm[b].miss += f->hm[b].miss;
+        sum->n_emissive[b] += f->n_emissive[b]; sum->n_unoccluded[b] += f->n_unoccluded[b];
+        sum->nodes_ext[b] += f->nodes_ext[b]; sum->tris_ext[b] += f->tris_ext[b];
+        sum->nodes_shadow[b] += f->nodes_shadow[b]; sum->tris_shadow[b] += f->tris_shadow[b];
+    }
+    if (threadIdx.x == 0) sum->n_primary += f->n_primary * frames;
+}
+
 __global__ void k_unpack_rays(const float4* A, const float4* B, const uint32_t* count, uint32_t width, RtRay* rays, uint32_t* pixels)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -636,6 +653,8 @@ struct rt_ctx
     int aov_always = 0;
     RtCamera prev_camera = {}, aov_prev_camera = {};
     DevCounters* counters = nullptr;
+    DevCounters* counters_sum = nullptr;           // rt_integrate_samples: the statistics summed over the call's samples
+    bool stats_summed = false;                     // rt_read_frame_stats reads counters_sum (after rt_integrate_samples) instead of counters
     FrameDyn* d_dyn = nullptr;
     bool pdl = true;               // RT_OPT_PDL
     int frame_kernel = 2;          // RT_OPT_FRAME_KERNEL: 1 rt_integrate launches ONE persistent kernel per frame (k_frame), 0 one kernel per phase, 2 by partition size
@@ -1005,7 +1024,7 @@ int rt_destroy(rt_ctx* c)
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->shadow_stream) cudaStreamSynchronize(c->shadow_stream);
     free_frame_buffers(c);
-    cudaFree(c->counters); cudaFree(c->scratch); cudaFree(c->d_dyn); cudaFree(c->d_bn); cudaFree(c->resolved_full[0]); cudaFree(c->resolved_full[1]);
+    cudaFree(c->counters); cudaFree(c->counters_sum); cudaFree(c->scratch); cudaFree(c->d_dyn); cudaFree(c->d_bn); cudaFree(c->resolved_full[0]); cudaFree(c->resolved_full[1]);
     if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
     if (c->graph) cudaGraphDestroy(c->graph);
     if (c->shadow_stream) { cudaStreamSynchronize(c->shadow_stream); cudaStreamDestroy(c->shadow_stream); }
@@ -1260,6 +1279,7 @@ int rt_generate_rays(rt_ctx* c)
     int rc = require_ready(c); if (rc) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
     RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
+    c->stats_summed = false;
     TimedLaunch t(c, RT_K_RAYGEN);
     {
         FrameDyn dyn = frame_dyn(c);
@@ -1538,27 +1558,41 @@ static int gather_signal(rt_ctx* c, bool copy_slab)
     return post_launch(c, "k_gather_signal");
 }
 
-// The whole frame as ONE persistent kernel (k_frame): a counter clear and a launch.
-static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces)
+// Launch shape of the one-kernel frames (k_frame, k_frame_regen): the CTAs that are resident at once, at most one per group of 32
+// pixels, and the slots of each CTA's region of every queue.
+static int frame_kernel_grid(rt_ctx* c, const void* k, int threads, size_t sm, uint32_t& grid, uint32_t& slots_per_cta)
+{
+    const int per_sm = std::min(resident_per_sm(c, k, threads, sm), 32);
+    const uint32_t n_groups = (c->n_local + 31u) / 32u;
+    grid = (uint32_t)(c->num_sms * per_sm / c->grid_div);
+    if (grid < (uint32_t)c->num_sms) grid = (uint32_t)c->num_sms;
+    if (grid > n_groups) grid = n_groups;
+    if (grid < 1) grid = 1;
+    slots_per_cta = ((n_groups + grid - 1u) / grid) * 32u;
+    if ((size_t)grid * slots_per_cta > c->n_alloc) RT_FAIL(c, RT_ERR_CUDA, "frame kernel: queue regions exceed the allocation");
+    return RT_OK;
+}
+
+// Does a frame run as the one-kernel frame?  (The traversal counters and the kernel timing need the per-phase kernels.)
+static bool one_kernel_frame(const rt_ctx* c) { return frame_kernel_selected(c) && !c->kernel_timing && !c->count_traversal; }
+
+// The whole frame as ONE persistent kernel (k_frame): a counter clear and a launch.  It pushes the fused gather's pixels itself
+// when `push`.  accumulate: the counters are not cleared, so k_frame's statistics add up over consecutive frames (every counter of
+// k_frame is an atomic add except n_primary, which it sets).
+static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumulate = false, bool push = true)
 {
     int rc = require_ready(c); if (rc) return rc;
     if ((rc = join_shadow(c))) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
-    RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
+    if (!accumulate) RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
     const int threads = frame_kernel_threads(c);
     const FrameDyn dyn = frame_dyn(c);
     FrameParams fp = frame_params(c);
-    fp.gather = c->gather_slab;
+    fp.gather = push ? c->gather_slab : nullptr;
     rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
         auto* k = k_frame<smem.value>;
-        const int per_sm = std::min(resident_per_sm(c, (const void*)k, threads, sm), 32);
-        const uint32_t n_groups = (c->n_local + 31u) / 32u;
-        uint32_t grid = (uint32_t)(c->num_sms * per_sm / c->grid_div);
-        if (grid < (uint32_t)c->num_sms) grid = (uint32_t)c->num_sms;
-        if (grid > n_groups) grid = n_groups;
-        if (grid < 1) grid = 1;
-        const uint32_t slots_per_cta = ((n_groups + grid - 1u) / grid) * 32u;
-        if ((size_t)grid * slots_per_cta > c->n_alloc) RT_FAIL(c, RT_ERR_CUDA, "frame kernel: queue regions exceed the allocation");
+        uint32_t grid, slots_per_cta;
+        int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
         TimedLaunch t(c, RT_K_MISC);
         k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
         return RT_OK;
@@ -1566,19 +1600,39 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces)
     if (rc || (rc = post_launch(c, "k_frame"))) return rc;
     c->frame_started = true; c->cur_bounce = max_bounces;
     ++c->sample_count;
-    return gather_signal(c, false);
+    return RT_OK;
 }
 
-int rt_integrate(rt_ctx* c, uint32_t max_bounces)
+// n_samples (<= RT_MAX_REGEN_SAMPLES) frames as ONE launch of the regenerating frame kernel (k_frame_regen), with k_frame's CTA
+// shape and queue regions.  The statistics go to counters_sum; it pushes the fused gather's pixels itself.
+static int integrate_regen_kernel(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
 {
-    RT_CHECK_CTX(c); RT_FANOUT(c, rt_integrate(k, max_bounces));
-    if (max_bounces > RT_MAX_BOUNCES) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "max_bounces %u exceeds RT_MAX_BOUNCES", max_bounces);
-    if (frame_kernel_selected(c) && !c->kernel_timing && !c->count_traversal) return integrate_frame_kernel(c, max_bounces);
-    if (!c->use_graph || c->kernel_timing || c->count_traversal)
-    {
-        int rc = integrate_body(c, max_bounces); if (rc) return rc;
-        return gather_signal(c, true);
-    }
+    const int threads = frame_kernel_threads(c);
+    const FrameDyn dyn = frame_dyn(c);
+    FrameParams fp = frame_params(c);
+    fp.gather = c->gather_slab;
+    int rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
+        auto* k = k_frame_regen<smem.value>;
+        uint32_t grid, slots_per_cta;
+        int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
+        TimedLaunch t(c, RT_K_MISC);
+        k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters_sum, c->radiance, aov_params(c), max_bounces, n_samples,
+                                            slots_per_cta, dyn);
+        return RT_OK;
+    });
+    if (rc || (rc = post_launch(c, "k_frame_regen"))) return rc;
+    c->frame_started = true; c->cur_bounce = max_bounces;
+    c->sample_count += n_samples;
+    return RT_OK;
+}
+
+// One frame on the schedule rt_integrate selects, without the fused gather's completion signal.  *pushed: the frame kernel has
+// pushed every pixel to the gather target already (otherwise the radiance slab has to be copied).
+static int integrate_frame(rt_ctx* c, uint32_t max_bounces, bool* pushed)
+{
+    *pushed = false;
+    if (one_kernel_frame(c)) { *pushed = true; return integrate_frame_kernel(c, max_bounces); }
+    if (!c->use_graph || c->kernel_timing || c->count_traversal) return integrate_body(c, max_bounces);
     int rc = require_ready(c); if (rc) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
     if (!c->graph_exec || c->graph_gen != c->config_gen || c->graph_max_bounces != max_bounces)
@@ -1596,7 +1650,83 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
     c->launches += c->graph_launches;
     c->frame_started = true; c->cur_bounce = max_bounces;
     ++c->sample_count;
-    return gather_signal(c, true);
+    return RT_OK;
+}
+
+int rt_integrate(rt_ctx* c, uint32_t max_bounces)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_integrate(k, max_bounces));
+    if (max_bounces > RT_MAX_BOUNCES) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "max_bounces %u exceeds RT_MAX_BOUNCES", max_bounces);
+    c->stats_summed = false;
+    bool pushed = false;
+    int rc = integrate_frame(c, max_bounces, &pushed); if (rc) return rc;
+    return gather_signal(c, !pushed);
+}
+
+// Which schedule rt_integrate_samples runs: the regenerating kernel only where RT_OPT_FRAME_KERNEL = 1 forces the one-kernel frame.
+// Measured on one H100 80GB HBM3 at 700 W (tools/spp_probe.py, 1080p x 8, rank 0 of 1/2/4/8-way partitions, N = 8 and 64, DESIGN.md
+// section 4) it never clearly beats N one-kernel frames: it ties on CornellBox (-3 % to +4 %) and is 5-29 % slower on ShaderBalls,
+// so every partition size takes the N-frame path.
+static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c); }
+
+// A multi-sample call leaves its summed statistics in counters_sum, which only rt_read_frame_stats reads: the counters that the
+// taps (rt_read_rays, rt_read_hits) take their entry counts from never exceed one frame's rays.
+int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_integrate_samples(k, max_bounces, n_samples));
+    if (max_bounces > RT_MAX_BOUNCES) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "max_bounces %u exceeds RT_MAX_BOUNCES", max_bounces);
+    if (n_samples == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_integrate_samples: n_samples must be at least 1");
+    if (n_samples > 0xFFFFFFFFu - c->sample_count)
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_integrate_samples: the sample count %u + %u would wrap", c->sample_count, n_samples);
+    if (n_samples > 1 && c->denoiser)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_integrate_samples: the temporal denoiser runs once per sample; render one sample per call with it");
+    if (n_samples > RT_MAX_REGEN_SAMPLES && regen_selected(c))
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_integrate_samples: the regenerating frame kernel (RT_OPT_FRAME_KERNEL 1) renders at most %u samples per call",
+                RT_MAX_REGEN_SAMPLES);
+    if (n_samples == 1) return rt_integrate(c, max_bounces);
+    int rc = require_ready(c); if (rc) return rc;
+    if ((rc = join_shadow(c))) return rc;
+    RT_CUDA(c, cudaSetDevice(c->device));
+    if (!c->counters_sum) RT_CUDA(c, cudaMalloc(&c->counters_sum, sizeof(DevCounters)));
+    RT_CUDA(c, cudaMemsetAsync(c->counters_sum, 0, sizeof(DevCounters), c->stream));
+    c->stats_summed = false;
+    bool pushed = true;
+    if (regen_selected(c))
+    {   // the taps find no rays of this call
+        RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
+        if ((rc = integrate_regen_kernel(c, max_bounces, n_samples))) return rc;
+    }
+    else if (one_kernel_frame(c))
+    {   // n k_frame launches that add up their statistics in c->counters, folded into counters_sum once per batch (a batch stays
+        // small enough that no 32-bit half of the packed 64-bit counters can carry into the other); only the last frame pushes
+        // to the gather target
+        const uint32_t batch = 0xFFFFFFFFu / std::max(c->n_local, 1u);
+        for (uint32_t s = 0; s < n_samples; ++s)
+        {
+            if (s % batch == 0) RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
+            if ((rc = integrate_frame_kernel(c, max_bounces, true, s + 1 == n_samples))) return rc;
+            if ((s + 1) % batch == 0 || s + 1 == n_samples)
+            {
+                TimedLaunch t(c, RT_K_MISC);
+                k_add_counters<<<1, 256, 0, c->stream>>>(c->counters_sum, c->counters, s % batch + 1);
+                if ((rc = post_launch(c, "k_add_counters"))) return rc;
+            }
+        }
+        RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));   // the taps find no rays of this call
+    }
+    else
+    {   // n frames of the per-phase schedule: they clear the counters at the start of every frame (their queue cursors), so each
+        // frame's statistics are added into counters_sum after it; the counters keep the last frame's, as after rt_integrate
+        for (uint32_t s = 0; s < n_samples; ++s)
+        {
+            if ((rc = integrate_frame(c, max_bounces, &pushed))) return rc;
+            TimedLaunch t(c, RT_K_MISC);
+            k_add_counters<<<1, 256, 0, c->stream>>>(c->counters_sum, c->counters, 1u);
+            if ((rc = post_launch(c, "k_add_counters"))) return rc;
+        }
+    }
+    c->stats_summed = true;
+    return gather_signal(c, !pushed);
 }
 
 // the resolve kernel of this context's rows into `out`, on its stream
@@ -1850,7 +1980,7 @@ int rt_read_frame_stats(rt_ctx* c, RtFrameStats* out)
     RT_CUDA(c, cudaSetDevice(c->device));
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
     static thread_local DevCounters h;
-    RT_CUDA(c, cudaMemcpy(&h, c->counters, sizeof(DevCounters), cudaMemcpyDeviceToHost));
+    RT_CUDA(c, cudaMemcpy(&h, c->stats_summed ? c->counters_sum : c->counters, sizeof(DevCounters), cudaMemcpyDeviceToHost));
     memset(out, 0, sizeof(*out));
     for (uint32_t b = 0; b <= RT_MAX_BOUNCES; ++b)
     {

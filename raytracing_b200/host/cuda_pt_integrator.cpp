@@ -118,10 +118,20 @@ void CUDAPathTraceIntegrator::EnableDenoiser(bool enable)
 
 void CUDAPathTraceIntegrator::Reset() { Check(rt_reset(ctx_), "Reset"); }
 
+void CUDAPathTraceIntegrator::SetSamplesPerFrame(std::uint32_t n)
+{
+    if (n == 0) throw std::runtime_error("SetSamplesPerFrame: a frame renders at least one sample");
+    samples_per_frame_ = n;
+}
+
 // ---- the per-frame steps.  kFrame: Integrate() (integrator.cpp:27-59, not virtual) calls them in a fixed order; they are
 // checked against that order and the frame is submitted as a whole in AdvanceSampleCount().
 void CUDAPathTraceIntegrator::GenerateRays()
 {
+    if (samples_per_frame_ > 1 && schedule_ != Schedule::kFrame)
+        throw std::runtime_error("GenerateRays: several samples per frame (SetSamplesPerFrame) need the kFrame schedule");
+    if (samples_per_frame_ > 1 && enable_denoiser_)
+        throw std::runtime_error("GenerateRays: several samples per frame (SetSamplesPerFrame) are not available with the denoiser, which runs once per sample");
     if (schedule_ == Schedule::kFrame) { frame_deferred_ = true; deferred_shaded_ = deferred_accumulated_ = 0; return; }
     Check(rt_generate_rays(ctx_), "GenerateRays");
 }
@@ -130,6 +140,8 @@ void CUDAPathTraceIntegrator::FlushDeferredFrame()
 {
     if (!frame_deferred_) return;
     frame_deferred_ = false;
+    if (samples_per_frame_ > 1)
+        throw std::runtime_error("several samples per frame (SetSamplesPerFrame) need the call order of Integrate(); this frame's steps arrived in another order");
     Check(rt_generate_rays(ctx_), "GenerateRays");
     for (std::uint32_t b = 0; b < deferred_shaded_; ++b)
     {
@@ -145,7 +157,8 @@ void CUDAPathTraceIntegrator::AdvanceSampleCount()
         if (deferred_shaded_ == max_bounces_ + 1 && deferred_accumulated_ == max_bounces_ + 1)
         {   // the canonical frame: one call, rt_integrate advances the sample count itself
             frame_deferred_ = false;
-            Check(rt_integrate(ctx_, max_bounces_), "Integrate (whole frame)");
+            if (samples_per_frame_ > 1) Check(rt_integrate_samples(ctx_, max_bounces_, samples_per_frame_), "Integrate (whole frame, several samples)");
+            else Check(rt_integrate(ctx_, max_bounces_), "Integrate (whole frame)");
             return;
         }
         FlushDeferredFrame();

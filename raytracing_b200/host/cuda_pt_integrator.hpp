@@ -19,6 +19,10 @@
  *                     end of each loop iteration of Integrate() the device state is the same as with
  *                     the stepwise schedule, bit for bit.
  *   kStepwise         one kernel per virtual, like the OpenCL backend.
+ * SetSamplesPerFrame(n): Integrate() renders n progressive samples, the same bits as n calls with one sample each.  kFrame only:
+ * AdvanceSampleCount() submits them with ONE rt_integrate_samples call (n frames on the device without a host round trip, or
+ * one launch of the regenerating frame kernel with RT_OPT_FRAME_KERNEL 1).  With n > 1 the kFused / kStepwise schedules, a call order other than
+ * Integrate()'s and the denoiser (it runs once per sample) throw std::runtime_error.
  * AOVs (ComputeAOVs) are produced inside the bounce-0 shading pass, and only when SetAOV selected a view other than
  * the shaded colour or the denoiser is on.  SetSamplerType(kBlueNoise) needs the sampler's three tables first
  * (SetBlueNoiseTables; the OpenCL backend reads them from utils/blue_noise_sampler.hpp, cl_pt_integrator.cpp:222-235).
@@ -62,6 +66,9 @@ public:
     // the device->host copies are asynchronous (several devices then read back in parallel)
     void SetResolveTarget(float* host_rgba, bool page_lock = false);
     void SetSchedule(Schedule s) { schedule_ = s; }
+    // samples rendered by one Integrate() (default 1); n > 1 needs the kFrame schedule and no denoiser
+    void SetSamplesPerFrame(std::uint32_t n);
+    std::uint32_t SamplesPerFrame() const { return samples_per_frame_; }
     rt_ctx* Context() const { return ctx_; }
 
 protected:
@@ -89,6 +96,7 @@ private:
     rt_ctx* ctx_ = nullptr;
     Schedule schedule_;
     std::uint32_t current_bounce_ = 0;
+    std::uint32_t samples_per_frame_ = 1;
     float* resolve_target_ = nullptr;
     bool resolve_target_locked_ = false;
     // kFrame bookkeeping: a frame is "deferred" from GenerateRays() until AdvanceSampleCount()

@@ -178,6 +178,10 @@ int rth_render_set_max_bounces(void* h, std::uint32_t b)
 {
     try { ((RenderHandle*)h)->render->SetMaxBounces(b); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_samples_per_frame(void* h, std::uint32_t n)
+{
+    try { ((RenderHandle*)h)->render->SetSamplesPerFrame(n); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_enable_white_furnace(void* h, int e)
 {
     try { ((RenderHandle*)h)->render->GetIntegrator().EnableWhiteFurnace(e != 0); return 0; } catch (std::exception& ex) { g_error = ex.what(); return -1; }

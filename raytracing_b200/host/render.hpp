@@ -39,6 +39,8 @@ public:
     AccelerationStructure& GetAccelerationStructure() { return *acc_structure_; }
     std::vector<float> const& GetImage() const { return image_; }     // resolved RGBA32F, width*height
     void SetMaxBounces(std::uint32_t b) { integrator_->SetMaxBounces(b); }
+    // progressive samples accumulated by one RenderFrame() (CUDAPathTraceIntegrator::SetSamplesPerFrame), default 1
+    void SetSamplesPerFrame(std::uint32_t n) { static_cast<CUDAPathTraceIntegrator&>(*integrator_).SetSamplesPerFrame(n); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 
 private:

@@ -42,6 +42,7 @@ def load_library():
     L.rth_render_create.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_char_p, C.c_int, C.c_int]
     L.rth_render_free.argtypes = [C.c_void_p]
     L.rth_render_set_max_bounces.argtypes = [C.c_void_p, C.c_uint32]
+    L.rth_render_set_samples_per_frame.argtypes = [C.c_void_p, C.c_uint32]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler_tables.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -201,6 +202,11 @@ class HostRender:
 
     def set_max_bounces(self, b):
         if self.L.rth_render_set_max_bounces(self.h, b) != 0:
+            raise _err(self.L)
+
+    def set_samples_per_frame(self, n):
+        """Progressive samples accumulated by one render_frame() (Render::SetSamplesPerFrame); needs the "frame" schedule for n > 1."""
+        if self.L.rth_render_set_samples_per_frame(self.h, n) != 0:
             raise _err(self.L)
 
     def enable_white_furnace(self, e):
