@@ -251,6 +251,35 @@ int rt_integrate(rt_ctx* ctx, uint32_t max_bounces);
  * temporal denoiser on (it runs once per sample).  Multi-device contexts fan out like rt_integrate. */
 int rt_integrate_samples(rt_ctx* ctx, uint32_t max_bounces, uint32_t n_samples);
 
+/* ---- adaptive sampling (new capability) ----------------------------------------------------------------------------------
+ * Stop tracing pixels whose image has settled.  While it is on, a frame traces primary rays only for the ACTIVE local pixels; a
+ * path is otherwise unchanged (its sample index is still the context's sample count), so a pixel that stops after n samples holds
+ * exactly the radiance and AOVs that n frames give it.  After every sample (rt_advance_sample_count, every frame of rt_integrate
+ * and rt_integrate_samples) each active pixel, now at n samples, updates its estimate of the standard error of its resolved
+ * (Reinhard) luminance and stops when
+ *     Y = luma(radiance) = (x * 0.299f + y * 0.587f) + z * 0.114f (float), then in double:
+ *     y = Y - Y_prev;  Q += y * y;  Y_prev = Y;  m = Y / n;  v = max(Q / n - m * m, 0);  e = sqrt(v / n) / ((1 + m) * (1 + m))
+ *     stop iff n >= min_samples and e <= max_error                         (NaN never stops)
+ * max_error is in display units (0.002 is about half an 8-bit step).  A stopped pixel keeps its sample count, radiance and AOVs and
+ * stays stopped until the next rt_reset.  After an rt_reset, an active pixel's sample count always equals rt_read_sample_count.
+ *
+ * max_error > 0 (finite) and min_samples >= 2 turn it on; max_error == 0 turns it off (min_samples is ignored); anything else is
+ * RT_ERR_INVALID_ARGUMENT.  The setting takes effect at the next rt_reset (like the Integrator's SetMaxBounces -> RequestReset);
+ * until then the previous one stays.  rt_reset with it on makes every local pixel active with a sample count of 0; so does
+ * rt_set_partition, which clears the radiance but not the context's sample count (the sample index continues; call rt_reset to
+ * start over, after which every active pixel's count equals the sample count again).  The per-pixel state (about 20 bytes per pixel) exists only while it is on.
+ * With it on: rt_resolve / rt_resolve_async divide the shaded colour by each pixel's own sample count (the AOV views are
+ * unchanged); n_ext[0] of rt_read_frame_stats counts the pixels active at the start of the frame; rt_integrate_samples always
+ * runs n frames of rt_integrate's schedule (never the regenerating kernel).  Multi-device contexts fan out: every device decides
+ * for its own rows, with the same result as one device.
+ * RT_ERR_UNSUPPORTED, whichever of the two calls comes second: the temporal denoiser, a fused-gather target
+ * (rt_set_gather_target), RT_OPT_PRESENT 1 on a multi-device context, and rt_resolve_gathered[_async]. */
+int rt_set_adaptive_sampling(rt_ctx* ctx, float max_error, uint32_t min_samples);
+/* Every local pixel's sample count as a full width*height uint32 image (rows of other ranks untouched).  Off: sample_count everywhere. */
+int rt_read_pixel_samples(rt_ctx* ctx, uint32_t* counts);
+/* Pixels that will trace the next sample (blocking; summed over the devices of a multi-device context).  Off: the local pixel count. */
+int rt_read_active_pixels(rt_ctx* ctx, uint32_t* n_active);
+
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);
 /* Hits of the rays currently in the incoming queue of `bounce` after rt_intersect(bounce): n = live rays;

@@ -32,7 +32,8 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_read_sample_count", "rt_read_aovs", "rt_kernel_times", "rt_launch_count", "rt_local_pixel_count",
            "rt_radiance_device_ptr", "rt_stream_handle",
            "rt_create_multi", "rt_device_count", "rt_gather_radiance", "rt_host_register", "rt_host_unregister", "rt_math_eval",
-           "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait"]
+           "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
+           "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels"]
 
 
 class RtSceneDesc(C.Structure):
@@ -111,6 +112,9 @@ def load_library():
     L.rt_ipc_open.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
     L.rt_set_gather_target.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     L.rt_gather_wait.argtypes = [C.c_void_p]
+    L.rt_set_adaptive_sampling.argtypes = [C.c_void_p, C.c_float, C.c_uint32]
+    L.rt_read_pixel_samples.argtypes = [C.c_void_p, C.c_void_p]
+    L.rt_read_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     _lib = L
     return L
 
@@ -237,6 +241,24 @@ class Context:
         self._ck(self.lib.rt_integrate_samples(self.h, max_bounces, n_samples))
 
     def sync(self): self._ck(self.lib.rt_sync(self.h))
+
+    # ---- adaptive sampling
+    def set_adaptive_sampling(self, max_error, min_samples=2):
+        """Stop tracing pixels whose resolved luminance has a standard error <= max_error after >= min_samples samples
+        (rt_set_adaptive_sampling); max_error 0 turns it off.  Takes effect at the next reset()."""
+        self._ck(self.lib.rt_set_adaptive_sampling(self.h, float(max_error), int(min_samples)))
+
+    def pixel_samples(self):
+        """-> (h, w) uint32: every local pixel's sample count (rows of other ranks left zero)."""
+        out = np.zeros((self.height, self.width), dtype="<u4")
+        self._ck(self.lib.rt_read_pixel_samples(self.h, out.ctypes.data))
+        return out
+
+    def active_pixels(self):
+        """Pixels that will trace the next sample (all local pixels when adaptive sampling is off)."""
+        n = C.c_uint32()
+        self._ck(self.lib.rt_read_active_pixels(self.h, C.byref(n)))
+        return n.value
 
     def integrate_stepwise(self, max_bounces):
         """The schedule of Integrator::Integrate (integrator.cpp:35-51), one call per reference virtual."""

@@ -26,6 +26,7 @@ struct CtaFrame
     unsigned long long emit[2];              // shadow rays (low word) and continuation rays (high word) spawned by S(b): slot reservation
     uint32_t n_emissive, n_unoccluded;
     uint32_t ended_n[2];                     // fused gather: pixels whose path ended at a hit in S(b) (no continuation), parity b & 1
+    uint32_t n_src;                          // entries of the primary-ray source: local pixels, or active pixels (adaptive sampling)
 };
 
 template <int SMEM>
@@ -43,13 +44,17 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
     // (queue pointers are re-read from the kernel parameters where they are used: nothing but `base` stays live across the
     // traversal and shading loops)
     if (threadIdx.x == 0)
-    {
-        const uint32_t n_groups = (p.n_local + 31u) / 32u;
+    {   // groups of 32 consecutive entries of the primary-ray source (local pixels, or the ascending active list) are dealt
+        // round-robin; with adaptive sampling the grid stays sized by the partition and the active count is read here
+        const uint32_t n_src = p.active ? *p.n_active : p.n_local;
+        const uint32_t n_groups = (n_src + 31u) / 32u;
         const uint32_t cta = blockIdx.x, n_cta = gridDim.x;
         const uint32_t my_groups = cta < n_groups ? (n_groups - cta + n_cta - 1u) / n_cta : 0u;
         s.cur_trace = 0; s.cur_shade = 0; s.ext_n[0] = my_groups * 32u; s.ext_n[1] = 0; s.shadow_n[0] = s.shadow_n[1] = 0;
         s.hm[0] = s.hm[1] = 0ull; s.emit[0] = s.emit[1] = 0ull; s.n_emissive = 0; s.n_unoccluded = 0; s.ended_n[0] = s.ended_n[1] = 0;
-        if (blockIdx.x == 0) ctr->n_primary = p.n_local;
+        s.n_src = n_src;
+        // n_primary adds up over the frames of a multi-sample call (the counters are not cleared between them) once it varies
+        if (blockIdx.x == 0) ctr->n_primary = p.active ? ctr->n_primary + n_src : p.n_local;
     }
     __syncthreads();
     uint32_t nv = 0, nt = 0;     // (not counted here: RT_OPT_COUNT_TRAVERSAL uses the per-phase kernels)
@@ -75,10 +80,10 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                     bool live = i < n_ext;
                     float4 a, bb;
                     if (b == 0)
-                    {   // primary rays generated in the first traversal pass; slot i <-> local pixel li
-                        const uint32_t li = (blockIdx.x + (i >> 5) * gridDim.x) * 32u + (uint32_t)lane;
-                        live = li < p.n_local;
-                        if (live) primary_ray(p, q, aov, 0, base + i, li, p.dyn->sample_idx, 0u, a, bb);
+                    {   // primary rays generated in the first traversal pass; slot i <-> source entry j: local pixel j, or active[j]
+                        const uint32_t j = (blockIdx.x + (i >> 5) * gridDim.x) * 32u + (uint32_t)lane;
+                        live = j < s.n_src;
+                        if (live) primary_ray(p, q, aov, 0, base + i, p.active ? p.active[j] : j, p.dyn->sample_idx, 0u, a, bb);
                     }
                     else if (live) { a = q.A[in][base + i]; bb = q.B[in][base + i]; }
                     closest_group<false, SMEM, true>(sc, mode, s_bvh, q, base, i, live, a, bb, &s.hm[in], nv, nt);

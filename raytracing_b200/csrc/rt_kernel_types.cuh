@@ -52,6 +52,20 @@ struct FrameParams
     const FrameDyn* dyn;
     float4* gather;                // k_frame only: this rank's slab of the gathered radiance on the presenting device (peer memory,
                                    // rt_set_gather_target) — a pixel's radiance is pushed there the moment its path ends; else nullptr
+    // adaptive sampling (rt_set_adaptive_sampling), else nullptr: primary rays are traced for the local pixels active[0 .. *n_active)
+    // (ascending) instead of every local pixel
+    const uint32_t* active;
+    const uint32_t* n_active;
+};
+
+// Adaptive sampling, device-resident control block of k_adaptive_update (one per context while the feature is on)
+struct AdaptiveCtl
+{
+    uint32_t n_active;             // entries of the active list: pixels that trace the next sample
+    uint32_t n_next;               // the compaction's new count, moved to n_active by the update's last CTA
+    uint32_t frames;               // samples since rt_reset = the sample count of every active pixel
+    uint32_t ticket, done;         // the update's CTA order (decoupled look-back) and completion count, back to 0 after every update
+    uint32_t epoch;                // tags the update's tile states: 1 .. 2^30 - 1, advanced by every update
 };
 
 // AOV outputs of bounce 0 (kernels/cl/aov.cl:44-110), written by the bounce-0 shading pass when enabled

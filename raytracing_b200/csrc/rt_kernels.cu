@@ -29,6 +29,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -289,14 +290,16 @@ __global__ void __launch_bounds__(256) k_reset(float4* radiance, uint32_t n)
     if (i < n) radiance[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 }
 
-// One thread per LOCAL pixel; slot i of queue 0 = local pixel i.
+// One thread per LOCAL pixel; slot i of queue 0 = local pixel i, or with adaptive sampling the i-th active pixel (the grid stays
+// sized by the partition, so that a captured frame graph serves every frame).
 __global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCounters* ctr, AovParams aov)
 {
-    uint32_t li = blockIdx.x * blockDim.x + threadIdx.x;
-    if (li == 0) ctr->n_primary = p.n_local;
-    if (li >= p.n_local) return;
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t n = p.active ? *p.n_active : p.n_local;
+    if (i == 0) ctr->n_primary = n;
+    if (i >= n) return;
     float4 a, b;
-    primary_ray(p, q, aov, 0, li, li, p.dyn->sample_idx, 0u, a, b);
+    primary_ray(p, q, aov, 0, i, p.active ? p.active[i] : i, p.dyn->sample_idx, 0u, a, b);
 }
 
 // IntersectRays (stepwise): closest hit of every live ray of bounce b -> hits[]
@@ -475,9 +478,9 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
 
 
 // resolve_radiance.cl:31-86: shaded colour (radiance / sample_count unless the denoiser is on, then Reinhard x/(1+x))
-// or one of the AOV views
+// or one of the AOV views.  counts (adaptive sampling, else nullptr): the shaded colour divides by the pixel's own sample count.
 __global__ void __launch_bounds__(256) k_resolve(const float4* radiance, float4* out, uint32_t n, uint32_t sample_count, int denoiser,
-                                                 int aov_index, AovParams aov)
+                                                 int aov_index, AovParams aov, const uint32_t* counts)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -489,9 +492,144 @@ __global__ void __launch_bounds__(256) k_resolve(const float4* radiance, float4*
     {
         float4 r = radiance[i];
         f3 hdr = mk3(r);
-        if (!denoiser) hdr = hdr / (float)sample_count;
+        if (!denoiser) hdr = hdr / (float)(counts ? counts[i] : sample_count);
         f3 ldr = hdr / (mk3(hdr.x + 1.0f, hdr.y + 1.0f, hdr.z + 1.0f));
         out[i] = make_float4(ldr.x, ldr.y, ldr.z, 1.0f);
+    }
+}
+
+// ---- adaptive sampling (rt_set_adaptive_sampling) ----------------------------------------------------------------
+struct AdaptiveState
+{
+    uint32_t* count;               // per local pixel: samples taken
+    float* y_prev;                 // per local pixel: luma of the radiance sum at the previous update
+    double* q;                     // per local pixel: sum of the squared per-sample luma increments
+    uint32_t* list;                // the active local pixels, ascending (n_local entries)
+    unsigned long long* tile;      // per tile of the update: (epoch << 2 | flag) << 32 | value, flag 1 aggregate, 2 inclusive prefix
+    AdaptiveCtl* ctl;
+};
+
+#define RT_AD_THREADS 256
+#define RT_AD_ITEMS 4
+#define RT_AD_TILE (RT_AD_THREADS * RT_AD_ITEMS)
+
+// rt_reset with the feature on: every local pixel active, in order; the per-pixel state is cleared by memsets beside this launch
+__global__ void __launch_bounds__(256) k_adaptive_init(AdaptiveState st, uint32_t n_local)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_local) st.list[i] = i;
+    if (i == 0) { st.ctl->n_active = n_local; st.ctl->n_next = 0; st.ctl->frames = 0; st.ctl->ticket = 0; st.ctl->done = 0; st.ctl->epoch = 1; }
+}
+
+// The convergence update after a sample: for every active pixel (now at n = frames + 1 samples) update the luma statistics and
+// decide whether it stops (DESIGN.md section 4):
+//     Y = luma(radiance), y = Y - Y_prev, Q += y^2, m = Y / n, v = max(Q / n - m^2, 0), e = sqrt(v / n) / (1 + m)^2,
+//     stop iff n >= min_samples and e <= max_error            (double precision; NaN never stops)
+// and compact the survivors into the same list, in place and ascending, in one pass.  Tile t = RT_AD_TILE consecutive list entries,
+// taken in CTA arrival order (a ticket), so that the decoupled look-back over the tiles before t only waits on CTAs that are running.
+// In place is safe: a tile publishes its count only after it has read its entries, and a survivor moves to an index no larger than
+// its own.  The grid is sized by the partition (a captured frame graph replays it unchanged); tiles past the active count only take
+// part in the completion count, whose last CTA moves the new count into n_active, advances frames and the epoch and re-arms the
+// ticket (every CTA has read them by then).
+__global__ void __launch_bounds__(RT_AD_THREADS) k_adaptive_update(const float4* radiance, AdaptiveState st, double max_error, uint32_t min_samples)
+{
+    __shared__ uint32_t s_t, s_n, s_frames, s_epoch, s_prefix;
+    __shared__ uint32_t s_warp[RT_AD_THREADS / 32];
+    if (threadIdx.x == 0)
+    {
+        volatile AdaptiveCtl* ctl = st.ctl;
+        s_n = ctl->n_active; s_frames = ctl->frames; s_epoch = ctl->epoch;
+        s_t = atomicAdd(&st.ctl->ticket, 1u);
+    }
+    __syncthreads();
+    const uint32_t t = s_t, n_act = s_n;
+    if ((size_t)t * RT_AD_TILE < n_act)
+    {
+        const uint32_t n = s_frames + 1u;
+        const double dn = (double)n;
+        const uint32_t first = t * RT_AD_TILE + threadIdx.x * RT_AD_ITEMS;
+        uint32_t li[RT_AD_ITEMS];
+        unsigned keep = 0u;
+#pragma unroll
+        for (int k = 0; k < RT_AD_ITEMS; ++k)
+        {
+            const uint32_t j = first + k;
+            li[k] = 0;
+            if (j >= n_act) continue;
+            const uint32_t pix = st.list[j];
+            li[k] = pix;
+            const float Y = luma(mk3(radiance[pix]));
+            const double y = (double)Y - (double)st.y_prev[pix];
+            const double Q = st.q[pix] + y * y;
+            st.q[pix] = Q; st.y_prev[pix] = Y; st.count[pix] = n;
+            const double m = (double)Y / dn;
+            double v = Q / dn - m * m;
+            if (v < 0.0) v = 0.0;
+            const double d = 1.0 + m;
+            const double e = sqrt(v / dn) / (d * d);
+            if (!(n >= min_samples && e <= max_error)) keep |= 1u << k;
+        }
+        // block-wide exclusive scan of the survivors, in list order
+        const uint32_t mine = (uint32_t)__popc(keep);
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        uint32_t incl = mine;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0)
+        {
+            uint32_t agg = 0;
+            if (lane == 0)
+                for (int w = 0; w < RT_AD_THREADS / 32; ++w) { const uint32_t c = s_warp[w]; s_warp[w] = agg; agg += c; }
+            agg = __shfl_sync(0xffffffffu, agg, 0);
+            // decoupled look-back: publish the aggregate, then add up the tiles before this one, 32 at a time (lane k looks at tile
+            // end - k), back to the nearest inclusive prefix
+            const unsigned long long tag = (unsigned long long)(s_epoch << 2);
+            volatile unsigned long long* tile = st.tile;
+            if (lane == 0) tile[t] = ((tag | (t == 0 ? 2ull : 1ull)) << 32) | agg;
+            uint32_t prefix = 0;
+            for (int32_t end = (int32_t)t - 1; end >= 0; end -= 32)
+            {
+                const int32_t u = end - lane;
+                unsigned long long w, flag;
+                do
+                {   // tiles before the first are an inclusive prefix of 0
+                    w = 0ull; flag = 2ull;
+                    if (u >= 0) { w = tile[u]; const unsigned long long wt = w >> 32; flag = (wt & ~3ull) == tag ? (wt & 3ull) : 0ull; }
+                } while (__any_sync(0xffffffffu, flag == 0ull));                  // a tile has not published for this update yet
+                const unsigned inc = __ballot_sync(0xffffffffu, flag == 2ull);
+                const int last = inc ? __ffs(inc) - 1 : 31;
+                uint32_t v = lane <= last ? (uint32_t)w : 0u;
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+                prefix += v;
+                if (inc) break;
+            }
+            if (lane == 0)
+            {
+                if (t > 0) tile[t] = ((tag | 2ull) << 32) | (prefix + agg);
+                s_prefix = prefix;
+                if ((size_t)(t + 1u) * RT_AD_TILE >= n_act) { st.ctl->n_next = prefix + agg; __threadfence(); }   // the last active tile
+            }
+        }
+        __syncthreads();
+        uint32_t at = s_prefix + s_warp[warp] + incl - mine;
+#pragma unroll
+        for (int k = 0; k < RT_AD_ITEMS; ++k)
+            if (keep & (1u << k)) st.list[at++] = li[k];
+    }
+    if (threadIdx.x == 0)
+    {
+        __threadfence();
+        if (atomicAdd(&st.ctl->done, 1u) == gridDim.x - 1u)
+        {   // every CTA has finished: the next update and the next frame see the new state
+            volatile AdaptiveCtl* ctl = st.ctl;
+            ctl->n_active = n_act ? ctl->n_next : 0u;
+            ctl->frames = s_frames + 1u;
+            ctl->epoch = s_epoch % 0x3FFFFFFFu + 1u;
+            ctl->ticket = 0; ctl->done = 0;
+        }
     }
 }
 
@@ -573,7 +711,8 @@ __global__ void k_math_eval(int fn, const float* a, const float* b, float* out, 
 }
 
 // rt_integrate_samples on the per-frame path: the statistics of `frames` frames (added up in f by k_frame, or one per-phase frame)
-// added into the call's sums (one CTA).  Every frame has f->n_primary primary rays.
+// added into the call's sums (one CTA).  Every frame has f->n_primary primary rays (with adaptive sampling k_frame adds them up
+// itself and frames is 1).
 __global__ void __launch_bounds__(256) k_add_counters(DevCounters* sum, const DevCounters* f, uint32_t frames)
 {
     for (uint32_t b = threadIdx.x; b <= RT_MAX_BOUNCES; b += blockDim.x)
@@ -677,6 +816,12 @@ struct rt_ctx
     std::vector<void*> scene_allocs;
     RtCamera camera = {};
     RayGenConsts raygen = {};
+
+    // adaptive sampling (rt_set_adaptive_sampling): the requested setting, which rt_reset makes the active one; max_error > 0 = on.
+    // The per-pixel state exists only while the active setting is on.
+    float ad_req_error = 0.0f; uint32_t ad_req_min = 0;
+    float ad_error = 0.0f; uint32_t ad_min = 0;
+    AdaptiveState ad = {};
 
     uint32_t sample_count = 0;
     uint32_t cur_bounce = 0;
@@ -783,12 +928,16 @@ int post_launch(rt_ctx* c, const char* what)
     return RT_OK;
 }
 
+bool adaptive_on(const rt_ctx* c);
+
 FrameParams frame_params(const rt_ctx* c)
 {
     FrameParams p;
     p.width = c->width; p.height = c->height; p.rank = c->rank; p.world = c->world; p.n_local = c->n_local;
     p.white_furnace = c->white_furnace; p.bn = c->sampler ? c->d_bn : nullptr; p.dyn = c->d_dyn;
     p.gather = nullptr;            // set by the one-kernel frame's launch only
+    p.active = adaptive_on(c) ? c->ad.list : nullptr;
+    p.n_active = adaptive_on(c) ? &c->ad.ctl->n_active : nullptr;
     return p;
 }
 
@@ -812,6 +961,58 @@ void free_frame_buffers(rt_ctx* c)
     freep(c->q.hitq); freep(c->q.missq);
     freep(c->radiance); freep(c->resolved); freep(c->resolved2);
     free_aov_buffers(c);
+    freep(c->ad.count); freep(c->ad.y_prev); freep(c->ad.q); freep(c->ad.list); freep(c->ad.tile); freep(c->ad.ctl);
+}
+
+// ---- adaptive sampling: the active setting is on / either setting is on (what the refused combinations check)
+bool adaptive_on(const rt_ctx* c) { return c->ad_error > 0.0f; }
+bool adaptive_wanted(const rt_ctx* c) { return c->ad_error > 0.0f || c->ad_req_error > 0.0f; }
+uint32_t adaptive_tiles(const rt_ctx* c) { return std::max((c->n_local + RT_AD_TILE - 1u) / RT_AD_TILE, 1u); }
+
+// The per-pixel state for the current partition (allocated on first use) reset to: every local pixel active, counts and
+// estimators zero.
+void free_adaptive(rt_ctx* c);
+
+int reset_adaptive(rt_ctx* c)
+{
+    const size_t n = std::max(c->n_local, 1u), tiles = adaptive_tiles(c);
+    // each buffer on its own: after a failed allocation the next call allocates only what is missing (free_adaptive frees all)
+    auto alloc = [&](auto*& ptr, size_t bytes) -> int {
+        if (ptr) return RT_OK;
+        ++c->config_gen;
+        RT_CUDA(c, cudaMalloc(&ptr, bytes));
+        return RT_OK;
+    };
+    int rc;
+    if ((rc = alloc(c->ad.count, n * 4)) || (rc = alloc(c->ad.y_prev, n * 4)) || (rc = alloc(c->ad.q, n * 8)) || (rc = alloc(c->ad.list, n * 4)) ||
+        (rc = alloc(c->ad.tile, tiles * 8)) || (rc = alloc(c->ad.ctl, sizeof(AdaptiveCtl))))
+    {   // the frames run with the feature off until a later rt_reset succeeds (the requested setting stays)
+        free_adaptive(c);
+        c->ad_error = 0.0f; c->ad_min = 0;
+        return rc;
+    }
+    RT_CUDA(c, cudaMemsetAsync(c->ad.count, 0, n * 4, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->ad.y_prev, 0, n * 4, c->stream));
+    RT_CUDA(c, cudaMemsetAsync(c->ad.q, 0, n * 8, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->ad.tile, 0, tiles * 8, c->stream));
+    TimedLaunch t(c, RT_K_MISC);
+    k_adaptive_init<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->ad, c->n_local);
+    return post_launch(c, "k_adaptive_init");
+}
+
+void free_adaptive(rt_ctx* c)
+{
+    if (!c->ad.count && !c->ad.y_prev && !c->ad.q && !c->ad.list && !c->ad.tile && !c->ad.ctl) return;
+    if (c->stream) cudaStreamSynchronize(c->stream);
+    cudaFree(c->ad.count); cudaFree(c->ad.y_prev); cudaFree(c->ad.q); cudaFree(c->ad.list); cudaFree(c->ad.tile); cudaFree(c->ad.ctl);
+    c->ad = AdaptiveState{};
+    ++c->config_gen;
+}
+
+// the convergence update that closes a sample (rt_advance_sample_count, after k_frame, and a node of the per-phase frame graph)
+int launch_adaptive_update(rt_ctx* c)
+{
+    TimedLaunch t(c, RT_K_MISC);
+    k_adaptive_update<<<adaptive_tiles(c), RT_AD_THREADS, 0, c->stream>>>(c->radiance, c->ad, (double)c->ad_error, c->ad_min);
+    return post_launch(c, "k_adaptive_update");
 }
 
 int alloc_frame_buffers(rt_ctx* c)
@@ -837,6 +1038,7 @@ int alloc_frame_buffers(rt_ctx* c)
     RT_CUDA(c, cudaMalloc(&c->radiance, n * 16)); RT_CUDA(c, cudaMalloc(&c->resolved, n * 16));
     RT_CUDA(c, cudaMemsetAsync(c->radiance, 0, n * 16, c->stream));
     c->copy_pending[0] = c->copy_pending[1] = false;          // both streams were drained above
+    if (adaptive_on(c)) { int rc = reset_adaptive(c); if (rc) return rc; }   // every pixel of the new partition active again
     if (aov_wanted(c)) return ensure_aov_buffers(c);           // a selected view / the denoiser keeps its buffers across a re-partition
     return RT_OK;
 }
@@ -1171,6 +1373,10 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
     if (key == RT_OPT_PRESENT)
     {
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "present mode must be 0 (parallel read-back) or 1 (gather to the first device)");
+        if (value == 1)
+            for (rt_ctx* k : c->children)
+                if (adaptive_wanted(k))
+                    RT_FAIL(c, RT_ERR_UNSUPPORTED, "RT_OPT_PRESENT 1 is not available with adaptive sampling (the gathered resolve has no per-pixel sample counts)");
         c->present = (int)value;
         if (!c->children.empty())
         {   // gather presentation: the children push their pixels into a buffer on the first device while they render (fused gather)
@@ -1199,6 +1405,8 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
     case RT_OPT_DENOISER:
         if (value != 0 && c->world != 1)
             RT_FAIL(c, RT_ERR_UNSUPPORTED, "the temporal denoiser reprojects across the whole image and is not available with a multi-GPU partition");
+        if (value != 0 && adaptive_wanted(c))
+            RT_FAIL(c, RT_ERR_UNSUPPORTED, "the temporal denoiser is not available with adaptive sampling (it replaces the radiance every frame)");
         c->denoiser = value != 0;
         if (aov_wanted(c)) { RT_CUDA(c, cudaSetDevice(c->device)); return ensure_aov_buffers(c); }
         return RT_OK;
@@ -1259,6 +1467,12 @@ int rt_reset(rt_ctx* c)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     RT_CUDA(c, cudaSetDevice(c->device));
     if (!c->denoiser) c->sample_count = 0;                                   // cl_pt_integrator.cpp:499-504
+    {   // the adaptive-sampling setting takes effect here; a changed setting changes the frame's launch arguments
+        if (c->ad_error != c->ad_req_error || c->ad_min != c->ad_req_min) ++c->config_gen;
+        c->ad_error = c->ad_req_error; c->ad_min = c->ad_req_min;
+        int rc = adaptive_on(c) ? reset_adaptive(c) : (free_adaptive(c), RT_OK);
+        if (rc) return rc;
+    }
     TimedLaunch t(c, RT_K_MISC);
     k_reset<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, c->n_local);
     return post_launch(c, "k_reset");
@@ -1268,7 +1482,67 @@ int rt_advance_sample_count(rt_ctx* c)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_advance_sample_count(k));
     int rc = join_shadow(c); if (rc) return rc;     // end of the bounce loop: everything of this frame is ordered on the render stream
+    if (adaptive_on(c))
+    {
+        RT_CUDA(c, cudaSetDevice(c->device));
+        if ((rc = launch_adaptive_update(c))) return rc;
+    }
     ++c->sample_count;
+    return RT_OK;
+}
+
+int rt_set_adaptive_sampling(rt_ctx* c, float max_error, uint32_t min_samples)
+{
+    RT_CHECK_CTX(c);
+    const bool on = max_error > 0.0f;
+    if (!(max_error == 0.0f || (on && std::isfinite(max_error) && min_samples >= 2)))
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_adaptive_sampling: need max_error == 0 (off), or a finite max_error > 0 and min_samples >= 2");
+    if (on && c->denoiser)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "adaptive sampling is not available with the temporal denoiser (it replaces the radiance every frame)");
+    if (on && !c->children.empty() && c->present == 1)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "adaptive sampling is not available with RT_OPT_PRESENT 1 (the gathered resolve has no per-pixel sample counts)");
+    if (on && c->gather_slab)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "adaptive sampling is not available with a fused-gather target (stopped pixels are never pushed)");
+    RT_FANOUT(c, rt_set_adaptive_sampling(k, max_error, min_samples));
+    c->ad_req_error = on ? max_error : 0.0f; c->ad_req_min = on ? min_samples : 0u;
+    return RT_OK;
+}
+
+int rt_read_pixel_samples(rt_ctx* c, uint32_t* counts)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_read_pixel_samples(k, counts));
+    { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
+    if (!counts) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_pixel_samples: null destination");
+    if (!adaptive_on(c))
+    {
+        for (uint32_t r = 0; r < c->local_rows; ++r)
+            std::fill_n(counts + ((size_t)c->rank + (size_t)r * c->world) * c->width, c->width, c->sample_count);
+        return RT_OK;
+    }
+    RT_CUDA(c, cudaSetDevice(c->device));
+    if (c->local_rows)
+        RT_CUDA(c, cudaMemcpy2DAsync(counts + (size_t)c->rank * c->width, (size_t)c->world * c->width * 4, c->ad.count,
+                                     (size_t)c->width * 4, (size_t)c->width * 4, c->local_rows, cudaMemcpyDeviceToHost, c->stream));
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+int rt_read_active_pixels(rt_ctx* c, uint32_t* n_active)
+{
+    RT_CHECK_CTX(c);
+    if (!n_active) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_active_pixels: null destination");
+    if (!c->children.empty())
+    {
+        uint32_t sum = 0, part = 0;
+        for (rt_ctx* k : c->children) { int rc = rt_read_active_pixels(k, &part); if (rc) { c->error = k->error; return rc; } sum += part; }
+        *n_active = sum;
+        return RT_OK;
+    }
+    { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
+    if (!adaptive_on(c)) { *n_active = c->n_local; return RT_OK; }
+    RT_CUDA(c, cudaSetDevice(c->device));
+    RT_CUDA(c, cudaMemcpyAsync(n_active, &c->ad.ctl->n_active, 4, cudaMemcpyDeviceToHost, c->stream));
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
     return RT_OK;
 }
 
@@ -1578,7 +1852,8 @@ static bool one_kernel_frame(const rt_ctx* c) { return frame_kernel_selected(c) 
 
 // The whole frame as ONE persistent kernel (k_frame): a counter clear and a launch.  It pushes the fused gather's pixels itself
 // when `push`.  accumulate: the counters are not cleared, so k_frame's statistics add up over consecutive frames (every counter of
-// k_frame is an atomic add except n_primary, which it sets).
+// k_frame is an atomic add except n_primary, which it sets, or adds to with adaptive sampling).  With adaptive sampling the
+// convergence update follows the frame.
 static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumulate = false, bool push = true)
 {
     int rc = require_ready(c); if (rc) return rc;
@@ -1598,6 +1873,7 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
         return RT_OK;
     });
     if (rc || (rc = post_launch(c, "k_frame"))) return rc;
+    if (adaptive_on(c) && (rc = launch_adaptive_update(c))) return rc;
     c->frame_started = true; c->cur_bounce = max_bounces;
     ++c->sample_count;
     return RT_OK;
@@ -1666,8 +1942,8 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
 // Which schedule rt_integrate_samples runs: the regenerating kernel only where RT_OPT_FRAME_KERNEL = 1 forces the one-kernel frame.
 // Measured on one H100 80GB HBM3 at 700 W (tools/spp_probe.py, 1080p x 8, rank 0 of 1/2/4/8-way partitions, N = 8 and 64, DESIGN.md
 // section 4) it never clearly beats N one-kernel frames: it ties on CornellBox (-3 % to +4 %) and is 5-29 % slower on ShaderBalls,
-// so every partition size takes the N-frame path.
-static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c); }
+// so every partition size takes the N-frame path.  Adaptive sampling decides between samples, so it always takes the N-frame path.
+static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c) && !adaptive_on(c); }
 
 // A multi-sample call leaves its summed statistics in counters_sum, which only rt_read_frame_stats reads: the counters that the
 // taps (rt_read_rays, rt_read_hits) take their entry counts from never exceed one frame's rays.
@@ -1706,9 +1982,9 @@ int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
             if (s % batch == 0) RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
             if ((rc = integrate_frame_kernel(c, max_bounces, true, s + 1 == n_samples))) return rc;
             if ((s + 1) % batch == 0 || s + 1 == n_samples)
-            {
+            {   // with adaptive sampling k_frame adds up n_primary itself (it varies from frame to frame)
                 TimedLaunch t(c, RT_K_MISC);
-                k_add_counters<<<1, 256, 0, c->stream>>>(c->counters_sum, c->counters, s % batch + 1);
+                k_add_counters<<<1, 256, 0, c->stream>>>(c->counters_sum, c->counters, adaptive_on(c) ? 1u : s % batch + 1);
                 if ((rc = post_launch(c, "k_add_counters"))) return rc;
             }
         }
@@ -1734,7 +2010,8 @@ static int launch_resolve(rt_ctx* c, float4* out)
 {
     TimedLaunch t(c, RT_K_RESOLVE);
     const AovParams ap = aov_params(c);
-    k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, out, c->n_local, c->sample_count, c->denoiser, ap.enabled ? c->aov : 0, ap);
+    k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, out, c->n_local, c->sample_count, c->denoiser, ap.enabled ? c->aov : 0, ap,
+                                                           adaptive_on(c) ? c->ad.count : nullptr);
     return post_launch(c, "k_resolve");
 }
 
@@ -1838,6 +2115,7 @@ static int resolve_gathered_impl(rt_ctx* c, const void* slabs, uint64_t stride_b
     if (stride_bytes % 16 != 0 || stride_bytes < rows_max * c->width * 16)
         RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_resolve_gathered: slab stride must be a multiple of 16 and hold %zu rows", rows_max);
     if (c->aov != 0 || c->denoiser) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_resolve_gathered resolves the shaded colour only (AOV views and the denoiser are single-GPU)");
+    if (adaptive_wanted(c)) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_resolve_gathered divides by one sample count: not available with adaptive sampling");
     RT_CUDA(c, cudaSetDevice(c->device));
     const size_t n = (size_t)c->width * c->height;
     int k = 0;
@@ -2234,6 +2512,7 @@ int rt_set_gather_target(rt_ctx* c, void* base, uint64_t stride_bytes)
     RT_CHECK_CTX(c); RT_NOT_ON_GROUP(c, "rt_set_gather_target");
     { int rc = join_shadow(c); if (rc) return rc; }
     if (!base) { c->gather_slab = nullptr; c->gather_flag = nullptr; return RT_OK; }
+    if (adaptive_wanted(c)) RT_FAIL(c, RT_ERR_UNSUPPORTED, "a fused-gather target is not available with adaptive sampling (stopped pixels are never pushed)");
     const size_t rows_max = ((size_t)c->height + c->world - 1) / c->world;
     if (stride_bytes % 16 != 0 || stride_bytes < rows_max * c->width * 16)
         RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_gather_target: slab stride must be a multiple of 16 and hold %zu rows", rows_max);

@@ -124,6 +124,21 @@ void CUDAPathTraceIntegrator::SetSamplesPerFrame(std::uint32_t n)
     samples_per_frame_ = n;
 }
 
+void CUDAPathTraceIntegrator::SetAdaptiveSampling(float max_error, std::uint32_t min_samples)
+{
+    Check(rt_set_adaptive_sampling(ctx_, max_error, min_samples), "SetAdaptiveSampling");
+    RequestReset();
+}
+
+std::uint32_t CUDAPathTraceIntegrator::ActivePixels() const
+{
+    std::uint32_t n = 0;
+    Check(rt_read_active_pixels(ctx_, &n), "ActivePixels");
+    return n;
+}
+
+void CUDAPathTraceIntegrator::ReadPixelSamples(std::uint32_t* counts) const { Check(rt_read_pixel_samples(ctx_, counts), "ReadPixelSamples"); }
+
 // ---- the per-frame steps.  kFrame: Integrate() (integrator.cpp:27-59, not virtual) calls them in a fixed order; they are
 // checked against that order and the frame is submitted as a whole in AdvanceSampleCount().
 void CUDAPathTraceIntegrator::GenerateRays()

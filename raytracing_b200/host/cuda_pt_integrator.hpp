@@ -23,6 +23,8 @@
  * AdvanceSampleCount() submits them with ONE rt_integrate_samples call (n frames on the device without a host round trip, or
  * one launch of the regenerating frame kernel with RT_OPT_FRAME_KERNEL 1).  With n > 1 the kFused / kStepwise schedules, a call order other than
  * Integrate()'s and the denoiser (it runs once per sample) throw std::runtime_error.
+ * SetAdaptiveSampling(max_error, min_samples): pixels stop tracing once they have settled (include/rt_b200.h); ActivePixels() tells
+ * a progressive loop when every pixel has.
  * AOVs (ComputeAOVs) are produced inside the bounce-0 shading pass, and only when SetAOV selected a view other than
  * the shaded colour or the denoiser is on.  SetSamplerType(kBlueNoise) needs the sampler's three tables first
  * (SetBlueNoiseTables; the OpenCL backend reads them from utils/blue_noise_sampler.hpp, cl_pt_integrator.cpp:222-235).
@@ -69,6 +71,13 @@ public:
     // samples rendered by one Integrate() (default 1); n > 1 needs the kFrame schedule and no denoiser
     void SetSamplesPerFrame(std::uint32_t n);
     std::uint32_t SamplesPerFrame() const { return samples_per_frame_; }
+    // adaptive sampling (rt_set_adaptive_sampling): stop tracing pixels whose resolved luminance has a standard error <= max_error
+    // after >= min_samples samples; max_error 0 turns it off.  Requests a reset, like SetMaxBounces: it applies from the next frame.
+    void SetAdaptiveSampling(float max_error, std::uint32_t min_samples);
+    // pixels that trace the next sample (all of them with adaptive sampling off); blocks
+    std::uint32_t ActivePixels() const;
+    // every pixel's sample count, width*height entries; blocks
+    void ReadPixelSamples(std::uint32_t* counts) const;
     rt_ctx* Context() const { return ctx_; }
 
 protected:

@@ -182,6 +182,14 @@ int rth_render_set_samples_per_frame(void* h, std::uint32_t n)
 {
     try { ((RenderHandle*)h)->render->SetSamplesPerFrame(n); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_adaptive_sampling(void* h, float max_error, std::uint32_t min_samples)
+{
+    try { ((RenderHandle*)h)->render->SetAdaptiveSampling(max_error, min_samples); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
+}
+int rth_render_active_pixels(void* h, std::uint32_t* n)
+{
+    try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_enable_white_furnace(void* h, int e)
 {
     try { ((RenderHandle*)h)->render->GetIntegrator().EnableWhiteFurnace(e != 0); return 0; } catch (std::exception& ex) { g_error = ex.what(); return -1; }

@@ -40,10 +40,14 @@ public:
     std::vector<float> const& GetImage() const { return image_; }     // resolved RGBA32F, width*height
     void SetMaxBounces(std::uint32_t b) { integrator_->SetMaxBounces(b); }
     // progressive samples accumulated by one RenderFrame() (CUDAPathTraceIntegrator::SetSamplesPerFrame), default 1
-    void SetSamplesPerFrame(std::uint32_t n) { static_cast<CUDAPathTraceIntegrator&>(*integrator_).SetSamplesPerFrame(n); }
+    void SetSamplesPerFrame(std::uint32_t n) { Cuda().SetSamplesPerFrame(n); }
+    // adaptive sampling (CUDAPathTraceIntegrator::SetAdaptiveSampling): applies from the next RenderFrame(), which starts over
+    void SetAdaptiveSampling(float max_error, std::uint32_t min_samples) { Cuda().SetAdaptiveSampling(max_error, min_samples); }
+    std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 
 private:
+    CUDAPathTraceIntegrator& Cuda() { return static_cast<CUDAPathTraceIntegrator&>(*integrator_); }
     void Init(RenderBackend backend, const char* env_map_path, const Image* env_image, const std::vector<int>* devices, int device);
     Scene& scene_;
     std::uint32_t width_, height_;

@@ -43,6 +43,8 @@ def load_library():
     L.rth_render_free.argtypes = [C.c_void_p]
     L.rth_render_set_max_bounces.argtypes = [C.c_void_p, C.c_uint32]
     L.rth_render_set_samples_per_frame.argtypes = [C.c_void_p, C.c_uint32]
+    L.rth_render_set_adaptive_sampling.argtypes = [C.c_void_p, C.c_float, C.c_uint32]
+    L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler_tables.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -208,6 +210,18 @@ class HostRender:
         """Progressive samples accumulated by one render_frame() (Render::SetSamplesPerFrame); needs the "frame" schedule for n > 1."""
         if self.L.rth_render_set_samples_per_frame(self.h, n) != 0:
             raise _err(self.L)
+
+    def set_adaptive_sampling(self, max_error, min_samples=2):
+        """Render::SetAdaptiveSampling: pixels stop tracing once they have settled; applies from the next render_frame()."""
+        if self.L.rth_render_set_adaptive_sampling(self.h, float(max_error), int(min_samples)) != 0:
+            raise _err(self.L)
+
+    def active_pixels(self):
+        """Render::ActivePixels: pixels that trace the next sample."""
+        n = C.c_uint32()
+        if self.L.rth_render_active_pixels(self.h, C.byref(n)) != 0:
+            raise _err(self.L)
+        return n.value
 
     def enable_white_furnace(self, e):
         if self.L.rth_render_enable_white_furnace(self.h, int(e)) != 0:
