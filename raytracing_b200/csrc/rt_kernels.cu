@@ -44,13 +44,20 @@
 using namespace rt;
 
 // minimum resident CTAs per SM requested from ptxas for the hot kernels (register budget = 65536 / (256 * N)):
-// 5 x 256 threads at <= 48 registers and 4 x 256 at <= 64 fill the 64 K-register file of an SM (the same on H100), see DESIGN.md section 4
+// 5 x 256 threads at <= 48 registers fill the 64 K-register file of an SM (the same on H100).  The shading kernel runs 3 x 256 at
+// <= 85 registers (80, no spills): on an H100 it is 12 % faster than 4 x 256 at 64 registers, which spills (DESIGN.md section 4)
 #ifndef RT_MINB_TRACE
 #define RT_MINB_TRACE 5
 #endif
 #ifndef RT_MINB_SHADE
-#define RT_MINB_SHADE 4
+#define RT_MINB_SHADE 3
 #endif
+// k_shade_queues<true> (large partitions) shades up to RT_SHADE_BATCH hit-queue entries per CTA at a time and writes their continuation rays out sorted by a
+// 6-bit key (RT_SORT_BINS keys): 48 B of shared memory per staged ray, so 1024 rays x 3 resident CTAs take 3 x 52 KB of an SM's 227 KB
+#ifndef RT_SHADE_BATCH
+#define RT_SHADE_BATCH 1024
+#endif
+#define RT_SORT_BINS 64
 // The whole-frame kernel (k_frame) is compiled for up to 1024 threads per CTA (64 registers): the CTA size is chosen at launch
 // (RT_OPT_FRAME_THREADS) — 1024 threads = one CTA per SM, all 32 warps of an SM in the same phase; 256 threads = 4 CTAs per SM
 // in different phases
@@ -233,12 +240,35 @@ __device__ __forceinline__ void shadow_group(const FrameParams& p, const DevScen
     warp_count(n_unoccluded, un);
 }
 
+// k_shade_queues' dynamic shared memory: one batch of continuation rays, written out in key order by a counting sort
+struct ContStage
+{
+    float4 mid;                                                        // centre of the scene's bounding box (the origin half of the key)
+    float4 A[RT_SHADE_BATCH], B[RT_SHADE_BATCH], C[RT_SHADE_BATCH];    // the rays as the warps staged them (queue planes A, B, C)
+    uint16_t perm[RT_SHADE_BATCH];                                     // output position -> staged ray
+    uint8_t key[RT_SHADE_BATCH];
+    uint32_t count[RT_SORT_BINS];                                      // rays per key, then the next output position of each key
+    uint32_t n, at, out;                                               // rays staged, the batch's first cursor entry, its first slot in the queue
+};
+
+// The key of a continuation ray: direction octant (high 3 bits) and the octant of the origin about the scene's centre.  It only
+// orders the queue, so that the warps of the next traversal and shading passes hold rays that start in the same part of the scene
+// and head the same way; no result depends on it.
+__device__ __forceinline__ uint32_t ray_key(f3 o, f3 d, float4 mid)
+{
+    return (d.x < 0.0f ? 8u : 0u) | (d.y < 0.0f ? 16u : 0u) | (d.z < 0.0f ? 32u : 0u)
+         | (o.x >= mid.x ? 1u : 0u) | (o.y >= mid.y ? 2u : 0u) | (o.z >= mid.z ? 4u : 0u);
+}
+
 // ShadeSurfaceHits (hit_surface.cl) of the hit h = (bc.x, bc.y, primitive_id bits, -) of the ray in entry i (hit lanes): shading,
 // emission into the radiance, and compaction of the two output streams — ONE 64-bit atomic per warp on `emit` reserves the slots
-// of both queues (shadow rays in the low word, continuation rays in the high).  Returns whether the lane's path ends at this hit
-// (no continuation ray); `pixel` is the packed pixel of the ray.
+// of both queues (shadow rays in the low word, continuation rays in the high).  With STAGE the continuation rays go to the CTA's
+// staging area `st` instead (flush_continuations writes them out and counts them) and the atomic reserves shadow-ray slots only.
+// Returns whether the lane's path ends at this hit (no continuation ray); `pixel` is the packed pixel of the ray.
+template <bool STAGE = false>
 __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevScene& sc, const AovParams& aov, const Queues& q, uint32_t base, uint32_t bounce,
-                                                bool hit, float4 h, uint32_t i, float4* radiance, unsigned long long* emit, uint32_t* n_emissive, uint32_t& pixel)
+                                                bool hit, float4 h, uint32_t i, float4* radiance, unsigned long long* emit, uint32_t* n_emissive, uint32_t& pixel,
+                                                ContStage* st = nullptr)
 {
     const int in = bounce & 1, out = (bounce + 1) & 1;
     ShadeOut so;
@@ -261,7 +291,8 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
     {
         if (lane == 0)
         {
-            slot = atomicAdd(emit, (unsigned long long)__popc(smask) | ((unsigned long long)__popc(nmask) << 32));
+            if (STAGE) { if (smask) slot = atomicAdd((uint32_t*)emit, (uint32_t)__popc(smask)); }
+            else slot = atomicAdd(emit, (unsigned long long)__popc(smask) | ((unsigned long long)__popc(nmask) << 32));
             if (emask) atomicAdd(n_emissive, (uint32_t)__popc(emask));
         }
         slot = __shfl_sync(0xffffffffu, slot, 0);
@@ -273,7 +304,25 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
         q.sB[si] = make_float4(so.s_dir.x, so.s_dir.y, so.s_dir.z, so.s_tmax);
         q.sC[si] = make_float4(so.s_sample.x, so.s_sample.y, so.s_sample.z, 0.0f);
     }
-    if (sn)
+    if (STAGE)
+    {
+        uint32_t j = 0;
+        if (nmask)
+        {
+            if (lane == 0) j = atomicAdd(&st->n, (uint32_t)__popc(nmask));
+            j = __shfl_sync(0xffffffffu, j, 0) + __popc(nmask & lt_mask);
+        }
+        if (sn)
+        {
+            st->A[j] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
+            st->B[j] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
+            st->C[j] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, 0.0f);
+            const uint32_t key = ray_key(so.n_origin, so.n_dir, st->mid);
+            st->key[j] = (uint8_t)key;
+            atomicAdd(&st->count[key], 1u);
+        }
+    }
+    else if (sn)
     {
         const uint32_t ni = base + (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
         q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
@@ -452,26 +501,102 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_both(FrameParams p
     shadow_phase<false, SMEM>(p, sc, mode, q, ctr, radiance, shadow_bounce, s_bvh);
 }
 
-// ShadeSurfaceHits over the hit queue, then ShadeMissedRays over the miss queue (independent pixels).
-__global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce, AovParams aov)
+// The staged continuation rays of a batch into ray queue `out`, sorted by key (counting sort in shared memory), at slots that
+// ONE atomic per CTA on `n_next` reserves.  The order of a ray queue never changes a result: at most one path per pixel is
+// alive, and the additions into a pixel's radiance are ordered by phase, not by queue slot.
+__device__ __forceinline__ void flush_continuations(ContStage& st, const Queues& q, int out, uint32_t* n_next)
 {
+    __syncthreads();                                            // every warp of the batch has staged its rays
+    const uint32_t n = st.n;
+    if (threadIdx.x < 32)
+    {   // exclusive scan of the key counts, two keys per lane
+        const int lane = threadIdx.x;
+        const uint32_t c0 = st.count[2 * lane], c1 = st.count[2 * lane + 1];
+        uint32_t s = c0 + c1;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1)
+        {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, s, o);
+            if (lane >= o) s += t;
+        }
+        s -= c0 + c1;
+        st.count[2 * lane] = s; st.count[2 * lane + 1] = s + c0;
+        if (lane == 0 && n) st.out = atomicAdd(n_next, n);
+    }
+    __syncthreads();
+    for (uint32_t j = threadIdx.x; j < n; j += blockDim.x) st.perm[atomicAdd(&st.count[st.key[j]], 1u)] = (uint16_t)j;
+    __syncthreads();
+    const uint32_t o = st.out;
+    for (uint32_t d = threadIdx.x; d < n; d += blockDim.x)
+    {   // coalesced stores in key order
+        const uint32_t j = st.perm[d];
+        q.A[out][o + d] = st.A[j]; q.B[out][o + d] = st.B[j]; q.C[out][o + d] = st.C[j];
+    }
+}
+
+// ShadeSurfaceHits over the hit queue, then ShadeMissedRays over the miss queue (independent pixels).
+// SORT = false: every warp takes 32 entries at a time and stores its continuation rays as it shades them.
+// SORT = true (large partitions, sorted_shading): the hits are taken by the CTA in batches of up to RT_SHADE_BATCH entries, one
+// cursor add each, so that their continuation rays leave sorted by ray_key (flush_continuations); the batch shrinks towards 256
+// entries when there are fewer than 4 full batches per CTA, so that the CTAs still finish together.  Misses past the last hit
+// batch are taken 32 at a time by each warp.
+template <bool SORT>
+__global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce,
+                                                                     AovParams aov, float4 scene_mid)
+{
+    extern __shared__ __align__(16) float4 s_dyn[];
+    ContStage& st = *reinterpret_cast<ContStage*>(s_dyn);
+    if (SORT && threadIdx.x == 0) st.mid = scene_mid;
     pdl_wait(); pdl_launch_dependents();
     const uint32_t n_hit = ctr->hm[bounce].hit, n_miss = ctr->hm[bounce].miss;
     const uint32_t hit_span = (n_hit + 31u) & ~31u;            // warps never mix hits and misses
-    const int lane = threadIdx.x & 31;
-    for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < hit_span + n_miss;)
+    const uint32_t total = hit_span + n_miss;
+    if (!SORT)
     {
-        if (at < hit_span)
+        const int lane = threadIdx.x & 31;
+        for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < total;)
         {
-            const uint32_t k = at + lane;
-            const bool hit = k < n_hit;
-            float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-            if (hit) h = q.hitq[k];
-            uint32_t pixel;
-            shade_hit_group(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
+            if (at < hit_span)
+            {
+                const uint32_t k = at + lane;
+                const bool hit = k < n_hit;
+                float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (hit) h = q.hitq[k];
+                uint32_t pixel;
+                shade_hit_group(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
+            }
+            else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
         }
-        else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
+        return;
     }
+    const uint32_t batch = min((uint32_t)RT_SHADE_BATCH, max(256u, (n_hit / (gridDim.x * 4u) + 31u) & ~31u));
+    const int lane = threadIdx.x & 31, in = bounce & 1;
+    for (uint32_t at;;)
+    {
+        __syncthreads();                                        // the previous batch is written out: staging area and counts are free
+        if (threadIdx.x < RT_SORT_BINS) st.count[threadIdx.x] = 0;
+        if (threadIdx.x == 0) { st.at = atomicAdd(&ctr->work_shade[bounce], batch); st.n = 0; }
+        __syncthreads();
+        at = st.at;
+        const uint32_t end = min(at + batch, total);
+        for (uint32_t g = at + (threadIdx.x & ~31u); g < end; g += blockDim.x)
+        {
+            if (g < hit_span)
+            {
+                const uint32_t k = g + lane;
+                const bool hit = k < n_hit;
+                float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (hit) h = q.hitq[k];
+                uint32_t pixel;
+                shade_hit_group<true>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
+            }
+            else if (g - hit_span + lane < n_miss) shade_miss(sc, p, q, in, q.missq[g - hit_span + lane], radiance);
+        }
+        if (at < hit_span) flush_continuations(st, q, in ^ 1, &ctr->emit[bounce].next);
+        if (at + batch >= hit_span) break;                      // every later entry is a miss
+    }
+    for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < total;)
+        if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, in, q.missq[at - hit_span + lane], radiance);
 }
 
 #include "rt_frame_kernel.cuh"
@@ -813,6 +938,7 @@ struct rt_ctx
     // scene
     bool scene_ready = false, camera_ready = false;
     DevScene scene = {};
+    float4 scene_mid = {};                         // centre of the root box: the origin half of k_shade_queues' sort key
     std::vector<void*> scene_allocs;
     RtCamera camera = {};
     RayGenConsts raygen = {};
@@ -1066,6 +1192,15 @@ int persistent_grid(rt_ctx* c, const void* kernel, size_t dyn_smem)
 }
 #define RT_PGRID(c, kern, smem) persistent_grid(c, (const void*)(kern), smem)
 
+// Does k_shade_queues write its continuation rays sorted by ray_key?  Measured on an H100 (DESIGN.md section 4): the sorted order
+// makes the next traversal 2-12 % faster, but the staging costs the shading pass more than that on a 1080p frame per GPU (15.7 K
+// pixels per SM on 132 SMs) and wins on a 4K frame (62.8 K): sorted above 32 K pixels per SM (a variant built with
+// -DRT_SORT_MIN_PIXELS_PER_SM=0 sorts at every size, tools/coherence_probe.py).
+#ifndef RT_SORT_MIN_PIXELS_PER_SM
+#define RT_SORT_MIN_PIXELS_PER_SM 32768u
+#endif
+bool sorted_shading(const rt_ctx* c) { return (uint64_t)c->n_local > (uint64_t)RT_SORT_MIN_PIXELS_PER_SM * (uint32_t)c->num_sms; }
+
 // Can the traversal kernel of the next bounce also run a deferred shadow pass (k_trace_both)?
 bool merged_trace_available(const rt_ctx* c) { return !c->count_traversal && !c->kernel_timing; }
 
@@ -1198,6 +1333,8 @@ int rt_create(uint32_t width, uint32_t height, int device, rt_ctx** out_ctx)
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail("cudaGetDeviceProperties", e);
     c->num_sms = prop.multiProcessorCount;
+    if ((e = cudaFuncSetAttribute(k_shade_queues<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess)
+        return fail("cudaFuncSetAttribute(k_shade_queues)", e);
     if ((e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
     if ((e = cudaMalloc(&c->counters, sizeof(DevCounters))) != cudaSuccess) return fail("cudaMalloc(counters)", e);
     if ((e = cudaMalloc(&c->d_dyn, sizeof(FrameDyn))) != cudaSuccess) return fail("cudaMalloc(frame constants)", e);
@@ -1340,6 +1477,9 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
         ds.wnodes_f4 = (uint32_t)wl.nodes.size(); ds.wtris_f4 = (uint32_t)wl.tris.size();
         ds.top_n = wl.top_n; ds.top_k = 0;
     }
+    const RtLinearBVHNode& root = s->nodes[0];
+    c->scene_mid = make_float4((root.bounds_min.x + root.bounds_max.x) * 0.5f, (root.bounds_min.y + root.bounds_max.y) * 0.5f,
+                               (root.bounds_min.z + root.bounds_max.z) * 0.5f, 0.0f);
     c->scene_ready = true;
     ++c->config_gen;
     return RT_OK;
@@ -1686,7 +1826,10 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     }
     { int rc = join_shadow(c); if (rc) return rc; }     // the shading pass accumulates into radiance and refills the shadow queue
     TimedLaunch t(c, RT_K_SHADE_QUEUES);
-    launch_chain(c, k_shade_queues, RT_PGRID(c, k_shade_queues, 0), 0, c->stream, frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
+    const bool sort = sorted_shading(c);
+    auto* k = sort ? k_shade_queues<true> : k_shade_queues<false>;
+    const size_t sm = sort ? sizeof(ContStage) : 0;
+    launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
     return post_launch(c, "k_shade_queues");
 }
 

@@ -1,4 +1,5 @@
-"""Issue-slot model (tools/simt_model.cpp): effect of CTA-local re-ordering of the ray queue (blocks of B rays sorted by a small key)."""
+"""Issue-slot model (tools/simt_model.cpp): effect of CTA-local re-ordering of the ray queue (blocks of B rays sorted by a small key).
+usage: simt_reorder.py [scene [width height max_bounces [bounces [blocks]]]]   (bounces and blocks comma-separated; block 0 = the whole queue)"""
 import ctypes as C, os, subprocess, sys, tempfile
 import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__)); REPO = os.path.dirname(HERE)
@@ -15,6 +16,7 @@ M.simt_model.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_voi
 name = sys.argv[1] if len(sys.argv) > 1 else "CornellBox"
 w, h, mb = (int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4])) if len(sys.argv) > 4 else (960, 540, 3)
 bounces = [int(b) for b in sys.argv[5].split(",")] if len(sys.argv) > 5 else [1, 2]
+blocks = [int(b) for b in sys.argv[6].split(",")] if len(sys.argv) > 6 else [1024, 2048, 4096, 16384, 0]     # 0 = the whole queue
 sc = scene_io.load_scene(name); o = Oracle(sc); cam = default_camera(w, h)
 nodes = np.ascontiguousarray(sc["nodes"]); tris = np.ascontiguousarray(sc["triangles"])
 costs = np.array([75.0, 24.0, 48.0, 66.0, 78.0, 90.0])
@@ -55,7 +57,7 @@ for bounce in bounces:
             "oct+org1": octant(d) * 8 + ocell(org, 1), "oct+org2": octant(d) * 64 + ocell(org, 2),
             "org2+oct": ocell(org, 2) * 8 + octant(d), "org2+dir2": ocell(org, 2) * 64 + dcell(d, 2), "dir2+org2": dcell(d, 2) * 64 + ocell(org, 2),
             "org3+dir3": ocell(org, 3) * 512 + dcell(d, 3), "dir3+org3": dcell(d, 3) * 512 + ocell(org, 3), "org2+dir3": ocell(org, 2) * 512 + dcell(d, 3)}
-    for B in (1024, 2048, 4096, 16384, n):
+    for B in [b or n for b in blocks]:
         line = f"   block {B if B != n else 'all':>6}: "
         for label, key in keys.items():
             out = run(np.ascontiguousarray(r[blocked(key, B)]))
