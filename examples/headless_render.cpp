@@ -6,12 +6,14 @@
  *
  *   g++ -std=c++17 -O2 -Iinclude -Iraytracing_b200/host examples/headless_render.cpp \
  *       -Lraytracing_b200 -lrt_host -lrt_b200 -Wl,-rpath,'$ORIGIN/../raytracing_b200' -o examples/headless_render
- *   examples/headless_render assets/CornellBox.obj assets/ibl/CGSkies_0036_free.hdr 1920 1080 64 out.pfm [all|d0,d1,...] [max_error=E]
+ *   examples/headless_render assets/CornellBox.obj assets/ibl/CGSkies_0036_free.hdr 1920 1080 64 out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ]
  *
  * The optional device list spreads the frame over several GPUs of the node behind the same Render / Integrator objects
  * ("all" = every CUDA device; the image is partitioned by scanline inside the library, rt_create_multi).
  * max_error=E turns on adaptive sampling (Render::SetAdaptiveSampling(E, 4)): `samples` becomes the budget, rendered in
  * RenderFrame() calls of 16 samples until no pixel is active any more or the budget is spent; the mean samples per pixel is printed.
+ * denoise=ITER,SC,SN,SZ turns on the spatial denoiser (Render::SetSpatialDenoiser: ITER passes, the colour, normal and depth sigmas)
+ * on a single-device render.
  *
  * Needs an H100 (there is no CPU fallback: Render's constructor throws without a CUDA device).
  */
@@ -28,13 +30,20 @@
 
 int main(int argc, char** argv)
 {
-    if (argc < 7) { std::fprintf(stderr, "usage: %s scene.obj env.hdr width height samples out.pfm [all|d0,d1,...] [max_error=E]\n", argv[0]); return 2; }
+    if (argc < 7) { std::fprintf(stderr, "usage: %s scene.obj env.hdr width height samples out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ]\n", argv[0]); return 2; }
     const unsigned width = (unsigned)std::atoi(argv[3]), height = (unsigned)std::atoi(argv[4]), samples = (unsigned)std::atoi(argv[5]);
     float max_error = 0.0f;                                                                         // 0: every pixel takes every sample
     const char* device_arg = nullptr;
+    unsigned denoise_iters = 0;                                                                     // 0: no spatial denoiser
+    float sigma_color = 0.0f, sigma_normal = 0.0f, sigma_depth = 0.0f;
     for (int i = 7; i < argc; ++i)
     {
         if (std::string(argv[i]).rfind("max_error=", 0) == 0) max_error = (float)std::atof(argv[i] + 10);
+        else if (std::string(argv[i]).rfind("denoise=", 0) == 0)
+        {
+            if (std::sscanf(argv[i] + 8, "%u,%f,%f,%f", &denoise_iters, &sigma_color, &sigma_normal, &sigma_depth) != 4)
+            { std::fprintf(stderr, "denoise=ITER,SC,SN,SZ expects four numbers\n"); return 2; }
+        }
         else device_arg = argv[i];
     }
     try
@@ -49,6 +58,7 @@ int main(int argc, char** argv)
                                                      : new rt_host::Render(width, height, rt_host::Render::RenderBackend::kCUDA, scene, argv[2]));
         rt_host::Render& render = *owner;
         render.SetMaxBounces(8);
+        if (denoise_iters > 0) render.SetSpatialDenoiser(denoise_iters, sigma_color, sigma_normal, sigma_depth);
         if (samples > 0 && max_error > 0.0f)
         {   // progressive: chunks of 16 samples until every pixel has settled or the budget is spent
             render.SetAdaptiveSampling(max_error, 4);

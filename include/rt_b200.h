@@ -207,7 +207,7 @@ int rt_gather_wait(rt_ctx* ctx);
 
 /* Parity tap for include/rt_math.h (the elementary functions shared with the oracle): out[i] = f(a[i], b[i]) evaluated on
  * `device`; host pointers, blocking.  fn: 0 sin, 1 cos, 2 tan, 3 atan2(a, b), 4 acos, 5 pow(a, b), 6 fmin, 7 fmax,
- * 8 1 / sqrt(a), 9 a / b. */
+ * 8 1 / sqrt(a), 9 a / b, 10 rt_expf(a). */
 int rt_math_eval(int device, int fn, const float* a, const float* b, float* out, uint64_t n);
 
 /* Pipelined read-back for frame loops: resolve on the render stream, device->host copy on a second stream (overlaps the
@@ -279,6 +279,30 @@ int rt_set_adaptive_sampling(rt_ctx* ctx, float max_error, uint32_t min_samples)
 int rt_read_pixel_samples(rt_ctx* ctx, uint32_t* counts);
 /* Pixels that will trace the next sample (blocking; summed over the devices of a multi-device context).  Off: the local pixel count. */
 int rt_read_active_pixels(rt_ctx* ctx, uint32_t* n_active);
+
+/* ---- spatial denoiser (new capability) -----------------------------------------------------------------------------------
+ * An edge-avoiding a-trous wavelet filter (Dammertz et al. 2010) on the shaded-colour view of rt_resolve / rt_resolve_async (the
+ * host image and the device resolve target), guided by the bounce-0 AOVs of the last frame rendered.  The accumulation is never
+ * touched: radiance, sample counts, AOVs, frame statistics and the AOV views 1-4 are what they are with the filter off.
+ * iterations 0 = off; 1..5 passes with tap spacing s = 2^i, i = 0 .. iterations-1.  The input of pass 0 is the image k_resolve
+ * produces (Reinhard colour in display units, from radiance / sample count, the per-pixel counts of adaptive sampling, or the
+ * radiance alone under the temporal denoiser); pass i maps image c to image c', all in float (no contraction):
+ *     kc = 1 / (sigma_color * sigma_color) * 2^i,  kn = 1 / (sigma_normal * sigma_normal),  kz = 1 / (sigma_depth * z_p)   (0 if sigma 0)
+ *     centre p: if c_p is not finite, the colour term uses c_p = 0 and kc = 0 for this pixel
+ *     for ty = -2..2, tx = -2..2 (row by row): q = p + s * (tx, ty); skip q outside the image and q whose colour is not finite;
+ *         dc = (dr*dr + dg*dg) + db*db of c_p - c_q;  dn = the same of n_p - n_q (shading normal xyz);  dz = |z_p - z_q| (depth)
+ *         term(d, k) = (k > 0 and d > 0) ? d * k : 0;   D = (term(dc, kc) + term(dn, kn)) + term(dz, kz)
+ *         w = (h[ty] * h[tx]) * rt_expf(-D),  h = (1/16, 1/4, 3/8, 1/4, 1/16)
+ *         if w > 0: W += w; S += w * c_q (per channel)
+ *     c'_p = S / W per channel if W > 0, else c_p; alpha 1.
+ * A sigma of 0 drops its term; a NaN or inf pixel never spreads, and a pixel with no usable tap keeps its value.
+ * Turning the filter on makes frames produce the AOVs (as an AOV view or the temporal denoiser do; the captured frame graph is
+ * re-captured).  rt_resolve / rt_resolve_async return RT_ERR_NOT_READY until a frame has written every local pixel's AOVs with the
+ * filter (or another AOV consumer) on: after turning it on, and, with adaptive sampling, until the first frame after an rt_reset.
+ * Two colour planes and one guide record (16 bytes each per pixel) are allocated while it is on.  Its launches count under
+ * RT_K_RESOLVE.  RT_ERR_INVALID_ARGUMENT: iterations > 5, a negative or non-finite sigma.  RT_ERR_UNSUPPORTED, whichever call comes
+ * second: a multi-device context, rt_set_partition with world > 1, and rt_resolve_gathered[_async]. */
+int rt_set_spatial_denoiser(rt_ctx* ctx, uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth);
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

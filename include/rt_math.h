@@ -248,6 +248,35 @@ RT_HD double rt_exp_d(double t)
     return ldexp(p, (int)kd);
 }
 
+/* exp of a float in float arithmetic only (the edge-stopping weights of the spatial denoiser: one per tap, 25 taps x 5 passes per
+ * pixel, where a double exp would cost more than the filter's memory traffic).  Cody-Waite reduction x = k ln2 + r, |r| <= ln2/2
+ * (ln2_hi has 16 significant bits, so k * ln2_hi is exact for |k| <= 256), the degree-7 Taylor polynomial of exp(r) (truncation
+ * error < 5e-9 relative) in Horner form, and a scale by 2^k built from its exponent bits.  Below ln(FLT_MIN) the result is 0
+ * (no subnormals), above ln(FLT_MAX) it is +inf; NaN in, NaN out.  Within 1.25 ulp of the exact exp over [-87.3, 88.7] (the bound
+ * tests/test_spatial_denoise_cpu.py checks). */
+RT_HD float rt_expf(float x)
+{
+    if (x != x) return x + x;
+    if (x > 88.72283935546875f) return INFINITY;
+    if (x < -87.33654022216797f) return 0.0f;
+    const float ln2_hi = 0.693145751953125f;
+    const float ln2_lo = 1.42860682030941723212e-06f;
+    const float kf = rintf(x * 1.44269502162933349609f);
+    float r = x - kf * ln2_hi;
+    r = r - kf * ln2_lo;
+    float p = 1.98412701e-04f;        /* 1/5040 */
+    p = p * r + 1.38888892e-03f;      /* 1/720 */
+    p = p * r + 8.33333377e-03f;      /* 1/120 */
+    p = p * r + 4.16666679e-02f;      /* 1/24 */
+    p = p * r + 1.66666672e-01f;      /* 1/6 */
+    p = p * r + 0.5f;
+    p = p * r + 1.0f;
+    p = p * r + 1.0f;
+    const int k = (int)kf;            /* -126 .. 128 */
+    if (k > 127) return (p * rt_bits_float(254u << 23)) * 2.0f;
+    return p * rt_bits_float((uint32_t)(k + 127) << 23);
+}
+
 /* pow(x, y).  The path only needs pow(x, 5.0f) (Schlick Fresnel, bxdf.h:71-74,
  * any sign of x) and pow(x in [0,1], 2.2f) (texture gamma, material.h:251-264).
  * y == 5 is evaluated as an exact-in-double product (also right for x < 0);

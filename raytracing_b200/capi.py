@@ -33,7 +33,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_radiance_device_ptr", "rt_stream_handle",
            "rt_create_multi", "rt_device_count", "rt_gather_radiance", "rt_host_register", "rt_host_unregister", "rt_math_eval",
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
-           "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels"]
+           "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser"]
 
 
 class RtSceneDesc(C.Structure):
@@ -115,6 +115,7 @@ def load_library():
     L.rt_set_adaptive_sampling.argtypes = [C.c_void_p, C.c_float, C.c_uint32]
     L.rt_read_pixel_samples.argtypes = [C.c_void_p, C.c_void_p]
     L.rt_read_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
+    L.rt_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
     _lib = L
     return L
 
@@ -260,6 +261,12 @@ class Context:
         self._ck(self.lib.rt_read_active_pixels(self.h, C.byref(n)))
         return n.value
 
+    # ---- spatial denoiser
+    def set_spatial_denoiser(self, iterations, sigma_color=0.0, sigma_normal=0.0, sigma_depth=0.0):
+        """Edge-avoiding a-trous filter on the shaded colour of resolve() / resolve_async() (rt_set_spatial_denoiser): iterations
+        0 (off) .. 5, guided by the last frame's normal and depth; a sigma of 0 drops its term."""
+        self._ck(self.lib.rt_set_spatial_denoiser(self.h, int(iterations), float(sigma_color), float(sigma_normal), float(sigma_depth)))
+
     def integrate_stepwise(self, max_bounces):
         """The schedule of Integrator::Integrate (integrator.cpp:35-51), one call per reference virtual."""
         self.generate_rays()
@@ -382,7 +389,7 @@ def host_unregister(array) -> None:
     load_library().rt_host_unregister(array.ctypes.data)
 
 
-MATH_FUNCTIONS = {"sin": 0, "cos": 1, "tan": 2, "atan2": 3, "acos": 4, "pow": 5, "fmin": 6, "fmax": 7, "rsqrt": 8, "div": 9}
+MATH_FUNCTIONS = {"sin": 0, "cos": 1, "tan": 2, "atan2": 3, "acos": 4, "pow": 5, "fmin": 6, "fmax": 7, "rsqrt": 8, "div": 9, "exp": 10}
 
 
 def math_eval(fn: str, a, b=None, device: int = 0):

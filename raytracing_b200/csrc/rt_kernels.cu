@@ -623,6 +623,70 @@ __global__ void __launch_bounds__(256) k_resolve(const float4* radiance, float4*
     }
 }
 
+// ---- spatial denoiser (rt_set_spatial_denoiser) -------------------------------------------------------------------
+// The guides of one pixel in one record: shading normal xyz and depth of the last frame's bounce-0 AOVs.
+__global__ void __launch_bounds__(256) k_sd_pack(const float4* normal, const float* depth, float4* guide, uint32_t n)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 nn = normal[i];
+    guide[i] = make_float4(nn.x, nn.y, nn.z, depth[i]);
+}
+
+__device__ __forceinline__ bool sd_finite(float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z); }
+// a term of the distance: its difference times its factor, added only when both are positive (a sigma of 0 drops the term)
+__device__ __forceinline__ float sd_term(float diff, float k) { return (k > 0.0f && diff > 0.0f) ? diff * k : 0.0f; }
+
+// One a-trous pass (the rule is stated with rt_set_spatial_denoiser in rt_b200.h): 5x5 taps at spacing `step` around every pixel,
+// B3-spline weights times rt_expf(-(colour + normal + depth distance)), taps outside the image skipped, taps of non-finite colour
+// skipped; taps summed row by row, left to right.  One thread per pixel over 32x8 tiles; the taps are read through L1.
+__global__ void __launch_bounds__(256) k_sd_pass(const float4* __restrict__ src, float4* __restrict__ dst, const float4* __restrict__ guide,
+                                                 uint32_t width, uint32_t height, int step, float kc, float kn, float sigma_depth)
+{
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    const float h[5] = { 0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f };
+    const uint32_t p = y * width + x;
+    const float4 cp = __ldg(&src[p]);
+    const float4 gp = __ldg(&guide[p]);
+    const bool cfin = sd_finite(cp);
+    const float c0x = cfin ? cp.x : 0.0f, c0y = cfin ? cp.y : 0.0f, c0z = cfin ? cp.z : 0.0f;
+    const float kcp = cfin ? kc : 0.0f;                        // a non-finite centre drops its colour term
+    const float kz = sigma_depth > 0.0f ? 1.0f / (sigma_depth * gp.w) : 0.0f;
+    float wsum = 0.0f, s0 = 0.0f, s1 = 0.0f, s2 = 0.0f;
+#pragma unroll
+    for (int ty = -2; ty <= 2; ++ty)
+    {
+        const int qy = (int)y + ty * step;
+        if (qy < 0 || qy >= (int)height) continue;
+#pragma unroll
+        for (int tx = -2; tx <= 2; ++tx)
+        {
+            const int qx = (int)x + tx * step;
+            if (qx < 0 || qx >= (int)width) continue;
+            const uint32_t q = (uint32_t)qy * width + (uint32_t)qx;
+            const float4 cq = __ldg(&src[q]);
+            if (!sd_finite(cq)) continue;
+            const float4 gq = __ldg(&guide[q]);
+            const float dr = c0x - cq.x, dg = c0y - cq.y, db = c0z - cq.z;
+            const float dc = (dr * dr + dg * dg) + db * db;
+            const float nx = gp.x - gq.x, ny = gp.y - gq.y, nz = gp.z - gq.z;
+            const float dn = (nx * nx + ny * ny) + nz * nz;
+            const float dz = fabsf(gp.w - gq.w);
+            float d = sd_term(dc, kcp);
+            d = d + sd_term(dn, kn);
+            d = d + sd_term(dz, kz);
+            const float w = (h[ty + 2] * h[tx + 2]) * rt_expf(-d);
+            if (w > 0.0f)
+            {
+                wsum = wsum + w;
+                s0 = s0 + w * cq.x; s1 = s1 + w * cq.y; s2 = s2 + w * cq.z;
+            }
+        }
+    }
+    dst[p] = wsum > 0.0f ? make_float4(s0 / wsum, s1 / wsum, s2 / wsum, 1.0f) : make_float4(cp.x, cp.y, cp.z, 1.0f);
+}
+
 // ---- adaptive sampling (rt_set_adaptive_sampling) ----------------------------------------------------------------
 struct AdaptiveState
 {
@@ -831,6 +895,7 @@ __global__ void k_math_eval(int fn, const float* a, const float* b, float* out, 
     case 7: r = rt_fmaxf(x, y); break;
     case 8: r = 1.0f / sqrtf(x); break;          // the normalize() building blocks: IEEE sqrt and division
     case 9: r = x / y; break;
+    case 10: r = rt_expf(x); break;
     }
     out[i] = r;
 }
@@ -948,6 +1013,14 @@ struct rt_ctx
     float ad_req_error = 0.0f; uint32_t ad_req_min = 0;
     float ad_error = 0.0f; uint32_t ad_min = 0;
     AdaptiveState ad = {};
+    bool ad_fresh = false;                         // no frame has run since the adaptive state was reset (every local pixel traces the next)
+
+    // spatial denoiser (rt_set_spatial_denoiser): passes (0 = off), sigmas, scratch planes (allocated while it is on)
+    uint32_t sd_iters = 0;
+    float sd_sigma_c = 0.0f, sd_sigma_n = 0.0f, sd_sigma_z = 0.0f;
+    float4* sd_col[2] = { nullptr, nullptr };
+    float4* sd_guide = nullptr;
+    bool aov_ready = false;                        // the AOV buffers hold the last frame's bounce-0 guides for every local pixel
 
     uint32_t sample_count = 0;
     uint32_t cur_bounce = 0;
@@ -1086,6 +1159,7 @@ void free_frame_buffers(rt_ctx* c)
     freep(c->q.sA); freep(c->q.sB); freep(c->q.sC); freep(c->q.hits); freep(c->q.shadow_flags);
     freep(c->q.hitq); freep(c->q.missq);
     freep(c->radiance); freep(c->resolved); freep(c->resolved2);
+    freep(c->sd_col[0]); freep(c->sd_col[1]); freep(c->sd_guide);
     free_aov_buffers(c);
     freep(c->ad.count); freep(c->ad.y_prev); freep(c->ad.q); freep(c->ad.list); freep(c->ad.tile); freep(c->ad.ctl);
 }
@@ -1119,6 +1193,7 @@ int reset_adaptive(rt_ctx* c)
     }
     RT_CUDA(c, cudaMemsetAsync(c->ad.count, 0, n * 4, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->ad.y_prev, 0, n * 4, c->stream));
     RT_CUDA(c, cudaMemsetAsync(c->ad.q, 0, n * 8, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->ad.tile, 0, tiles * 8, c->stream));
+    c->ad_fresh = true;
     TimedLaunch t(c, RT_K_MISC);
     k_adaptive_init<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->ad, c->n_local);
     return post_launch(c, "k_adaptive_init");
@@ -1260,7 +1335,17 @@ FrameDyn frame_dyn(const rt_ctx* c)
     return dyn;
 }
 
-bool aov_wanted(const rt_ctx* c) { return c->aov != 0 || c->denoiser != 0 || c->aov_always != 0; }
+bool aov_wanted(const rt_ctx* c) { return c->aov != 0 || c->denoiser != 0 || c->aov_always != 0 || c->sd_iters != 0; }
+
+// A frame starts: its bounce-0 pass writes the AOVs of the pixels it traces.  They hold a complete set of guides (aov_ready) after a
+// frame with AOVs on in which every local pixel traced — with adaptive sampling, the first frame after a reset; later frames keep
+// them complete, since a stopped pixel keeps its AOVs — until a frame runs with them off.
+void note_frame_aovs(rt_ctx* c)
+{
+    if (!(aov_wanted(c) && c->aov_albedo)) c->aov_ready = false;
+    else if (!adaptive_on(c) || c->ad_fresh) c->aov_ready = true;
+    c->ad_fresh = false;
+}
 
 AovCam aov_cam(const RtCamera& cam)
 {
@@ -1287,6 +1372,7 @@ int ensure_aov_buffers(rt_ctx* c)
 {
     if (c->aov_albedo) return RT_OK;
     ++c->config_gen;
+    c->aov_ready = false;
     size_t n = c->n_local ? c->n_local : 1;
     RT_CUDA(c, cudaMalloc(&c->aov_albedo, n * 16)); RT_CUDA(c, cudaMalloc(&c->aov_depth, n * 4));
     RT_CUDA(c, cudaMalloc(&c->aov_normal, n * 16)); RT_CUDA(c, cudaMalloc(&c->aov_velocity, n * 8));
@@ -1303,6 +1389,7 @@ void free_aov_buffers(rt_ctx* c)
     cudaFree(c->prev_radiance); cudaFree(c->prev_depth);
     c->aov_albedo = nullptr; c->aov_depth = nullptr; c->aov_normal = nullptr; c->aov_velocity = nullptr;
     c->prev_radiance = nullptr; c->prev_depth = nullptr;
+    c->aov_ready = false;
 }   // 8 CTAs x 256 threads = full occupancy target per SM
 
 } // namespace
@@ -1387,6 +1474,8 @@ int rt_set_partition(rt_ctx* c, uint32_t rank, uint32_t world)
     if (world == 0 || rank >= world) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_partition: need rank < world, world >= 1");
     if (world > 1 && c->denoiser)
         RT_FAIL(c, RT_ERR_UNSUPPORTED, "the temporal denoiser reprojects across the whole image and is not available with a multi-GPU partition");
+    if (world > 1 && c->sd_iters)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "the spatial denoiser is not available with a multi-GPU partition (neighbouring rows live on other ranks)");
     RT_CUDA(c, cudaSetDevice(c->device));
     c->rank = rank; c->world = world;
     c->gather_slab = nullptr; c->gather_flag = nullptr;       // a gather target belongs to the partition it was set for
@@ -1648,6 +1737,31 @@ int rt_set_adaptive_sampling(rt_ctx* c, float max_error, uint32_t min_samples)
     return RT_OK;
 }
 
+int rt_set_spatial_denoiser(rt_ctx* c, uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth)
+{
+    RT_CHECK_CTX(c);
+    auto ok = [](float s) { return std::isfinite(s) && s >= 0.0f; };
+    if (iterations > 5 || !ok(sigma_color) || !ok(sigma_normal) || !ok(sigma_depth))
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_spatial_denoiser: need iterations <= 5 and finite sigmas >= 0");
+    if (iterations != 0 && !c->children.empty())
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "the spatial denoiser is not available on a multi-device context (neighbouring rows live on other devices)");
+    if (iterations != 0 && c->world != 1)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "the spatial denoiser is not available with a multi-GPU partition (neighbouring rows live on other ranks)");
+    RT_CUDA(c, cudaSetDevice(c->device));
+    if ((iterations != 0) != (c->sd_iters != 0)) ++c->config_gen;   // the frames produce the AOVs or stop doing so: re-capture
+    c->sd_iters = iterations;
+    c->sd_sigma_c = sigma_color; c->sd_sigma_n = sigma_normal; c->sd_sigma_z = sigma_depth;
+    if (iterations != 0) return ensure_aov_buffers(c);
+    if (c->sd_col[0] || c->sd_col[1] || c->sd_guide)
+    {   // the scratch planes exist only while the filter is on
+        if (c->copy_stream) RT_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+        RT_CUDA(c, cudaStreamSynchronize(c->stream));
+        cudaFree(c->sd_col[0]); cudaFree(c->sd_col[1]); cudaFree(c->sd_guide);
+        c->sd_col[0] = c->sd_col[1] = c->sd_guide = nullptr;
+    }
+    return RT_OK;
+}
+
 int rt_read_pixel_samples(rt_ctx* c, uint32_t* counts)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_read_pixel_samples(k, counts));
@@ -1701,6 +1815,7 @@ int rt_generate_rays(rt_ctx* c)
         ++c->launches;
     }
     k_raygen<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->q, c->counters, aov_params(c));
+    note_frame_aovs(c);
     c->frame_started = true;
     return post_launch(c, "k_raygen");
 }
@@ -1904,13 +2019,14 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
     if (c->overlap == 1 && (rc = ensure_shadow_stream(c))) return rc;      // created outside the capture
     const uint32_t saved_samples = c->sample_count, saved_bounce = c->cur_bounce;
     const uint64_t saved_launches = c->launches;
-    const bool saved_started = c->frame_started;
+    const bool saved_started = c->frame_started, saved_aov_ready = c->aov_ready, saved_ad_fresh = c->ad_fresh;
     RT_CUDA(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
     rc = integrate_body(c, max_bounces);
     cudaGraph_t graph = nullptr;
     cudaError_t e = cudaStreamEndCapture(c->stream, &graph);
     c->graph_launches = c->launches - saved_launches;
     c->sample_count = saved_samples; c->cur_bounce = saved_bounce; c->launches = saved_launches; c->frame_started = saved_started;
+    c->aov_ready = saved_aov_ready; c->ad_fresh = saved_ad_fresh;
     c->shadow_pending = false; c->shadow_deferred = false;
     if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
     if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
@@ -2016,6 +2132,7 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
         return RT_OK;
     });
     if (rc || (rc = post_launch(c, "k_frame"))) return rc;
+    note_frame_aovs(c);
     if (adaptive_on(c) && (rc = launch_adaptive_update(c))) return rc;
     c->frame_started = true; c->cur_bounce = max_bounces;
     ++c->sample_count;
@@ -2040,6 +2157,7 @@ static int integrate_regen_kernel(rt_ctx* c, uint32_t max_bounces, uint32_t n_sa
         return RT_OK;
     });
     if (rc || (rc = post_launch(c, "k_frame_regen"))) return rc;
+    note_frame_aovs(c);
     c->frame_started = true; c->cur_bounce = max_bounces;
     c->sample_count += n_samples;
     return RT_OK;
@@ -2066,6 +2184,7 @@ static int integrate_frame(rt_ctx* c, uint32_t max_bounces, bool* pushed)
     kp.func = c->graph_set_frame_func; kp.gridDim = dim3(1); kp.blockDim = dim3(1); kp.sharedMemBytes = 0; kp.kernelParams = args; kp.extra = nullptr;
     RT_CUDA(c, cudaGraphExecKernelNodeSetParams(c->graph_exec, c->graph_set_frame_node, &kp));
     RT_CUDA(c, cudaGraphLaunch(c->graph_exec, c->stream));
+    note_frame_aovs(c);
     c->launches += c->graph_launches;
     c->frame_started = true; c->cur_bounce = max_bounces;
     ++c->sample_count;
@@ -2149,13 +2268,46 @@ int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
 }
 
 // the resolve kernel of this context's rows into `out`, on its stream
+// With the spatial denoiser on and the shaded-colour view, k_resolve writes into a scratch plane, a pack kernel gathers the guides,
+// and the passes ping-pong between the scratch planes; the last pass writes `out`.  Every launch counts under RT_K_RESOLVE.
 static int launch_resolve(rt_ctx* c, float4* out)
 {
-    TimedLaunch t(c, RT_K_RESOLVE);
     const AovParams ap = aov_params(c);
-    k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, out, c->n_local, c->sample_count, c->denoiser, ap.enabled ? c->aov : 0, ap,
-                                                           adaptive_on(c) ? c->ad.count : nullptr);
-    return post_launch(c, "k_resolve");
+    const int view = ap.enabled ? c->aov : 0;
+    const bool filter = c->sd_iters != 0 && view == 0;
+    if (filter)
+    {
+        if (!c->aov_ready)
+            RT_FAIL(c, RT_ERR_NOT_READY, "the spatial denoiser needs the AOVs of a frame rendered with it on: render a frame first");
+        const size_t n = std::max(c->n_local, 1u);
+        for (float4** p : { &c->sd_col[0], &c->sd_col[1], &c->sd_guide })
+            if (!*p) RT_CUDA(c, cudaMalloc(p, n * 16));
+    }
+    {
+        TimedLaunch t(c, RT_K_RESOLVE);
+        k_resolve<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, filter ? c->sd_col[0] : out, c->n_local, c->sample_count, c->denoiser,
+                                                               view, ap, adaptive_on(c) ? c->ad.count : nullptr);
+        int rc = post_launch(c, "k_resolve"); if (rc) return rc;
+    }
+    if (!filter) return RT_OK;
+    {
+        TimedLaunch t(c, RT_K_RESOLVE);
+        k_sd_pack<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->aov_normal, c->aov_depth, c->sd_guide, c->n_local);
+        int rc = post_launch(c, "k_sd_pack"); if (rc) return rc;
+    }
+    const float kc = c->sd_sigma_c > 0.0f ? 1.0f / (c->sd_sigma_c * c->sd_sigma_c) : 0.0f;
+    const float kn = c->sd_sigma_n > 0.0f ? 1.0f / (c->sd_sigma_n * c->sd_sigma_n) : 0.0f;
+    const dim3 block(32, 8), grid((c->width + 31u) / 32u, (c->local_rows + 7u) / 8u);
+    for (uint32_t i = 0; i < c->sd_iters; ++i)
+    {
+        const float4* src = c->sd_col[i & 1u];
+        float4* dst = (i + 1 == c->sd_iters) ? out : c->sd_col[(i + 1) & 1u];
+        TimedLaunch t(c, RT_K_RESOLVE);
+        if (c->local_rows)
+            k_sd_pass<<<grid, block, 0, c->stream>>>(src, dst, c->sd_guide, c->width, c->local_rows, 1 << i, kc * (float)(1u << i), kn, c->sd_sigma_z);
+        int rc = post_launch(c, "k_sd_pass"); if (rc) return rc;
+    }
+    return RT_OK;
 }
 
 // the pipelined read-back's copy stream and its events
@@ -2259,6 +2411,7 @@ static int resolve_gathered_impl(rt_ctx* c, const void* slabs, uint64_t stride_b
         RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_resolve_gathered: slab stride must be a multiple of 16 and hold %zu rows", rows_max);
     if (c->aov != 0 || c->denoiser) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_resolve_gathered resolves the shaded colour only (AOV views and the denoiser are single-GPU)");
     if (adaptive_wanted(c)) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_resolve_gathered divides by one sample count: not available with adaptive sampling");
+    if (c->sd_iters) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_resolve_gathered has no guides of other ranks: not available with the spatial denoiser");
     RT_CUDA(c, cudaSetDevice(c->device));
     const size_t n = (size_t)c->width * c->height;
     int k = 0;
@@ -2680,7 +2833,7 @@ int rt_gather_wait(rt_ctx* c)
  * fn: 0 sin 1 cos 2 tan 3 atan2(a, b) 4 acos 5 pow(a, b) 6 fmin 7 fmax 8 1/sqrt(a) 9 a / b. */
 int rt_math_eval(int device, int fn, const float* a, const float* b, float* out, uint64_t n)
 {
-    if (!a || !b || !out || fn < 0 || fn > 9) return RT_ERR_INVALID_ARGUMENT;
+    if (!a || !b || !out || fn < 0 || fn > 10) return RT_ERR_INVALID_ARGUMENT;
     if (n == 0) return RT_OK;
     if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); g_create_error = "rt_math_eval: no such CUDA device"; return RT_ERR_NO_DEVICE; }
     float *da = nullptr, *db = nullptr, *dout = nullptr;

@@ -130,6 +130,11 @@ void CUDAPathTraceIntegrator::SetAdaptiveSampling(float max_error, std::uint32_t
     RequestReset();
 }
 
+void CUDAPathTraceIntegrator::SetSpatialDenoiser(std::uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth)
+{
+    Check(rt_set_spatial_denoiser(ctx_, iterations, sigma_color, sigma_normal, sigma_depth), "SetSpatialDenoiser");
+}
+
 std::uint32_t CUDAPathTraceIntegrator::ActivePixels() const
 {
     std::uint32_t n = 0;

@@ -25,6 +25,7 @@
  * Integrate()'s and the denoiser (it runs once per sample) throw std::runtime_error.
  * SetAdaptiveSampling(max_error, min_samples): pixels stop tracing once they have settled (include/rt_b200.h); ActivePixels() tells
  * a progressive loop when every pixel has.
+ * SetSpatialDenoiser(iterations, sigmas): ResolveRadiance() filters the shaded colour (include/rt_b200.h states the rule).
  * AOVs (ComputeAOVs) are produced inside the bounce-0 shading pass, and only when SetAOV selected a view other than
  * the shaded colour or the denoiser is on.  SetSamplerType(kBlueNoise) needs the sampler's three tables first
  * (SetBlueNoiseTables; the OpenCL backend reads them from utils/blue_noise_sampler.hpp, cl_pt_integrator.cpp:222-235).
@@ -78,6 +79,9 @@ public:
     std::uint32_t ActivePixels() const;
     // every pixel's sample count, width*height entries; blocks
     void ReadPixelSamples(std::uint32_t* counts) const;
+    // spatial denoiser (rt_set_spatial_denoiser): an edge-avoiding a-trous filter on the resolved shaded colour, guided by the
+    // bounce-0 normal and depth; iterations 0 turns it off.  No reset: the accumulation is unaffected.
+    void SetSpatialDenoiser(std::uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

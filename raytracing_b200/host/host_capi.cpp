@@ -186,6 +186,11 @@ int rth_render_set_adaptive_sampling(void* h, float max_error, std::uint32_t min
 {
     try { ((RenderHandle*)h)->render->SetAdaptiveSampling(max_error, min_samples); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_spatial_denoiser(void* h, std::uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth)
+{
+    try { ((RenderHandle*)h)->render->SetSpatialDenoiser(iterations, sigma_color, sigma_normal, sigma_depth); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_active_pixels(void* h, std::uint32_t* n)
 {
     try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

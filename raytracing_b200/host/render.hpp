@@ -43,6 +43,11 @@ public:
     void SetSamplesPerFrame(std::uint32_t n) { Cuda().SetSamplesPerFrame(n); }
     // adaptive sampling (CUDAPathTraceIntegrator::SetAdaptiveSampling): applies from the next RenderFrame(), which starts over
     void SetAdaptiveSampling(float max_error, std::uint32_t min_samples) { Cuda().SetAdaptiveSampling(max_error, min_samples); }
+    // spatial denoiser (CUDAPathTraceIntegrator::SetSpatialDenoiser): filters the image of every later RenderFrame()
+    void SetSpatialDenoiser(std::uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth)
+    {
+        Cuda().SetSpatialDenoiser(iterations, sigma_color, sigma_normal, sigma_depth);
+    }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

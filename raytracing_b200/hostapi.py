@@ -44,6 +44,7 @@ def load_library():
     L.rth_render_set_max_bounces.argtypes = [C.c_void_p, C.c_uint32]
     L.rth_render_set_samples_per_frame.argtypes = [C.c_void_p, C.c_uint32]
     L.rth_render_set_adaptive_sampling.argtypes = [C.c_void_p, C.c_float, C.c_uint32]
+    L.rth_render_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
@@ -214,6 +215,11 @@ class HostRender:
     def set_adaptive_sampling(self, max_error, min_samples=2):
         """Render::SetAdaptiveSampling: pixels stop tracing once they have settled; applies from the next render_frame()."""
         if self.L.rth_render_set_adaptive_sampling(self.h, float(max_error), int(min_samples)) != 0:
+            raise _err(self.L)
+
+    def set_spatial_denoiser(self, iterations, sigma_color=0.0, sigma_normal=0.0, sigma_depth=0.0):
+        """Render::SetSpatialDenoiser: edge-avoiding a-trous filter (0 = off .. 5 passes) on the image of every later render_frame()."""
+        if self.L.rth_render_set_spatial_denoiser(self.h, int(iterations), float(sigma_color), float(sigma_normal), float(sigma_depth)) != 0:
             raise _err(self.L)
 
     def active_pixels(self):
