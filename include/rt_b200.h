@@ -52,7 +52,7 @@ typedef struct RtSceneDesc {
     const RtLight* lights;              uint64_t n_lights;         /* >= 1 (light.h:46 divides by the count) */
     const RtTexture* textures;          uint64_t n_textures;
     const uint32_t* texture_data;       uint64_t n_texture_data;
-    const uint32_t* emissive_indices;   uint64_t n_emissive;       /* uploaded, never sampled (light.h:30-65) */
+    const uint32_t* emissive_indices;   uint64_t n_emissive;       /* triangle ids; sampled only with RT_OPT_EMITTER_SAMPLING 1 */
     const float* env_image;             uint32_t env_width, env_height;   /* RGBA32F rows, first row = v 0 */
     RtSceneInfo scene_info;
 } RtSceneDesc;
@@ -93,9 +93,12 @@ typedef enum RtOption {
     RT_OPT_PRESENT = 27,        /* multi-device contexts, rt_resolve: 0 (default) parallel read-back of every device's rows,
                                    1 gather to devices[0] over NVLink, resolve and read back there */
     RT_OPT_FRAME_THREADS = 28,  /* threads per CTA of the one-kernel frame: 0 (default) by partition size, else a multiple of 32 <= 1024 */
-    RT_OPT_TOP_SMEM = 29        /* scenes whose traversal records do not fit shared memory: number of top-of-tree interior records
+    RT_OPT_TOP_SMEM = 29,       /* scenes whose traversal records do not fit shared memory: number of top-of-tree interior records
                                    (breadth-first, 64 B each, <= 640 = 40 KB) that every traversal CTA stages with one TMA bulk copy;
                                    0 (default) = none.  Results are bit-identical */
+    RT_OPT_EMITTER_SAMPLING = 30 /* 0 (default): emissive triangles add light only when a BSDF-sampled ray hits them; 1: next-event
+                                   estimation on the emissive triangles too, combined with BSDF sampling by MIS (the rule is stated
+                                   in the emitter-sampling block below; the image converges to the same expectation) */
 } RtOption;
 
 #define RT_MAX_BOUNCES 255u     /* bounce index range supported per frame (reference GUI: 0..5) */
@@ -303,6 +306,40 @@ int rt_read_active_pixels(rt_ctx* ctx, uint32_t* n_active);
  * RT_K_RESOLVE.  RT_ERR_INVALID_ARGUMENT: iterations > 5, a negative or non-finite sigma.  RT_ERR_UNSUPPORTED, whichever call comes
  * second: a multi-device context, rt_set_partition with world > 1, and rt_resolve_gathered[_async]. */
 int rt_set_spatial_denoiser(rt_ctx* ctx, uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth);
+
+/* ---- emitter sampling (new capability): rt_set_option(ctx, RT_OPT_EMITTER_SAMPLING, 1) ------------------------------------
+ * Next-event estimation on the emissive triangles, combined with BSDF sampling by multiple importance sampling (power heuristic).
+ * The estimator has the expectation of the option off; only the noise changes.  All float, no contraction, in the order written.
+ * Emitter table (raytracing_b200/csrc/rt_emitters.h), a pure function of the upload: the emitters are emissive_indices (leaf-ordered
+ * triangle ids, upload order); A_t = 0.5f * sqrtf((cx*cx + cy*cy) + cz*cz), c = cross(p2 - p1, p3 - p1); w_t = A_t * luma(E_t), E_t the
+ * material's constant emission, luma = (r*0.299f + g*0.587f) + b*0.114f, non-finite or negative w_t -> 0; cdf[i] = S_i / S_n (running
+ * float sum in list order), cdf[n-1] = 1; pmf_i = cdf[i] - cdf[i-1]; pdfA[t] = (P_e * pmf_i) / A_t where pmf_i > 0, else 0 (and 0 off
+ * the list).  P_e = 0 if S_n is not finite and > 0 or in white-furnace mode (the frame is then bit-identical to the option off);
+ * 1 if every analytic light has zero radiance; else 0.5.
+ * At a hit of bounce b < max_bounces (the last max_bounces passed to rt_integrate / rt_integrate_samples; the stepwise steps, which
+ * are not told max_bounces, use the value of the most recent such call, RT_MAX_BOUNCES before any), with kRandom draws r_k = hash(dimension 0x10000 + 4*b + k) whatever
+ * the sampler:
+ *     emitter iff P_e == 1 or r_0 < P_e;  else the analytic light sample of the option off, divided by (1 - P_e)
+ *     emitter: i = first entry with cdf[i] > min(r_1, 0x1.fffffep-1), t = list[i]; s = sqrtf(r_2);
+ *              y = (p1*(1-s) + p2*(s*(1-r_3))) + p3*(s*r_3); Le = emission of t's material at the same barycentrics' uv;
+ *              o = position + geometry_normal * EPS; v = y - o; d2 = dot(v, v); d = sqrtf(d2); w = normalize(v);
+ *              cos_e = -dot(w, n_t) (geometric normal of t); nothing if cos_e <= 0;  p_l = pdfA[t] * d2 / cos_e;
+ *              g, p_b = the BSDF that sample_bxdf integrates and its non-delta lobe density for w (rt_device.cuh bxdf_eval_sampled;
+ *              0 for pass-through materials, no specular term for alpha <= 1e-4 or where the specular sampler has no density:
+ *              n.h <= 0 or h.o <= 0, h = normalize(i + w));
+ *              sample = ((T * g) * Le) * (mis(p_l, p_b) / p_l), mis(p, q) = 1 / (1 + (q/p)^2) (NaN -> 0); shadow ray from o along w,
+ *              t_max = 0.999f * d, spawned iff p_l > 0 and dot(sample, sample) > 0
+ *     the continuation ray carries p_b of its direction (0 after a delta lobe: a pass-through or an alpha <= 1e-4 specular sample)
+ * At a BSDF hit of an emitter with carried p_b > 0 and pdfA[prim] > 0: emission * mis(p_b, p_l), p_l = pdfA[prim] * dot(x - o, x - o) /
+ * -dot(dir, n_prim) (x the hit, o the ray's origin); otherwise the emission of the option off.  At b = max_bounces nothing changes.
+ * With the option on, an emissive index >= n_triangles or listed twice is RT_ERR_INVALID_ARGUMENT (at rt_upload_scene, or at
+ * rt_set_option when the scene is already uploaded); values other than 0 and 1 too.  The setting applies from the next frame and keeps
+ * the accumulation.  Stepwise callers: a frame driven through the step calls samples emitters at every bounce below that value, so
+ * a caller whose last step bounce is below it gets emitter light from its last vertex, which BSDF sampling never adds (its
+ * continuation is not traced): its image converges to a brighter value than with the option off.  Call rt_integrate (or
+ * rt_integrate_samples) with the same max_bounces once before driving the steps.
+ * Device memory: 4 B per triangle and 8 B per emitter while it is on.  rt_integrate_samples runs n frames of
+ * rt_integrate's schedule with it on (the regenerating kernel keeps its path state where the carried p_b goes). */
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

@@ -19,6 +19,7 @@ OPT_WHITE_FURNACE, OPT_SAMPLER, OPT_AOV, OPT_DENOISER = 0, 1, 2, 3
 BN_SOBOL_COUNT, BN_TILE_COUNT = 65536, 131072
 OPT_COUNT_TRAVERSAL, OPT_KERNEL_TIMING, OPT_TRAVERSAL = 16, 17, 18
 OPT_AOV_ALWAYS, OPT_SMEM_BVH, OPT_OVERLAP, OPT_GRAPH, OPT_PDL, OPT_FRAME_KERNEL, OPT_PRESENT, OPT_FRAME_THREADS, OPT_TOP_SMEM = 21, 22, 23, 24, 25, 26, 27, 28, 29
+OPT_EMITTER_SAMPLING = 30       # 1: next-event estimation on the emissive triangles, MIS with BSDF sampling (include/rt_b200.h)
 KERNEL_CLASSES = ["raygen", "intersect", "miss", "hit", "intersect_shadow", "accumulate", "extend_shade",
                   "shadow_accumulate", "resolve", "aov", "misc", "trace_closest", "shade_queues", "trace_both"]
 

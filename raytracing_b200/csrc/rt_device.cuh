@@ -147,6 +147,12 @@ struct DevScene
     uint32_t top_n;                // interior records [0, top_n) are the top of the tree in breadth-first order
     uint32_t top_k;                // of those, the records a kernel staged into shared memory (set per launch; 0 = none)
     int root_ref;
+    // emitter sampling (RT_OPT_EMITTER_SAMPLING, rt_emitters.h): nullptr / 0 while it is off or inactive (P_e = 0)
+    const float* emit_pdfA;        // per triangle
+    const float* emit_cdf;         // per emitter
+    const uint32_t* emit_list;     // per emitter: triangle id
+    uint32_t n_emit;
+    float emit_pe;
 };
 
 // ---------------------------------------------------------------------------- environment
@@ -367,6 +373,56 @@ __device__ __forceinline__ f3 sample_bxdf(float s1, f2 s, Material m, f3 normal,
         pdf *= diffuse_pdf;
     }
     return bxdf;
+}
+
+// Emitter sampling (include/rt_b200.h, RT_OPT_EMITTER_SAMPLING): the BSDF that sample_bxdf integrates, evaluated for a given
+// direction `o`, and the density p_b(o) of its non-delta lobes.  Same lobe weights as sample_bxdf:
+//   spec = alpha > 1e-4 and n.h > 0 and h.o > 0 ? (fresnel * (D * G)) * max(n.o, 0) : 0,  h = normalize(i + o), D = ggx_d(alpha, n.h),
+//          G = v_smith(n.i, n.o, alpha)
+//   diff = ((1 - fresnel) * (diffuse_albedo / pi)) * max(n.o, 0);   g = spec + diff;   0 for pass-through materials
+//   p_b  = (n.h > 0 and h.o > 0 ? specular_pdf * (D * n.h / (4 * h.o)) : 0) + diffuse_pdf * (max(n.o, 0) * (1 / pi))
+// The specular terms are 0 when alpha <= 1e-4 (a delta lobe, left to BSDF sampling).  `spec_pdf` and `alpha` let the caller tell
+// whether the lobe sample_bxdf picked with s1 was a delta.
+__device__ __forceinline__ f3 bxdf_eval_sampled(const Material& m, f3 normal, f3 incoming, f3 o, float& p_b, float& spec_pdf, float& alpha)
+{
+    alpha = m.roughness * m.roughness;
+    float f0_dielectric = ior_to_f0(1.0f, m.ior);
+    f3 f0 = mix(splat(f0_dielectric), m.specular_albedo, m.metalness);
+    f3 diffuse_albedo = (1.0f - m.metalness) * m.diffuse_albedo;
+    f3 specular_albedo = mix(m.specular_albedo, splat(1.0f), m.metalness);
+    f3 fresnel = fresnel_schlick(f0, dot(normal, incoming)) * specular_albedo;
+    float specular_weight = luma(specular_albedo * fresnel);
+    float diffuse_weight = luma(diffuse_albedo * (1.0f - fresnel));
+    float weight_sum = diffuse_weight + specular_weight;
+    spec_pdf = specular_weight / weight_sum;
+    float diffuse_pdf = diffuse_weight / weight_sum;
+    p_b = 0.0f;
+    if (m.transparency < 0.5f) return splat(0.0f);
+    const float cos_o = fmaxf(dot(o, normal), 0.0f);
+    f3 g = (1.0f - fresnel) * (diffuse_albedo * RT_INV_PI) * cos_o;
+    float ps = 0.0f;
+    if (alpha > 1e-4f)
+    {
+        f3 h = normalize(incoming + o);
+        float n_dot_h = dot(normal, h), h_dot_o = dot(h, o);
+        float D = ggx_d(alpha, n_dot_h);
+        if (n_dot_h > 0.0f && h_dot_o > 0.0f)
+        {   // the directions the specular sampler reaches with a positive density (it never continues a path elsewhere)
+            float G = v_smith_ggx_correlated(dot(normal, incoming), dot(normal, o), alpha);
+            g = fresnel * splat(D * G) * cos_o + g;
+            ps = spec_pdf * (D * n_dot_h / (4.0f * h_dot_o));
+        }
+    }
+    p_b = ps + diffuse_pdf * (cos_o * RT_INV_PI);
+    return g;
+}
+
+// MIS weight of a strategy with density `p` against one with density `q` (power heuristic, beta 2): 1 / (1 + (q/p)^2), NaN -> 0
+__device__ __forceinline__ float mis_power(float p, float q)
+{
+    float r = q / p;
+    float w = 1.0f / (1.0f + r * r);
+    return w == w ? w : 0.0f;
 }
 
 // kernels/common/light.h:30-65 followed by hit_surface.cl:122-123 (length + normalize of the direction).

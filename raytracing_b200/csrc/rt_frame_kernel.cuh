@@ -29,7 +29,7 @@ struct CtaFrame
     uint32_t n_src;                          // entries of the primary-ray source: local pixels, or active pixels (adaptive sampling)
 };
 
-template <int SMEM>
+template <int SMEM, bool EMIT = false>
 __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p, DevScene sc, int mode, Queues q, DevCounters* ctr, float4* radiance,
                                                               AovParams aov, uint32_t max_bounces, uint32_t slots_per_cta,
                                                               const __grid_constant__ FrameDyn dyn)
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                     float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                     if (hit) h = q.hitq[base + k];
                     uint32_t pixel;
-                    const bool ends = shade_hit_group(p, sc, aov, q, base, b, hit, h, __float_as_uint(h.w), radiance, &s.emit[in], &s.n_emissive, pixel);
+                    const bool ends = shade_hit_group<false, EMIT>(p, sc, aov, q, base, b, hit, h, __float_as_uint(h.w), radiance, &s.emit[in], &s.n_emissive, pixel);
                     if (p.gather)
                     {   // paths that end at this hit (no continuation ray): final once their shadow ray is accumulated in T(b+1)
                         const unsigned dmask = __ballot_sync(0xffffffffu, ends);
@@ -256,7 +256,7 @@ __device__ __forceinline__ bool shade_hit_regen(const FrameParams& p, const DevS
     {
         const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
         pixel = __float_as_uint(a.w); state = __float_as_uint(c.w); bounce = state & 0xFFu;
-        shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), __float_as_uint(h.z), h.x, h.y, state >> 8, so);
+        shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), 0.0f, __float_as_uint(h.z), h.x, h.y, state >> 8, so);
         li = local_index(p, pixel);
         if (so.emissive) add_radiance(radiance, li, so.emission_add);
     }

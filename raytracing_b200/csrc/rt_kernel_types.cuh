@@ -78,7 +78,9 @@ struct AovParams
 
 struct FrameDyn
 {
-    uint32_t sample_idx, pad[3];
+    uint32_t sample_idx;
+    uint32_t max_bounces;          // emitter sampling: the frame's last bounce, which samples analytic lights only
+    uint32_t pad[2];
     RayGenConsts raygen;
     AovCam cam, prev;
 };

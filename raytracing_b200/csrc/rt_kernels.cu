@@ -40,6 +40,7 @@
 #include "rt_b200.h"
 #include "rt_bvh_layout.h"
 #include "rt_device.cuh"
+#include "rt_emitters.h"
 
 using namespace rt;
 
@@ -76,6 +77,7 @@ struct ShadeOut
     f3 emission_add;
     f3 s_origin, s_dir, s_sample; float s_tmax;
     f3 n_origin, n_dir, n_throughput;
+    float n_pdf;                   // C.w of the continuation ray: its p_b with emitter sampling on, else 0
 };
 
 // kernels/cl/miss.cl:41-77: radiance += sky * throughput, for the ray in slot `slot` of ray queue `in`
@@ -88,9 +90,14 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
     if (p.gather) p.gather[li] = r;        // the path ends here: its pixel is final (its last shadow ray was accumulated a phase ago)
 }
 
-// kernels/cl/hit_surface.cl:30-186, for the path of sample p.dyn->sample_idx + sample_offset (a later sample of a multi-sample call)
+// kernels/cl/hit_surface.cl:30-186, for the path of sample p.dyn->sample_idx + sample_offset (a later sample of a multi-sample call).
+// prev_pdf: C.w of the ray (emitter sampling: p_b of its direction at the previous vertex, 0 for primary rays and after a delta lobe).
+// EMIT: the scene has an active emitter table (sc.emit_*, RT_OPT_EMITTER_SAMPLING); a template flag, so that the kernels without it
+// are the code of the option off.
+template <bool EMIT = false>
 __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
-                                          f3 ray_origin, f3 ray_dir, f3 hit_throughput, uint32_t prim, float u, float v, uint32_t sample_offset, ShadeOut& out)
+                                          f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
+                                          uint32_t sample_offset, ShadeOut& out)
 {
     f3 incoming = -ray_dir;
     uint32_t px = pxy & 0xFFFFu, py = pxy >> 16;
@@ -120,13 +127,78 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         aov.velocity[li] = make_float2(s0.x - s1.x, s0.y - s1.y);
     }
 
+    // emitter sampling (RT_OPT_EMITTER_SAMPLING): on at this vertex iff the scene has an active emitter table and the frame traces the
+    // continuation ray of this bounce
+    const bool emit_on = EMIT && bounce < p.dyn->max_bounces;
     out.emissive = false;
     if (!p.white_furnace && dot(material.emission, splat(1.0f)) > 0.0f)
     {
         out.emissive = true;
         out.emission_add = hit_throughput * material.emission;
+        if (EMIT && prev_pdf > 0.0f)
+        {   // BSDF sample of an emitter: weighted against the emitter strategy that could have produced this direction
+            const float pdfA = __ldg(sc.emit_pdfA + prim);
+            if (pdfA > 0.0f)
+            {
+                f3 dv = position - ray_origin;
+                float cos_e = -dot(ray_dir, geometry_normal);
+                float p_l = pdfA * dot(dv, dv) / cos_e;
+                out.emission_add = out.emission_add * mis_power(prev_pdf, p_l);
+            }
+        }
     }
     uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx + sample_offset);
+    out.spawn_shadow = false;
+    bool pick_emitter = false;
+    if (EMIT && emit_on)
+    {   // light kind: c < P_e (P_e is 1 or 0.5)
+        const float ck = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce);
+        pick_emitter = sc.emit_pe >= 1.0f || ck < sc.emit_pe;
+    }
+    if (pick_emitter)
+    {   // next-event estimation on an emissive triangle
+        float k1 = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce + 1u);
+        const float k2 = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce + 2u);
+        const float k3 = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce + 3u);
+        k1 = fminf(k1, 0.99999994f);
+        uint32_t lo = 0, hi = sc.n_emit - 1u;
+        while (lo < hi)
+        {   // first CDF entry above k1
+            const uint32_t mid = (lo + hi) >> 1;
+            if (__ldg(sc.emit_cdf + mid) > k1) hi = mid; else lo = mid + 1u;
+        }
+        const uint32_t t = __ldg(sc.emit_list + lo);
+        const float4* ep = sc.tri_shade + (size_t)t * 7;
+        float4 e0 = __ldg(ep), e1 = __ldg(ep + 1), e2 = __ldg(ep + 2), e3 = __ldg(ep + 3);
+        const float sq = sqrtf(k2);
+        const float b0 = 1.0f - sq, b1 = sq * (1.0f - k3), b2 = sq * k3;
+        f3 y = mk3(e0) * b0 + mk3(e1) * b1 + mk3(e2) * b2;
+        const uint32_t emtl = __float_as_uint(e0.w);
+        f2 euv; euv.x = 0.0f; euv.y = 0.0f;
+        if (__float_as_uint(__ldg(sc.mat_rec + (size_t)emtl * 4 + 3).y) != 0u)
+        {
+            float4 e4 = __ldg(ep + 4), e5 = __ldg(ep + 5), e6 = __ldg(ep + 6);
+            euv.x = e4.w * b0 + e6.x * b1 + e6.z * b2; euv.y = e5.w * b0 + e6.y * b1 + e6.w * b2;
+        }
+        const f3 le = load_material(sc, emtl, euv).emission;
+        const f3 o = position + geometry_normal * RT_EPS;
+        const f3 dv = y - o;
+        const float d2 = dot(dv, dv);
+        const float d = sqrtf(d2);
+        const f3 w = normalize(dv);
+        const float cos_e = -dot(w, mk3(e1.w, e2.w, e3.w));
+        if (cos_e > 0.0f)
+        {
+            const float p_l = __ldg(sc.emit_pdfA + t) * d2 / cos_e;
+            float p_b, spec_pdf, alpha;
+            const f3 g = bxdf_eval_sampled(material, normal, incoming, w, p_b, spec_pdf, alpha);
+            const f3 ls = hit_throughput * g * le * (mis_power(p_l, p_b) / p_l);
+            out.spawn_shadow = (p_l > 0.0f) && (dot(ls, ls) > 0.0f);
+            out.s_origin = o;
+            out.s_dir = w; out.s_tmax = 0.999f * d; out.s_sample = ls;
+        }
+    }
+    else
     {   // direct lighting (next-event estimation on analytic lights)
         float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx + sample_offset, bounce * 5u + SAMPLE_LIGHT)
                              : sample_random(pixel_seed, bounce, SAMPLE_LIGHT);
@@ -136,11 +208,11 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         // dot(sample, sample) > 0 (hit_surface.cl:127-129).  When max(n.l, 0) is 0 every component of the sample is
         // +-0 or NaN whatever the BRDF evaluates to, so the ray is never spawned: the BRDF evaluation is skipped then.
         const float cos_l = fmaxf(dot(outgoing, normal), 0.0f);
-        out.spawn_shadow = false;
         if (cos_l > 0.0f)
         {
             f3 brdf = evaluate_material(material, normal, incoming, outgoing);
             f3 ls = light_radiance * hit_throughput * brdf / pdf * cos_l;
+            if (EMIT && emit_on) ls = ls / (1.0f - sc.emit_pe);
             out.spawn_shadow = (pdf > 0.0f) && (dot(ls, ls) > 0.0f);
             out.s_origin = position + normal * RT_EPS;
             out.s_dir = outgoing; out.s_tmax = distance_to_light; out.s_sample = ls;
@@ -169,6 +241,14 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         out.spawn_next = pdf > 0.0f;
         out.n_origin = position + geometry_normal * RT_EPS * offset;
         out.n_dir = outgoing;
+        out.n_pdf = 0.0f;
+        if (EMIT && emit_on)
+        {   // the continuation's p_b for the MIS weight of an emitter it hits (0 after a delta lobe)
+            float p_b, spec_pdf, alpha;
+            bxdf_eval_sampled(material, normal, incoming, outgoing, p_b, spec_pdf, alpha);
+            const bool delta = material.transparency < 0.5f || (s1 <= spec_pdf && alpha <= 1e-4f);
+            out.n_pdf = delta ? 0.0f : p_b;
+        }
     }
 }
 
@@ -265,7 +345,7 @@ __device__ __forceinline__ uint32_t ray_key(f3 o, f3 d, float4 mid)
 // of both queues (shadow rays in the low word, continuation rays in the high).  With STAGE the continuation rays go to the CTA's
 // staging area `st` instead (flush_continuations writes them out and counts them) and the atomic reserves shadow-ray slots only.
 // Returns whether the lane's path ends at this hit (no continuation ray); `pixel` is the packed pixel of the ray.
-template <bool STAGE = false>
+template <bool STAGE = false, bool EMIT = false>
 __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevScene& sc, const AovParams& aov, const Queues& q, uint32_t base, uint32_t bounce,
                                                 bool hit, float4 h, uint32_t i, float4* radiance, unsigned long long* emit, uint32_t* n_emissive, uint32_t& pixel,
                                                 ContStage* st = nullptr)
@@ -278,7 +358,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
     {
         const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
         pixel = __float_as_uint(a.w);
-        shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), __float_as_uint(h.z), h.x, h.y, 0u, so);
+        shade_hit<EMIT>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, 0u, so);
         if (so.emissive) add_radiance(radiance, local_index(p, pixel), so.emission_add);
     }
     const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
@@ -316,7 +396,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
         {
             st->A[j] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
             st->B[j] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
-            st->C[j] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, 0.0f);
+            st->C[j] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, so.n_pdf);
             const uint32_t key = ray_key(so.n_origin, so.n_dir, st->mid);
             st->key[j] = (uint8_t)key;
             atomicAdd(&st->count[key], 1u);
@@ -327,7 +407,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
         const uint32_t ni = base + (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
         q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
         q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
-        q.C[out][ni] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, 0.0f);
+        q.C[out][ni] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, so.n_pdf);
     }
     return hit && !so.spawn_next;
 }
@@ -384,6 +464,7 @@ __global__ void __launch_bounds__(256) k_shade_miss(FrameParams p, DevScene sc, 
 }
 
 // ShadeSurfaceHits (stepwise)
+template <bool EMIT>
 __global__ void __launch_bounds__(256) k_shade_hits(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce, AovParams aov)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -396,7 +477,7 @@ __global__ void __launch_bounds__(256) k_shade_hits(FrameParams p, DevScene sc, 
         hit = __float_as_uint(h.z) != RT_INVALID_ID;
     }
     uint32_t pixel;
-    shade_hit_group(p, sc, aov, q, 0, bounce, hit, h, i, radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
+    shade_hit_group<false, EMIT>(p, sc, aov, q, 0, bounce, hit, h, i, radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
 }
 
 // IntersectShadowRays (stepwise): any-hit -> flags (0 = occluded, INVALID_ID = unoccluded)
@@ -540,7 +621,7 @@ __device__ __forceinline__ void flush_continuations(ContStage& st, const Queues&
 // cursor add each, so that their continuation rays leave sorted by ray_key (flush_continuations); the batch shrinks towards 256
 // entries when there are fewer than 4 full batches per CTA, so that the CTAs still finish together.  Misses past the last hit
 // batch are taken 32 at a time by each warp.
-template <bool SORT>
+template <bool SORT, bool EMIT = false>
 __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce,
                                                                      AovParams aov, float4 scene_mid)
 {
@@ -563,7 +644,7 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                 if (hit) h = q.hitq[k];
                 uint32_t pixel;
-                shade_hit_group(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
+                shade_hit_group<false, EMIT>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
             }
             else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
         }
@@ -588,7 +669,7 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                 if (hit) h = q.hitq[k];
                 uint32_t pixel;
-                shade_hit_group<true>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
+                shade_hit_group<true, EMIT>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
             }
             else if (g - hit_span + lane < n_miss) shade_miss(sc, p, q, in, q.missq[g - hit_span + lane], radiance);
         }
@@ -1015,6 +1096,17 @@ struct rt_ctx
     AdaptiveState ad = {};
     bool ad_fresh = false;                         // no frame has run since the adaptive state was reset (every local pixel traces the next)
 
+    // emitter sampling (RT_OPT_EMITTER_SAMPLING): the upload's emitter list and what the table needs of it (kept so that the option can be
+    // turned on after the upload), the device table (scene.emit_*, allocated while the option is on and P_e > 0)
+    int emitter_sampling = 0;
+    uint32_t emit_max_bounces = RT_MAX_BOUNCES;    // FrameDyn::max_bounces: the max_bounces of the last rt_integrate[_samples] call
+    std::vector<uint32_t> emit_idx;
+    std::vector<RtTriangle> emit_tris;             // emit_tris[i]: triangle emit_idx[i] (zero where the index is out of range)
+    std::vector<RtPackedMaterial> emit_mats;
+    std::vector<RtLight> emit_lights;
+    uint64_t emit_n_tris = 0;
+    std::vector<void*> emit_allocs;
+
     // spatial denoiser (rt_set_spatial_denoiser): passes (0 = off), sigmas, scratch planes (allocated while it is on)
     uint32_t sd_iters = 0;
     float sd_sigma_c = 0.0f, sd_sigma_n = 0.0f, sd_sigma_z = 0.0f;
@@ -1330,7 +1422,7 @@ FrameDyn frame_dyn(const rt_ctx* c)
 {
     FrameDyn dyn;
     memset(&dyn, 0, sizeof(dyn));
-    dyn.sample_idx = c->sample_count; dyn.raygen = c->raygen;
+    dyn.sample_idx = c->sample_count; dyn.max_bounces = c->emit_max_bounces; dyn.raygen = c->raygen;
     dyn.cam = aov_cam(c->camera); dyn.prev = aov_cam(c->aov_prev_camera);
     return dyn;
 }
@@ -1420,7 +1512,8 @@ int rt_create(uint32_t width, uint32_t height, int device, rt_ctx** out_ctx)
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail("cudaGetDeviceProperties", e);
     c->num_sms = prop.multiProcessorCount;
-    if ((e = cudaFuncSetAttribute(k_shade_queues<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess)
+    if ((e = cudaFuncSetAttribute(k_shade_queues<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess ||
+        (e = cudaFuncSetAttribute(k_shade_queues<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess)
         return fail("cudaFuncSetAttribute(k_shade_queues)", e);
     if ((e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
     if ((e = cudaMalloc(&c->counters, sizeof(DevCounters))) != cudaSuccess) return fail("cudaMalloc(counters)", e);
@@ -1459,6 +1552,7 @@ int rt_destroy(rt_ctx* c)
     for (int i = 0; i < 2; ++i) { if (c->resolve_done[i]) cudaEventDestroy(c->resolve_done[i]); if (c->copy_done[i]) cudaEventDestroy(c->copy_done[i]); }
     if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
     cudaFree(c->own_gather);
+    for (void* p : c->emit_allocs) cudaFree(p);
     for (void* p : c->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void* p : c->scene_allocs) cudaFree(p);
     for (auto& t : c->timed) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
@@ -1480,6 +1574,40 @@ int rt_set_partition(rt_ctx* c, uint32_t rank, uint32_t world)
     c->rank = rank; c->world = world;
     c->gather_slab = nullptr; c->gather_flag = nullptr;       // a gather target belongs to the partition it was set for
     return alloc_frame_buffers(c);
+}
+
+// (Re)builds the device emitter table from the kept upload data: rt_emitters.h.  Inactive (no table, scene.emit_* null) while the
+// option is off, before an upload, in white-furnace mode and when no emitter can be selected; the frames are then those of the
+// option off.  The caller has validated the indices.
+static int refresh_emitters(rt_ctx* c)
+{
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));     // a frame in flight may still read the old table
+    for (void* p : c->emit_allocs) cudaFree(p);
+    c->emit_allocs.clear();
+    DevScene& ds = c->scene;
+    ds.emit_pdfA = nullptr; ds.emit_cdf = nullptr; ds.emit_list = nullptr; ds.n_emit = 0; ds.emit_pe = 0.0f;
+    ++c->config_gen;
+    if (!c->emitter_sampling || !c->scene_ready) return RT_OK;
+    rtemit::Table t;
+    rtemit::build([&](uint64_t i) -> const RtTriangle& { return c->emit_tris[i]; }, c->emit_idx.data(), c->emit_idx.size(), c->emit_n_tris,
+                  c->emit_mats.data(), c->emit_lights.data(), ds.light_count, c->white_furnace != 0, t);
+    if (t.p_e == 0.0f) return RT_OK;
+    auto upload = [&](const void* src, size_t bytes, const void** dst) -> int {
+        void* d = nullptr;
+        RT_CUDA(c, cudaMalloc(&d, bytes));
+        c->emit_allocs.push_back(d);
+        RT_CUDA(c, cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
+        *dst = d;
+        return RT_OK;
+    };
+    int rc;
+    if ((rc = upload(t.pdfA.data(), t.pdfA.size() * 4, (const void**)&ds.emit_pdfA))) return rc;
+    if ((rc = upload(t.cdf.data(), t.cdf.size() * 4, (const void**)&ds.emit_cdf))) return rc;
+    if ((rc = upload(t.list.data(), t.list.size() * 4, (const void**)&ds.emit_list))) return rc;
+    ds.n_emit = (uint32_t)t.list.size(); ds.emit_pe = t.p_e;
+    return RT_OK;
 }
 
 int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
@@ -1512,6 +1640,14 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
         if (t.width <= 0 || t.height <= 0 || t.data_start < 0 || (uint64_t)t.data_start + (uint64_t)t.width * t.height > s->n_texture_data)
             RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: texture %llu lies outside the texel array", (unsigned long long)i);
     }
+    if (c->emitter_sampling)
+    {
+        if (s->n_emissive && !s->emissive_indices)
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: emitter sampling is on and n_emissive > 0 with no emissive_indices");
+        std::string err;
+        if (!rtemit::check_indices(s->emissive_indices, s->n_emissive, s->n_triangles, err))
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: emitter sampling is on and %s", err.c_str());
+    }
 
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = join_shadow(c); if (rc) return rc; }     // a shadow pass of an unfinished frame may still read the old scene
@@ -1519,6 +1655,9 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     for (void* p : c->scene_allocs) cudaFree(p);
     c->scene_allocs.clear();
     c->scene_ready = false;
+    for (void* p : c->emit_allocs) cudaFree(p);
+    c->emit_allocs.clear();
+    c->scene.emit_pdfA = nullptr; c->scene.emit_cdf = nullptr; c->scene.emit_list = nullptr; c->scene.n_emit = 0; c->scene.emit_pe = 0.0f;
 
     auto upload = [&](const void* src, size_t bytes, const void** dst) -> int {
         void* d = nullptr;
@@ -1569,9 +1708,19 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     const RtLinearBVHNode& root = s->nodes[0];
     c->scene_mid = make_float4((root.bounds_min.x + root.bounds_max.x) * 0.5f, (root.bounds_min.y + root.bounds_max.y) * 0.5f,
                                (root.bounds_min.z + root.bounds_max.z) * 0.5f, 0.0f);
+    // what the emitter table needs is kept only for a scene that lists emitters (a list with a null pointer counts as empty: with
+    // the option off the array was never read, and such uploads stay accepted)
+    const uint64_t n_emit = s->emissive_indices ? s->n_emissive : 0;
+    c->emit_idx.assign(s->emissive_indices, s->emissive_indices + n_emit);
+    c->emit_tris.assign(n_emit, RtTriangle{});
+    for (uint64_t i = 0; i < n_emit; ++i)
+        if (s->emissive_indices[i] < s->n_triangles) c->emit_tris[i] = s->triangles[s->emissive_indices[i]];
+    if (n_emit) { c->emit_mats.assign(s->materials, s->materials + s->n_materials); c->emit_lights.assign(s->lights, s->lights + s->n_lights); }
+    else { c->emit_mats.clear(); c->emit_lights.clear(); }
+    c->emit_n_tris = s->n_triangles;
     c->scene_ready = true;
     ++c->config_gen;
-    return RT_OK;
+    return refresh_emitters(c);
 }
 
 int rt_set_camera(rt_ctx* c, const RtCamera* cam)
@@ -1620,7 +1769,21 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
     ++c->config_gen;
     switch (key)
     {
-    case RT_OPT_WHITE_FURNACE: c->white_furnace = value != 0; return RT_OK;
+    case RT_OPT_WHITE_FURNACE:
+        if ((value != 0) == (c->white_furnace != 0)) return RT_OK;
+        c->white_furnace = value != 0;
+        return c->emitter_sampling ? refresh_emitters(c) : RT_OK;
+    case RT_OPT_EMITTER_SAMPLING:
+        if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "emitter sampling must be 0 (off) or 1 (emissive triangles with MIS)");
+        if (value == 1 && c->scene_ready)
+        {
+            std::string err;
+            if (!rtemit::check_indices(c->emit_idx.data(), c->emit_idx.size(), c->emit_n_tris, err))
+                RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "emitter sampling: the uploaded scene's %s", err.c_str());
+        }
+        if ((int)value == c->emitter_sampling) return RT_OK;
+        c->emitter_sampling = (int)value;
+        return refresh_emitters(c);
     case RT_OPT_SAMPLER:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "sampler type must be 0 (kRandom) or 1 (kBlueNoise)");
         if (value == 1 && !c->d_bn)
@@ -1867,7 +2030,7 @@ int rt_shade_hits(rt_ctx* c, uint32_t bounce)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     c->cur_bounce = bounce;
     TimedLaunch t(c, RT_K_HIT);
-    k_shade_hits<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
+    (c->scene.emit_pdfA ? k_shade_hits<true> : k_shade_hits<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
     return post_launch(c, "k_shade_hits");
 }
 
@@ -1942,7 +2105,8 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     { int rc = join_shadow(c); if (rc) return rc; }     // the shading pass accumulates into radiance and refills the shadow queue
     TimedLaunch t(c, RT_K_SHADE_QUEUES);
     const bool sort = sorted_shading(c);
-    auto* k = sort ? k_shade_queues<true> : k_shade_queues<false>;
+    auto* k = c->scene.emit_pdfA ? (sort ? k_shade_queues<true, true> : k_shade_queues<false, true>)
+                                 : (sort ? k_shade_queues<true> : k_shade_queues<false>);
     const size_t sm = sort ? sizeof(ContStage) : 0;
     launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
     return post_launch(c, "k_shade_queues");
@@ -2124,7 +2288,7 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
     FrameParams fp = frame_params(c);
     fp.gather = push ? c->gather_slab : nullptr;
     rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
-        auto* k = k_frame<smem.value>;
+        auto* k = c->scene.emit_pdfA ? k_frame<smem.value, true> : k_frame<smem.value>;
         uint32_t grid, slots_per_cta;
         int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
         TimedLaunch t(c, RT_K_MISC);
@@ -2196,6 +2360,7 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_integrate(k, max_bounces));
     if (max_bounces > RT_MAX_BOUNCES) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "max_bounces %u exceeds RT_MAX_BOUNCES", max_bounces);
     c->stats_summed = false;
+    c->emit_max_bounces = max_bounces;
     bool pushed = false;
     int rc = integrate_frame(c, max_bounces, &pushed); if (rc) return rc;
     return gather_signal(c, !pushed);
@@ -2205,7 +2370,7 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
 // Measured on one H100 80GB HBM3 at 700 W (tools/spp_probe.py, 1080p x 8, rank 0 of 1/2/4/8-way partitions, N = 8 and 64, DESIGN.md
 // section 4) it never clearly beats N one-kernel frames: it ties on CornellBox (-3 % to +4 %) and is 5-29 % slower on ShaderBalls,
 // so every partition size takes the N-frame path.  Adaptive sampling decides between samples, so it always takes the N-frame path.
-static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c) && !adaptive_on(c); }
+static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c) && !adaptive_on(c) && !c->emitter_sampling; }
 
 // A multi-sample call leaves its summed statistics in counters_sum, which only rt_read_frame_stats reads: the counters that the
 // taps (rt_read_rays, rt_read_hits) take their entry counts from never exceed one frame's rays.
@@ -2222,6 +2387,7 @@ int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
         RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_integrate_samples: the regenerating frame kernel (RT_OPT_FRAME_KERNEL 1) renders at most %u samples per call",
                 RT_MAX_REGEN_SAMPLES);
     if (n_samples == 1) return rt_integrate(c, max_bounces);
+    c->emit_max_bounces = max_bounces;
     int rc = require_ready(c); if (rc) return rc;
     if ((rc = join_shadow(c))) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));

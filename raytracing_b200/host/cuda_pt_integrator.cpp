@@ -135,6 +135,11 @@ void CUDAPathTraceIntegrator::SetSpatialDenoiser(std::uint32_t iterations, float
     Check(rt_set_spatial_denoiser(ctx_, iterations, sigma_color, sigma_normal, sigma_depth), "SetSpatialDenoiser");
 }
 
+void CUDAPathTraceIntegrator::SetEmitterSampling(bool on)
+{
+    Check(rt_set_option(ctx_, RT_OPT_EMITTER_SAMPLING, on ? 1u : 0u), "SetEmitterSampling");
+}
+
 std::uint32_t CUDAPathTraceIntegrator::ActivePixels() const
 {
     std::uint32_t n = 0;

@@ -26,6 +26,8 @@
  * SetAdaptiveSampling(max_error, min_samples): pixels stop tracing once they have settled (include/rt_b200.h); ActivePixels() tells
  * a progressive loop when every pixel has.
  * SetSpatialDenoiser(iterations, sigmas): ResolveRadiance() filters the shaded colour (include/rt_b200.h states the rule).
+ * SetEmitterSampling(on): next-event estimation on the emissive triangles as well, combined with BSDF sampling by MIS
+ * (RT_OPT_EMITTER_SAMPLING; the image converges to the same expectation, so the accumulation is kept).
  * AOVs (ComputeAOVs) are produced inside the bounce-0 shading pass, and only when SetAOV selected a view other than
  * the shaded colour or the denoiser is on.  SetSamplerType(kBlueNoise) needs the sampler's three tables first
  * (SetBlueNoiseTables; the OpenCL backend reads them from utils/blue_noise_sampler.hpp, cl_pt_integrator.cpp:222-235).
@@ -82,6 +84,9 @@ public:
     // spatial denoiser (rt_set_spatial_denoiser): an edge-avoiding a-trous filter on the resolved shaded colour, guided by the
     // bounce-0 normal and depth; iterations 0 turns it off.  No reset: the accumulation is unaffected.
     void SetSpatialDenoiser(std::uint32_t iterations, float sigma_color, float sigma_normal, float sigma_depth);
+    // emitter sampling (RT_OPT_EMITTER_SAMPLING): sample the emissive triangles at every hit too, with MIS.  No reset: the estimator has
+    // the same expectation, so it applies from the next frame and keeps the accumulation.
+    void SetEmitterSampling(bool on);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

@@ -191,6 +191,10 @@ int rth_render_set_spatial_denoiser(void* h, std::uint32_t iterations, float sig
     try { ((RenderHandle*)h)->render->SetSpatialDenoiser(iterations, sigma_color, sigma_normal, sigma_depth); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_emitter_sampling(void* h, int on)
+{
+    try { ((RenderHandle*)h)->render->SetEmitterSampling(on != 0); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_active_pixels(void* h, std::uint32_t* n)
 {
     try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

@@ -48,6 +48,8 @@ public:
     {
         Cuda().SetSpatialDenoiser(iterations, sigma_color, sigma_normal, sigma_depth);
     }
+    // emitter sampling (CUDAPathTraceIntegrator::SetEmitterSampling): applies from the next RenderFrame(), keeps the accumulation
+    void SetEmitterSampling(bool on) { Cuda().SetEmitterSampling(on); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

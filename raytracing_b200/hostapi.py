@@ -45,6 +45,7 @@ def load_library():
     L.rth_render_set_samples_per_frame.argtypes = [C.c_void_p, C.c_uint32]
     L.rth_render_set_adaptive_sampling.argtypes = [C.c_void_p, C.c_float, C.c_uint32]
     L.rth_render_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
+    L.rth_render_set_emitter_sampling.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
@@ -220,6 +221,11 @@ class HostRender:
     def set_spatial_denoiser(self, iterations, sigma_color=0.0, sigma_normal=0.0, sigma_depth=0.0):
         """Render::SetSpatialDenoiser: edge-avoiding a-trous filter (0 = off .. 5 passes) on the image of every later render_frame()."""
         if self.L.rth_render_set_spatial_denoiser(self.h, int(iterations), float(sigma_color), float(sigma_normal), float(sigma_depth)) != 0:
+            raise _err(self.L)
+
+    def set_emitter_sampling(self, on):
+        """Render::SetEmitterSampling: next-event estimation on the emissive triangles too (MIS); applies from the next render_frame()."""
+        if self.L.rth_render_set_emitter_sampling(self.h, int(bool(on))) != 0:
             raise _err(self.L)
 
     def active_pixels(self):
