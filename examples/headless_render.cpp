@@ -6,7 +6,7 @@
  *
  *   g++ -std=c++17 -O2 -Iinclude -Iraytracing_b200/host examples/headless_render.cpp \
  *       -Lraytracing_b200 -lrt_host -lrt_b200 -Wl,-rpath,'$ORIGIN/../raytracing_b200' -o examples/headless_render
- *   examples/headless_render assets/CornellBox.obj assets/ibl/CGSkies_0036_free.hdr 1920 1080 64 out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1]
+ *   examples/headless_render assets/CornellBox.obj assets/ibl/CGSkies_0036_free.hdr 1920 1080 64 out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1] [env=1] [lights=WA,WE,WV]
  *
  * The optional device list spreads the frame over several GPUs of the node behind the same Render / Integrator objects
  * ("all" = every CUDA device; the image is partitioned by scanline inside the library, rt_create_multi).
@@ -15,6 +15,8 @@
  * denoise=ITER,SC,SN,SZ turns on the spatial denoiser (Render::SetSpatialDenoiser: ITER passes, the colour, normal and depth sigmas)
  * on a single-device render.
  * emitters=1 turns on emitter sampling (Render::SetEmitterSampling: next-event estimation on the emissive triangles, with MIS).
+ * env=1 turns on environment sampling (Render::SetEnvironmentSampling: next-event estimation on the environment map, with MIS).
+ * lights=WA,WE,WV sets the weights of the light kind drawn at each vertex (Render::SetLightSelection: analytic, emitters, environment).
  *
  * Needs an H100 (there is no CPU fallback: Render's constructor throws without a CUDA device).
  */
@@ -31,17 +33,25 @@
 
 int main(int argc, char** argv)
 {
-    if (argc < 7) { std::fprintf(stderr, "usage: %s scene.obj env.hdr width height samples out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1]\n", argv[0]); return 2; }
+    if (argc < 7) { std::fprintf(stderr, "usage: %s scene.obj env.hdr width height samples out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1] [env=1] [lights=WA,WE,WV]\n", argv[0]); return 2; }
     const unsigned width = (unsigned)std::atoi(argv[3]), height = (unsigned)std::atoi(argv[4]), samples = (unsigned)std::atoi(argv[5]);
     float max_error = 0.0f;                                                                         // 0: every pixel takes every sample
     const char* device_arg = nullptr;
     unsigned denoise_iters = 0;                                                                     // 0: no spatial denoiser
     float sigma_color = 0.0f, sigma_normal = 0.0f, sigma_depth = 0.0f;
     bool emitters = false;                                                                          // emitter sampling off
+    bool env = false;                                                                               // environment sampling off
+    float light_w[3] = { 0.0f, 0.0f, 0.0f };                                                        // 0: the default weights
     for (int i = 7; i < argc; ++i)
     {
         if (std::string(argv[i]).rfind("max_error=", 0) == 0) max_error = (float)std::atof(argv[i] + 10);
         else if (std::string(argv[i]).rfind("emitters=", 0) == 0) emitters = std::atoi(argv[i] + 9) != 0;
+        else if (std::string(argv[i]).rfind("env=", 0) == 0) env = std::atoi(argv[i] + 4) != 0;
+        else if (std::string(argv[i]).rfind("lights=", 0) == 0)
+        {
+            if (std::sscanf(argv[i] + 7, "%f,%f,%f", &light_w[0], &light_w[1], &light_w[2]) != 3)
+            { std::fprintf(stderr, "lights= takes three weights WA,WE,WV\n"); return 2; }
+        }
         else if (std::string(argv[i]).rfind("denoise=", 0) == 0)
         {
             if (std::sscanf(argv[i] + 8, "%u,%f,%f,%f", &denoise_iters, &sigma_color, &sigma_normal, &sigma_depth) != 4)
@@ -62,6 +72,8 @@ int main(int argc, char** argv)
         rt_host::Render& render = *owner;
         render.SetMaxBounces(8);
         if (emitters) render.SetEmitterSampling(true);
+        if (env) render.SetEnvironmentSampling(true);
+        if (light_w[0] != 0.0f || light_w[1] != 0.0f || light_w[2] != 0.0f) render.SetLightSelection(light_w[0], light_w[1], light_w[2]);
         if (denoise_iters > 0) render.SetSpatialDenoiser(denoise_iters, sigma_color, sigma_normal, sigma_depth);
         if (samples > 0 && max_error > 0.0f)
         {   // progressive: chunks of 16 samples until every pixel has settled or the budget is spent

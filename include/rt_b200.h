@@ -96,9 +96,12 @@ typedef enum RtOption {
     RT_OPT_TOP_SMEM = 29,       /* scenes whose traversal records do not fit shared memory: number of top-of-tree interior records
                                    (breadth-first, 64 B each, <= 640 = 40 KB) that every traversal CTA stages with one TMA bulk copy;
                                    0 (default) = none.  Results are bit-identical */
-    RT_OPT_EMITTER_SAMPLING = 30 /* 0 (default): emissive triangles add light only when a BSDF-sampled ray hits them; 1: next-event
+    RT_OPT_EMITTER_SAMPLING = 30, /* 0 (default): emissive triangles add light only when a BSDF-sampled ray hits them; 1: next-event
                                    estimation on the emissive triangles too, combined with BSDF sampling by MIS (the rule is stated
                                    in the emitter-sampling block below; the image converges to the same expectation) */
+    RT_OPT_ENV_SAMPLING = 31    /* 0 (default): the environment map adds light only when a BSDF-sampled ray misses; 1: next-event
+                                   estimation on the environment map too, combined with BSDF sampling by MIS (the environment-sampling
+                                   block below; the image converges to the same expectation) */
 } RtOption;
 
 #define RT_MAX_BOUNCES 255u     /* bounce index range supported per frame (reference GUI: 0..5) */
@@ -315,7 +318,8 @@ int rt_set_spatial_denoiser(rt_ctx* ctx, uint32_t iterations, float sigma_color,
  * material's constant emission, luma = (r*0.299f + g*0.587f) + b*0.114f, non-finite or negative w_t -> 0; cdf[i] = S_i / S_n (running
  * float sum in list order), cdf[n-1] = 1; pmf_i = cdf[i] - cdf[i-1]; pdfA[t] = (P_e * pmf_i) / A_t where pmf_i > 0, else 0 (and 0 off
  * the list).  P_e = 0 if S_n is not finite and > 0 or in white-furnace mode (the frame is then bit-identical to the option off);
- * 1 if every analytic light has zero radiance; else 0.5.
+ * 1 if every analytic light has zero radiance; else 0.5.  (Those are the default weights of rt_set_light_selection; the light-kind
+ * block below states P_e and the analytic divisor for any weights and with environment sampling.)
  * At a hit of bounce b < max_bounces (the last max_bounces passed to rt_integrate / rt_integrate_samples; the stepwise steps, which
  * are not told max_bounces, use the value of the most recent such call, RT_MAX_BOUNCES before any), with kRandom draws r_k = hash(dimension 0x10000 + 4*b + k) whatever
  * the sampler:
@@ -340,6 +344,42 @@ int rt_set_spatial_denoiser(rt_ctx* ctx, uint32_t iterations, float sigma_color,
  * rt_integrate_samples) with the same max_bounces once before driving the steps.
  * Device memory: 4 B per triangle and 8 B per emitter while it is on.  rt_integrate_samples runs n frames of
  * rt_integrate's schedule with it on (the regenerating kernel keeps its path state where the carried p_b goes). */
+
+/* ---- environment sampling (new capability): rt_set_option(ctx, RT_OPT_ENV_SAMPLING, 1) --------------------------------------
+ * Next-event estimation on the environment map, combined with BSDF sampling by MIS (power heuristic, as for emitters); same
+ * expectation as the option off.  All float, no contraction, in the order written; sin / cos / atan2 / acos are rt_math.h's.
+ * Environment table (raytracing_b200/csrc/rt_envmap.h), a pure function of the uploaded image (w x h texels) and the flags:
+ *     W_ij = luma(texel i of row j) * sin(pi * ((j + 0.5f) / h)), a luma that is not finite and >= 0 counting as 0;
+ *     marginal CDF over the row sums and one conditional CDF per row, running float sums, last entry 1;
+ *     T = the sum of the row sums; p_uv(i, j) = ((w * h) * W_ij) / T; table[i, j] = P_v * p_uv(i, j).
+ *     Active iff T is finite and > 0, the option is on and white-furnace mode is off; else the frame is that of the option off.
+ * p_v(dir) = table[cell of dir] / (2pi^2 * sqrtf(max(1 - z*z, 0))), the cell holding sample_sky's texture coordinates
+ * (cx = (atan2(x, y) + pi) / 2pi, cy = acos(z) / pi, wrapped to [0, 1), times w / h, truncated); one function for both sides.
+ * At a hit of bounce b < max_bounces (as for emitters) that draws the environment kind (below):
+ *     row j = first marginal entry > min(r_1, 0x1.fffffep-1), column i = first entry of row j > min(r_2, 0x1.fffffep-1), r_1..r_3 the
+ *     emitter draws of the bounce and r_4 = hash(dimension 0x20000 + b) (kRandom whatever the sampler); u = (i + r_3) / w,
+ *     v = (j + r_4) / h; phi = u * 2pi - pi, theta = v * pi; dir = (sin theta sin phi, sin theta cos phi, cos theta);
+ *     Le = sample_sky(dir) (what a miss adds); g, p_b as for emitters; sample = ((T * g) * Le) * (mis(p_v, p_b) / p_v) with
+ *     p_v = p_v(dir); shadow ray from position + geometry_normal * EPS along dir, t_max = RT_MAX_RENDER_DIST (unoccluded exactly
+ *     where a continuation ray would miss), spawned iff p_v > 0 and dot(sample, sample) > 0.
+ * A continuation ray that misses with carried p_b > 0 while the table is active adds (sky * T) * mis(p_b, p_v(dir)); every other miss
+ * (primary rays, after a delta lobe, with the table inactive) is unchanged.  Values other than 0 and 1 are RT_ERR_INVALID_ARGUMENT.
+ * The setting applies from the next frame and keeps the accumulation.  Device memory while it is active: 8 B per texel + 4 B per row,
+ * built from the device copy of the image.  As for emitters, the stepwise steps use the last max_bounces, and rt_integrate_samples
+ * runs n frames of rt_integrate's schedule.
+ *
+ * ---- light-kind selection: rt_set_light_selection(ctx, analytic, emitters, environment) ------------------------------------------
+ * Relative weights of the light kind drawn at each vertex while emitter or environment sampling is active; default (1, 1, 1).
+ * A kind's weight counts only while the kind is active (analytic: an analytic light has non-zero radiance; emitters: the emitter
+ * table is active; environment: the environment table is active), else it is 0: w_a, w_e, w_v.  S = (w_a + w_e) + w_v,
+ * P_e = w_e / S, P_v = w_v / S (pdfA of the emitter table uses this P_e).  With r_0 = hash(dimension 0x10000 + 4*b):
+ *     emitter iff P_e >= 1 or r_0 < P_e;  else environment iff the environment table is active and (w_a == 0 or r_0 < P_e + P_v);
+ *     else the analytic light sample of the options off, divided by (1 - (P_e + P_v)).
+ * With RT_OPT_ENV_SAMPLING 0 and the default weights this is the emitter rule above bit for bit (P_e = 0.5 or 1); with both options
+ * off nothing is drawn and the frame is the reference's.  A weight that is not finite or <= 0, or a sum that is not finite, is
+ * RT_ERR_INVALID_ARGUMENT (a zero weight on an active kind would bias the estimator).  Applies from the next frame, keeps the
+ * accumulation, and works with either option alone. */
+int rt_set_light_selection(rt_ctx* ctx, float analytic, float emitters, float environment);
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

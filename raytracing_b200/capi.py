@@ -20,6 +20,7 @@ BN_SOBOL_COUNT, BN_TILE_COUNT = 65536, 131072
 OPT_COUNT_TRAVERSAL, OPT_KERNEL_TIMING, OPT_TRAVERSAL = 16, 17, 18
 OPT_AOV_ALWAYS, OPT_SMEM_BVH, OPT_OVERLAP, OPT_GRAPH, OPT_PDL, OPT_FRAME_KERNEL, OPT_PRESENT, OPT_FRAME_THREADS, OPT_TOP_SMEM = 21, 22, 23, 24, 25, 26, 27, 28, 29
 OPT_EMITTER_SAMPLING = 30       # 1: next-event estimation on the emissive triangles, MIS with BSDF sampling (include/rt_b200.h)
+OPT_ENV_SAMPLING = 31           # 1: next-event estimation on the environment map, MIS with BSDF sampling (include/rt_b200.h)
 KERNEL_CLASSES = ["raygen", "intersect", "miss", "hit", "intersect_shadow", "accumulate", "extend_shade",
                   "shadow_accumulate", "resolve", "aov", "misc", "trace_closest", "shade_queues", "trace_both"]
 
@@ -34,7 +35,8 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_radiance_device_ptr", "rt_stream_handle",
            "rt_create_multi", "rt_device_count", "rt_gather_radiance", "rt_host_register", "rt_host_unregister", "rt_math_eval",
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
-           "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser"]
+           "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
+           "rt_set_light_selection"]
 
 
 class RtSceneDesc(C.Structure):
@@ -117,6 +119,7 @@ def load_library():
     L.rt_read_pixel_samples.argtypes = [C.c_void_p, C.c_void_p]
     L.rt_read_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rt_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
+    L.rt_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
     _lib = L
     return L
 
@@ -267,6 +270,11 @@ class Context:
         """Edge-avoiding a-trous filter on the shaded colour of resolve() / resolve_async() (rt_set_spatial_denoiser): iterations
         0 (off) .. 5, guided by the last frame's normal and depth; a sigma of 0 drops its term."""
         self._ck(self.lib.rt_set_spatial_denoiser(self.h, int(iterations), float(sigma_color), float(sigma_normal), float(sigma_depth)))
+
+    def set_light_selection(self, analytic=1.0, emitters=1.0, environment=1.0):
+        """Relative weights of the light kind drawn at each vertex while emitter or environment sampling is active
+        (rt_set_light_selection; a kind's weight counts only while it is active); each finite and > 0."""
+        self._ck(self.lib.rt_set_light_selection(self.h, float(analytic), float(emitters), float(environment)))
 
     def integrate_stepwise(self, max_bounces):
         """The schedule of Integrator::Integrate (integrator.cpp:35-51), one call per reference virtual."""

@@ -153,6 +153,13 @@ struct DevScene
     const uint32_t* emit_list;     // per emitter: triangle id
     uint32_t n_emit;
     float emit_pe;
+    // environment sampling (RT_OPT_ENV_SAMPLING, rt_envmap.h): nullptr while it is off or inactive
+    const float* env_marg;         // per row
+    const float* env_cond;         // per texel
+    const float* env_pdf;          // per texel: P_v * p_uv
+    // light-kind draw (rt_set_light_selection) while either table exists: P_e + P_v, and whether the analytic kind has weight 0
+    float light_pev;
+    uint32_t no_analytic;
 };
 
 // ---------------------------------------------------------------------------- environment

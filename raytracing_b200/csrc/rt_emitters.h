@@ -62,10 +62,11 @@ inline float emission_luma(const RtPackedMaterial& m)
     return (r * 0.299f + g * 0.587f) + b * 0.114f;
 }
 
-// tri(i) returns the RtTriangle of emitters[i] (the caller has checked the indices).
+// tri(i) returns the RtTriangle of emitters[i] (the caller has checked the indices).  p_e_sel >= 0: the P_e of the light-selection
+// rule (rt_envmap.h rtenv::select) replaces the default 1 / 0.5 of an active table.
 template <class TriOf>
 inline void build(TriOf tri, const uint32_t* idx, uint64_t n, uint64_t n_tris, const RtPackedMaterial* mats,
-                  const RtLight* lights, uint32_t n_analytic, bool white_furnace, Table& out)
+                  const RtLight* lights, uint32_t n_analytic, bool white_furnace, Table& out, float p_e_sel = -1.0f)
 {
     out.list.assign(idx, idx + n);
     out.cdf.assign(n, 0.0f);
@@ -88,7 +89,7 @@ inline void build(TriOf tri, const uint32_t* idx, uint64_t n, uint64_t n_tris, c
     bool dark = true;
     for (uint32_t l = 0; l < n_analytic; ++l)
         if (lights[l].radiance.x != 0.0f || lights[l].radiance.y != 0.0f || lights[l].radiance.z != 0.0f) dark = false;
-    out.p_e = dark ? 1.0f : 0.5f;
+    out.p_e = p_e_sel >= 0.0f ? p_e_sel : (dark ? 1.0f : 0.5f);
     for (uint64_t i = 0; i < n; ++i)
     {
         float pmf = out.cdf[i] - (i ? out.cdf[i - 1] : 0.0f);

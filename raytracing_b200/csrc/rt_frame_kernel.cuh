@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                         }
                     }
                 }
-                else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, in, base + q.missq[base + at - hit_span + lane], radiance);
+                else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, base + q.missq[base + at - hit_span + lane], radiance);
             }
             __syncthreads();
             if (threadIdx.x == 0)

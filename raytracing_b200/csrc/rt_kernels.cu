@@ -41,6 +41,7 @@
 #include "rt_bvh_layout.h"
 #include "rt_device.cuh"
 #include "rt_emitters.h"
+#include "rt_envmap.h"
 
 using namespace rt;
 
@@ -77,23 +78,29 @@ struct ShadeOut
     f3 emission_add;
     f3 s_origin, s_dir, s_sample; float s_tmax;
     f3 n_origin, n_dir, n_throughput;
-    float n_pdf;                   // C.w of the continuation ray: its p_b with emitter sampling on, else 0
+    float n_pdf;                   // C.w of the continuation ray: its p_b with emitter or environment sampling on, else 0
 };
 
-// kernels/cl/miss.cl:41-77: radiance += sky * throughput, for the ray in slot `slot` of ray queue `in`
+// kernels/cl/miss.cl:41-77: radiance += sky * throughput, for the ray in slot `slot` of ray queue `in`.
+// EMIT (the sampled-light instance, shade_hit): with an environment table, a BSDF-sampled ray (C.w = p_b > 0) adds
+// (sky * throughput) * mis(p_b, p_v(dir)), weighted against the environment strategy that could have drawn its direction.
+template <bool EMIT = false>
 __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams& p, const Queues& q, int in, uint32_t slot, float4* radiance)
 {
     const float4 a = q.A[in][slot], b = q.B[in][slot], c = q.C[in][slot];
     f3 sky = p.white_furnace ? splat(0.5f) : sample_sky(sc, mk3(b));
     uint32_t li = local_index(p, __float_as_uint(a.w));
-    float4 r = add_radiance(radiance, li, sky * mk3(c));
+    f3 add = sky * mk3(c);
+    if (EMIT && c.w > 0.0f && sc.env_pdf)
+        add = add * mis_power(c.w, rtenv::pdf_dir(sc.env_pdf, sc.env_w, sc.env_h, b.x, b.y, b.z));
+    float4 r = add_radiance(radiance, li, add);
     if (p.gather) p.gather[li] = r;        // the path ends here: its pixel is final (its last shadow ray was accumulated a phase ago)
 }
 
 // kernels/cl/hit_surface.cl:30-186, for the path of sample p.dyn->sample_idx + sample_offset (a later sample of a multi-sample call).
-// prev_pdf: C.w of the ray (emitter sampling: p_b of its direction at the previous vertex, 0 for primary rays and after a delta lobe).
-// EMIT: the scene has an active emitter table (sc.emit_*, RT_OPT_EMITTER_SAMPLING); a template flag, so that the kernels without it
-// are the code of the option off.
+// prev_pdf: C.w of the ray (sampled lights: p_b of its direction at the previous vertex, 0 for primary rays and after a delta lobe).
+// EMIT: the scene has an active emitter table (sc.emit_*, RT_OPT_EMITTER_SAMPLING) or environment table (sc.env_*,
+// RT_OPT_ENV_SAMPLING), each read only while it exists; a template flag, so that the kernels without it are the code of both options off.
 template <bool EMIT = false>
 __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
                                           f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
@@ -127,15 +134,15 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         aov.velocity[li] = make_float2(s0.x - s1.x, s0.y - s1.y);
     }
 
-    // emitter sampling (RT_OPT_EMITTER_SAMPLING): on at this vertex iff the scene has an active emitter table and the frame traces the
-    // continuation ray of this bounce
+    // sampled lights (RT_OPT_EMITTER_SAMPLING, RT_OPT_ENV_SAMPLING): on at this vertex iff the scene has an active emitter or
+    // environment table and the frame traces the continuation ray of this bounce
     const bool emit_on = EMIT && bounce < p.dyn->max_bounces;
     out.emissive = false;
     if (!p.white_furnace && dot(material.emission, splat(1.0f)) > 0.0f)
     {
         out.emissive = true;
         out.emission_add = hit_throughput * material.emission;
-        if (EMIT && prev_pdf > 0.0f)
+        if (EMIT && prev_pdf > 0.0f && sc.emit_pdfA)
         {   // BSDF sample of an emitter: weighted against the emitter strategy that could have produced this direction
             const float pdfA = __ldg(sc.emit_pdfA + prim);
             if (pdfA > 0.0f)
@@ -149,11 +156,13 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
     }
     uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx + sample_offset);
     out.spawn_shadow = false;
-    bool pick_emitter = false;
+    bool pick_emitter = false, pick_env = false;
     if (EMIT && emit_on)
-    {   // light kind: c < P_e (P_e is 1 or 0.5)
+    {   // light kind (rt_set_light_selection): emitter iff P_e >= 1 or c < P_e, else environment iff the analytic weight is 0 or
+        // c < P_e + P_v, else analytic (P_e = 0 without an emitter table, P_v = 0 without an environment table)
         const float ck = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce);
         pick_emitter = sc.emit_pe >= 1.0f || ck < sc.emit_pe;
+        pick_env = !pick_emitter && sc.env_pdf && (sc.no_analytic || ck < sc.light_pev);
     }
     if (pick_emitter)
     {   // next-event estimation on an emissive triangle
@@ -198,6 +207,23 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
             out.s_dir = w; out.s_tmax = 0.999f * d; out.s_sample = ls;
         }
     }
+    else if (pick_env)
+    {   // next-event estimation on the environment map: its shadow ray is unoccluded exactly where a continuation ray would miss
+        const float k1 = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce + 1u);
+        const float k2 = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce + 2u);
+        const float k3 = sample_random(pixel_seed, 0u, 0x10000u + 4u * bounce + 3u);
+        const float k4 = sample_random(pixel_seed, 0u, 0x20000u + bounce);
+        f3 w;
+        rtenv::sample(sc.env_marg, sc.env_cond, sc.env_w, sc.env_h, k1, k2, k3, k4, w.x, w.y, w.z);
+        const float p_v = rtenv::pdf_dir(sc.env_pdf, sc.env_w, sc.env_h, w.x, w.y, w.z);
+        const f3 le = sample_sky(sc, w);
+        float p_b, spec_pdf, alpha;
+        const f3 g = bxdf_eval_sampled(material, normal, incoming, w, p_b, spec_pdf, alpha);
+        const f3 ls = hit_throughput * g * le * (mis_power(p_v, p_b) / p_v);
+        out.spawn_shadow = (p_v > 0.0f) && (dot(ls, ls) > 0.0f);
+        out.s_origin = position + geometry_normal * RT_EPS;
+        out.s_dir = w; out.s_tmax = RT_MAX_RENDER_DIST; out.s_sample = ls;
+    }
     else
     {   // direct lighting (next-event estimation on analytic lights)
         float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx + sample_offset, bounce * 5u + SAMPLE_LIGHT)
@@ -212,7 +238,7 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         {
             f3 brdf = evaluate_material(material, normal, incoming, outgoing);
             f3 ls = light_radiance * hit_throughput * brdf / pdf * cos_l;
-            if (EMIT && emit_on) ls = ls / (1.0f - sc.emit_pe);
+            if (EMIT && emit_on) ls = ls / (1.0f - sc.light_pev);
             out.spawn_shadow = (pdf > 0.0f) && (dot(ls, ls) > 0.0f);
             out.s_origin = position + normal * RT_EPS;
             out.s_dir = outgoing; out.s_tmax = distance_to_light; out.s_sample = ls;
@@ -243,7 +269,7 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         out.n_dir = outgoing;
         out.n_pdf = 0.0f;
         if (EMIT && emit_on)
-        {   // the continuation's p_b for the MIS weight of an emitter it hits (0 after a delta lobe)
+        {   // the continuation's p_b for the MIS weight of an emitter it hits or of the sky it misses into (0 after a delta lobe)
             float p_b, spec_pdf, alpha;
             bxdf_eval_sampled(material, normal, incoming, outgoing, p_b, spec_pdf, alpha);
             const bool delta = material.transparency < 0.5f || (s1 <= spec_pdf && alpha <= 1e-4f);
@@ -450,6 +476,7 @@ __global__ void __launch_bounds__(256) k_intersect(FrameParams p, DevScene sc, i
 }
 
 // ShadeMissedRays (stepwise)
+template <bool EMIT>
 __global__ void __launch_bounds__(256) k_shade_miss(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -458,7 +485,7 @@ __global__ void __launch_bounds__(256) k_shade_miss(FrameParams p, DevScene sc, 
     if (i < n)
     {
         miss = __float_as_uint(q.hits[i].z) == RT_INVALID_ID;
-        if (miss) shade_miss(sc, p, q, bounce & 1, i, radiance);
+        if (miss) shade_miss<EMIT>(sc, p, q, bounce & 1, i, radiance);
     }
     warp_count(&ctr->hm[bounce].miss, miss);
 }
@@ -646,7 +673,7 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 uint32_t pixel;
                 shade_hit_group<false, EMIT>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
             }
-            else if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
+            else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
         }
         return;
     }
@@ -671,13 +698,13 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 uint32_t pixel;
                 shade_hit_group<true, EMIT>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
             }
-            else if (g - hit_span + lane < n_miss) shade_miss(sc, p, q, in, q.missq[g - hit_span + lane], radiance);
+            else if (g - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, q.missq[g - hit_span + lane], radiance);
         }
         if (at < hit_span) flush_continuations(st, q, in ^ 1, &ctr->emit[bounce].next);
         if (at + batch >= hit_span) break;                      // every later entry is a miss
     }
     for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < total;)
-        if (at - hit_span + lane < n_miss) shade_miss(sc, p, q, in, q.missq[at - hit_span + lane], radiance);
+        if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, q.missq[at - hit_span + lane], radiance);
 }
 
 #include "rt_frame_kernel.cuh"
@@ -1105,7 +1132,12 @@ struct rt_ctx
     std::vector<RtPackedMaterial> emit_mats;
     std::vector<RtLight> emit_lights;
     uint64_t emit_n_tris = 0;
-    std::vector<void*> emit_allocs;
+    std::vector<void*> emit_allocs;                // the device emitter and environment tables
+    // environment sampling (RT_OPT_ENV_SAMPLING, its table scene.env_* built from the device image) and the light-kind weights
+    // (rt_set_light_selection; analytic_lit: an analytic light of the upload has non-zero radiance)
+    int env_sampling = 0;
+    float light_w[3] = { 1.0f, 1.0f, 1.0f };
+    bool analytic_lit = false;
 
     // spatial denoiser (rt_set_spatial_denoiser): passes (0 = off), sigmas, scratch planes (allocated while it is on)
     uint32_t sd_iters = 0;
@@ -1576,24 +1608,44 @@ int rt_set_partition(rt_ctx* c, uint32_t rank, uint32_t world)
     return alloc_frame_buffers(c);
 }
 
-// (Re)builds the device emitter table from the kept upload data: rt_emitters.h.  Inactive (no table, scene.emit_* null) while the
-// option is off, before an upload, in white-furnace mode and when no emitter can be selected; the frames are then those of the
-// option off.  The caller has validated the indices.
-static int refresh_emitters(rt_ctx* c)
+static void clear_light_tables(rt_ctx* c)
 {
-    RT_CUDA(c, cudaSetDevice(c->device));
-    { int rc = join_shadow(c); if (rc) return rc; }
-    RT_CUDA(c, cudaStreamSynchronize(c->stream));     // a frame in flight may still read the old table
     for (void* p : c->emit_allocs) cudaFree(p);
     c->emit_allocs.clear();
     DevScene& ds = c->scene;
     ds.emit_pdfA = nullptr; ds.emit_cdf = nullptr; ds.emit_list = nullptr; ds.n_emit = 0; ds.emit_pe = 0.0f;
+    ds.env_marg = nullptr; ds.env_cond = nullptr; ds.env_pdf = nullptr; ds.light_pev = 0.0f; ds.no_analytic = 0;
+}
+
+// (Re)builds the device emitter table (rt_emitters.h) from the kept upload data and the environment table (rt_envmap.h) from the
+// device's environment image, with the light-kind probabilities of the current weights.  A table is inactive (not allocated, its
+// scene.* pointers null) while its option is off, before an upload, in white-furnace mode and when it has nothing to select; with
+// both inactive the frames are those of both options off.  The caller has validated the emitter indices.
+static int refresh_lights(rt_ctx* c)
+{
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));     // a frame in flight may still read the old tables
+    clear_light_tables(c);
     ++c->config_gen;
-    if (!c->emitter_sampling || !c->scene_ready) return RT_OK;
-    rtemit::Table t;
-    rtemit::build([&](uint64_t i) -> const RtTriangle& { return c->emit_tris[i]; }, c->emit_idx.data(), c->emit_idx.size(), c->emit_n_tris,
-                  c->emit_mats.data(), c->emit_lights.data(), ds.light_count, c->white_furnace != 0, t);
-    if (t.p_e == 0.0f) return RT_OK;
+    if ((!c->emitter_sampling && !c->env_sampling) || !c->scene_ready) return RT_OK;
+    DevScene& ds = c->scene;
+    auto tri_of = [&](uint64_t i) -> const RtTriangle& { return c->emit_tris[i]; };
+    rtemit::Table et;
+    if (c->emitter_sampling)
+        rtemit::build(tri_of, c->emit_idx.data(), c->emit_idx.size(), c->emit_n_tris, c->emit_mats.data(), c->emit_lights.data(),
+                      ds.light_count, c->white_furnace != 0, et);
+    const bool emit_active = et.p_e > 0.0f;
+    rtenv::Table vt;
+    bool env_active = false;
+    if (c->env_sampling && !c->white_furnace)
+    {   // the image is read back from the device: the context keeps no host copy of it
+        std::vector<float> img((size_t)ds.env_w * ds.env_h * 4);
+        RT_CUDA(c, cudaMemcpy(img.data(), ds.env, img.size() * 4, cudaMemcpyDeviceToHost));
+        env_active = rtenv::build(img.data(), (uint32_t)ds.env_w, (uint32_t)ds.env_h, vt);
+    }
+    if (!emit_active && !env_active) return RT_OK;
+    const rtenv::Selection sel = rtenv::select(c->analytic_lit, emit_active, env_active, c->light_w[0], c->light_w[1], c->light_w[2]);
     auto upload = [&](const void* src, size_t bytes, const void** dst) -> int {
         void* d = nullptr;
         RT_CUDA(c, cudaMalloc(&d, bytes));
@@ -1603,12 +1655,28 @@ static int refresh_emitters(rt_ctx* c)
         return RT_OK;
     };
     int rc;
-    if ((rc = upload(t.pdfA.data(), t.pdfA.size() * 4, (const void**)&ds.emit_pdfA))) return rc;
-    if ((rc = upload(t.cdf.data(), t.cdf.size() * 4, (const void**)&ds.emit_cdf))) return rc;
-    if ((rc = upload(t.list.data(), t.list.size() * 4, (const void**)&ds.emit_list))) return rc;
-    ds.n_emit = (uint32_t)t.list.size(); ds.emit_pe = t.p_e;
+    if (emit_active)
+    {
+        rtemit::build(tri_of, c->emit_idx.data(), c->emit_idx.size(), c->emit_n_tris, c->emit_mats.data(), c->emit_lights.data(),
+                      ds.light_count, c->white_furnace != 0, et, sel.p_e);
+        if ((rc = upload(et.pdfA.data(), et.pdfA.size() * 4, (const void**)&ds.emit_pdfA))) return rc;
+        if ((rc = upload(et.cdf.data(), et.cdf.size() * 4, (const void**)&ds.emit_cdf))) return rc;
+        if ((rc = upload(et.list.data(), et.list.size() * 4, (const void**)&ds.emit_list))) return rc;
+        ds.n_emit = (uint32_t)et.list.size(); ds.emit_pe = et.p_e;
+    }
+    if (env_active)
+    {
+        rtenv::scale(vt, sel.p_v);
+        if ((rc = upload(vt.marg.data(), vt.marg.size() * 4, (const void**)&ds.env_marg))) return rc;
+        if ((rc = upload(vt.cond.data(), vt.cond.size() * 4, (const void**)&ds.env_cond))) return rc;
+        if ((rc = upload(vt.pdf.data(), vt.pdf.size() * 4, (const void**)&ds.env_pdf))) return rc;
+    }
+    ds.light_pev = sel.p_ev; ds.no_analytic = sel.no_analytic ? 1u : 0u;
     return RT_OK;
 }
+
+// Either table exists: the sampled-light instances of the shading kernels run
+static bool lights_sampled(const rt_ctx* c) { return c->scene.emit_pdfA || c->scene.env_pdf; }
 
 int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
 {
@@ -1655,9 +1723,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     for (void* p : c->scene_allocs) cudaFree(p);
     c->scene_allocs.clear();
     c->scene_ready = false;
-    for (void* p : c->emit_allocs) cudaFree(p);
-    c->emit_allocs.clear();
-    c->scene.emit_pdfA = nullptr; c->scene.emit_cdf = nullptr; c->scene.emit_list = nullptr; c->scene.n_emit = 0; c->scene.emit_pe = 0.0f;
+    clear_light_tables(c);
 
     auto upload = [&](const void* src, size_t bytes, const void** dst) -> int {
         void* d = nullptr;
@@ -1718,9 +1784,10 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     if (n_emit) { c->emit_mats.assign(s->materials, s->materials + s->n_materials); c->emit_lights.assign(s->lights, s->lights + s->n_lights); }
     else { c->emit_mats.clear(); c->emit_lights.clear(); }
     c->emit_n_tris = s->n_triangles;
+    c->analytic_lit = rtenv::analytic_lit(s->lights, s->scene_info.analytic_light_count);
     c->scene_ready = true;
     ++c->config_gen;
-    return refresh_emitters(c);
+    return refresh_lights(c);
 }
 
 int rt_set_camera(rt_ctx* c, const RtCamera* cam)
@@ -1772,7 +1839,7 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
     case RT_OPT_WHITE_FURNACE:
         if ((value != 0) == (c->white_furnace != 0)) return RT_OK;
         c->white_furnace = value != 0;
-        return c->emitter_sampling ? refresh_emitters(c) : RT_OK;
+        return (c->emitter_sampling || c->env_sampling) ? refresh_lights(c) : RT_OK;
     case RT_OPT_EMITTER_SAMPLING:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "emitter sampling must be 0 (off) or 1 (emissive triangles with MIS)");
         if (value == 1 && c->scene_ready)
@@ -1783,7 +1850,12 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
         }
         if ((int)value == c->emitter_sampling) return RT_OK;
         c->emitter_sampling = (int)value;
-        return refresh_emitters(c);
+        return refresh_lights(c);
+    case RT_OPT_ENV_SAMPLING:
+        if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "environment sampling must be 0 (off) or 1 (the environment map with MIS)");
+        if ((int)value == c->env_sampling) return RT_OK;
+        c->env_sampling = (int)value;
+        return refresh_lights(c);
     case RT_OPT_SAMPLER:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "sampler type must be 0 (kRandom) or 1 (kBlueNoise)");
         if (value == 1 && !c->d_bn)
@@ -1925,6 +1997,18 @@ int rt_set_spatial_denoiser(rt_ctx* c, uint32_t iterations, float sigma_color, f
     return RT_OK;
 }
 
+int rt_set_light_selection(rt_ctx* c, float analytic, float emitters, float environment)
+{
+    RT_CHECK_CTX(c);
+    auto ok = [](float w) { return std::isfinite(w) && w > 0.0f; };
+    if (!ok(analytic) || !ok(emitters) || !ok(environment) || !std::isfinite((analytic + emitters) + environment))
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_light_selection: every weight must be finite and > 0, and so must their sum");
+    RT_FANOUT(c, rt_set_light_selection(k, analytic, emitters, environment));
+    if (c->light_w[0] == analytic && c->light_w[1] == emitters && c->light_w[2] == environment) return RT_OK;
+    c->light_w[0] = analytic; c->light_w[1] = emitters; c->light_w[2] = environment;
+    return (c->emitter_sampling || c->env_sampling) ? refresh_lights(c) : RT_OK;
+}
+
 int rt_read_pixel_samples(rt_ctx* c, uint32_t* counts)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_read_pixel_samples(k, counts));
@@ -2017,7 +2101,7 @@ int rt_shade_miss(rt_ctx* c, uint32_t bounce)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_shade_miss(k, bounce));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     TimedLaunch t(c, RT_K_MISS);
-    k_shade_miss<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce);
+    (lights_sampled(c) ? k_shade_miss<true> : k_shade_miss<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce);
     return post_launch(c, "k_shade_miss");
 }
 
@@ -2030,7 +2114,7 @@ int rt_shade_hits(rt_ctx* c, uint32_t bounce)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     c->cur_bounce = bounce;
     TimedLaunch t(c, RT_K_HIT);
-    (c->scene.emit_pdfA ? k_shade_hits<true> : k_shade_hits<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
+    (lights_sampled(c) ? k_shade_hits<true> : k_shade_hits<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
     return post_launch(c, "k_shade_hits");
 }
 
@@ -2105,7 +2189,7 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     { int rc = join_shadow(c); if (rc) return rc; }     // the shading pass accumulates into radiance and refills the shadow queue
     TimedLaunch t(c, RT_K_SHADE_QUEUES);
     const bool sort = sorted_shading(c);
-    auto* k = c->scene.emit_pdfA ? (sort ? k_shade_queues<true, true> : k_shade_queues<false, true>)
+    auto* k = lights_sampled(c) ? (sort ? k_shade_queues<true, true> : k_shade_queues<false, true>)
                                  : (sort ? k_shade_queues<true> : k_shade_queues<false>);
     const size_t sm = sort ? sizeof(ContStage) : 0;
     launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
@@ -2288,7 +2372,7 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
     FrameParams fp = frame_params(c);
     fp.gather = push ? c->gather_slab : nullptr;
     rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
-        auto* k = c->scene.emit_pdfA ? k_frame<smem.value, true> : k_frame<smem.value>;
+        auto* k = lights_sampled(c) ? k_frame<smem.value, true> : k_frame<smem.value>;
         uint32_t grid, slots_per_cta;
         int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
         TimedLaunch t(c, RT_K_MISC);
@@ -2370,7 +2454,7 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
 // Measured on one H100 80GB HBM3 at 700 W (tools/spp_probe.py, 1080p x 8, rank 0 of 1/2/4/8-way partitions, N = 8 and 64, DESIGN.md
 // section 4) it never clearly beats N one-kernel frames: it ties on CornellBox (-3 % to +4 %) and is 5-29 % slower on ShaderBalls,
 // so every partition size takes the N-frame path.  Adaptive sampling decides between samples, so it always takes the N-frame path.
-static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c) && !adaptive_on(c) && !c->emitter_sampling; }
+static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c) && !adaptive_on(c) && !c->emitter_sampling && !c->env_sampling; }
 
 // A multi-sample call leaves its summed statistics in counters_sum, which only rt_read_frame_stats reads: the counters that the
 // taps (rt_read_rays, rt_read_hits) take their entry counts from never exceed one frame's rays.

@@ -140,6 +140,16 @@ void CUDAPathTraceIntegrator::SetEmitterSampling(bool on)
     Check(rt_set_option(ctx_, RT_OPT_EMITTER_SAMPLING, on ? 1u : 0u), "SetEmitterSampling");
 }
 
+void CUDAPathTraceIntegrator::SetEnvironmentSampling(bool on)
+{
+    Check(rt_set_option(ctx_, RT_OPT_ENV_SAMPLING, on ? 1u : 0u), "SetEnvironmentSampling");
+}
+
+void CUDAPathTraceIntegrator::SetLightSelection(float analytic, float emitters, float environment)
+{
+    Check(rt_set_light_selection(ctx_, analytic, emitters, environment), "SetLightSelection");
+}
+
 std::uint32_t CUDAPathTraceIntegrator::ActivePixels() const
 {
     std::uint32_t n = 0;

@@ -28,6 +28,8 @@
  * SetSpatialDenoiser(iterations, sigmas): ResolveRadiance() filters the shaded colour (include/rt_b200.h states the rule).
  * SetEmitterSampling(on): next-event estimation on the emissive triangles as well, combined with BSDF sampling by MIS
  * (RT_OPT_EMITTER_SAMPLING; the image converges to the same expectation, so the accumulation is kept).
+ * SetEnvironmentSampling(on): the same for the environment map (RT_OPT_ENV_SAMPLING); SetLightSelection(a, e, v): relative weights of
+ * the light kind drawn at each vertex (rt_set_light_selection).  Neither resets the accumulation.
  * AOVs (ComputeAOVs) are produced inside the bounce-0 shading pass, and only when SetAOV selected a view other than
  * the shaded colour or the denoiser is on.  SetSamplerType(kBlueNoise) needs the sampler's three tables first
  * (SetBlueNoiseTables; the OpenCL backend reads them from utils/blue_noise_sampler.hpp, cl_pt_integrator.cpp:222-235).
@@ -87,6 +89,10 @@ public:
     // emitter sampling (RT_OPT_EMITTER_SAMPLING): sample the emissive triangles at every hit too, with MIS.  No reset: the estimator has
     // the same expectation, so it applies from the next frame and keeps the accumulation.
     void SetEmitterSampling(bool on);
+    // environment sampling (RT_OPT_ENV_SAMPLING): sample the environment map at every hit too, with MIS.  No reset, as above.
+    void SetEnvironmentSampling(bool on);
+    // light-kind weights (rt_set_light_selection): analytic, emitters, environment, each finite and > 0.  No reset, as above.
+    void SetLightSelection(float analytic, float emitters, float environment);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

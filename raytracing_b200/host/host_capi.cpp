@@ -195,6 +195,15 @@ int rth_render_set_emitter_sampling(void* h, int on)
 {
     try { ((RenderHandle*)h)->render->SetEmitterSampling(on != 0); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_environment_sampling(void* h, int on)
+{
+    try { ((RenderHandle*)h)->render->SetEnvironmentSampling(on != 0); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
+}
+int rth_render_set_light_selection(void* h, float analytic, float emitters, float environment)
+{
+    try { ((RenderHandle*)h)->render->SetLightSelection(analytic, emitters, environment); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_active_pixels(void* h, std::uint32_t* n)
 {
     try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

@@ -50,6 +50,9 @@ public:
     }
     // emitter sampling (CUDAPathTraceIntegrator::SetEmitterSampling): applies from the next RenderFrame(), keeps the accumulation
     void SetEmitterSampling(bool on) { Cuda().SetEmitterSampling(on); }
+    // environment sampling and light-kind weights (CUDAPathTraceIntegrator): apply from the next RenderFrame(), keep the accumulation
+    void SetEnvironmentSampling(bool on) { Cuda().SetEnvironmentSampling(on); }
+    void SetLightSelection(float analytic, float emitters, float environment) { Cuda().SetLightSelection(analytic, emitters, environment); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

@@ -46,6 +46,8 @@ def load_library():
     L.rth_render_set_adaptive_sampling.argtypes = [C.c_void_p, C.c_float, C.c_uint32]
     L.rth_render_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
     L.rth_render_set_emitter_sampling.argtypes = [C.c_void_p, C.c_int]
+    L.rth_render_set_environment_sampling.argtypes = [C.c_void_p, C.c_int]
+    L.rth_render_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
@@ -226,6 +228,16 @@ class HostRender:
     def set_emitter_sampling(self, on):
         """Render::SetEmitterSampling: next-event estimation on the emissive triangles too (MIS); applies from the next render_frame()."""
         if self.L.rth_render_set_emitter_sampling(self.h, int(bool(on))) != 0:
+            raise _err(self.L)
+
+    def set_environment_sampling(self, on):
+        """Render::SetEnvironmentSampling: next-event estimation on the environment map too (MIS); applies from the next render_frame()."""
+        if self.L.rth_render_set_environment_sampling(self.h, int(bool(on))) != 0:
+            raise _err(self.L)
+
+    def set_light_selection(self, analytic=1.0, emitters=1.0, environment=1.0):
+        """Render::SetLightSelection: relative weights of the light kind drawn at each vertex; applies from the next render_frame()."""
+        if self.L.rth_render_set_light_selection(self.h, float(analytic), float(emitters), float(environment)) != 0:
             raise _err(self.L)
 
     def active_pixels(self):
