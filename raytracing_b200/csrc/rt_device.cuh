@@ -384,8 +384,9 @@ __device__ __forceinline__ f3 sample_bxdf(float s1, f2 s, Material m, f3 normal,
 
 // Emitter sampling (include/rt_b200.h, RT_OPT_EMITTER_SAMPLING): the BSDF that sample_bxdf integrates, evaluated for a given
 // direction `o`, and the density p_b(o) of its non-delta lobes.  Same lobe weights as sample_bxdf:
-//   spec = alpha > 1e-4 and n.h > 0 and h.o > 0 ? (fresnel * (D * G)) * max(n.o, 0) : 0,  h = normalize(i + o), D = ggx_d(alpha, n.h),
-//          G = v_smith(n.i, n.o, alpha)
+//   spec = alpha > 1e-4 and n.h > 0 and h.o > 0 and n.o > 0 ? (fresnel * (D * G)) * n.o : 0,  h = normalize(i + o), D = ggx_d(alpha, n.h),
+//          G = v_smith(n.i, n.o, alpha) (evaluated only above the horizon: below it, with alpha^2 under half an ulp of 1, its
+//          denominator is exactly 0, and inf * 0 would make g NaN)
 //   diff = ((1 - fresnel) * (diffuse_albedo / pi)) * max(n.o, 0);   g = spec + diff;   0 for pass-through materials
 //   p_b  = (n.h > 0 and h.o > 0 ? specular_pdf * (D * n.h / (4 * h.o)) : 0) + diffuse_pdf * (max(n.o, 0) * (1 / pi))
 // The specular terms are 0 when alpha <= 1e-4 (a delta lobe, left to BSDF sampling).  `spec_pdf` and `alpha` let the caller tell
@@ -415,8 +416,11 @@ __device__ __forceinline__ f3 bxdf_eval_sampled(const Material& m, f3 normal, f3
         float D = ggx_d(alpha, n_dot_h);
         if (n_dot_h > 0.0f && h_dot_o > 0.0f)
         {   // the directions the specular sampler reaches with a positive density (it never continues a path elsewhere)
-            float G = v_smith_ggx_correlated(dot(normal, incoming), dot(normal, o), alpha);
-            g = fresnel * splat(D * G) * cos_o + g;
+            if (cos_o > 0.0f)
+            {
+                float G = v_smith_ggx_correlated(dot(normal, incoming), dot(normal, o), alpha);
+                g = fresnel * splat(D * G) * cos_o + g;
+            }
             ps = spec_pdf * (D * n_dot_h / (4.0f * h_dot_o));
         }
     }

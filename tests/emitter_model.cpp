@@ -47,8 +47,11 @@ inline V3 BxdfEvalSampled(const Material& m, V3 normal, V3 incoming, V3 o, float
         float D = GGX_D(*alpha, n_dot_h);
         if (n_dot_h > 0.0f && h_dot_o > 0.0f)
         {
-            float G = V_SmithGGXCorrelated(dot(normal, incoming), dot(normal, o), *alpha);
-            g = fresnel * splat(D * G) * cos_o + g;
+            if (cos_o > 0.0f)
+            {
+                float G = V_SmithGGXCorrelated(dot(normal, incoming), dot(normal, o), *alpha);
+                g = fresnel * splat(D * G) * cos_o + g;
+            }
             ps = *spec_pdf * (D * n_dot_h / (4.0f * h_dot_o));
         }
     }
