@@ -6,7 +6,7 @@
  *
  *   g++ -std=c++17 -O2 -Iinclude -Iraytracing_b200/host examples/headless_render.cpp \
  *       -Lraytracing_b200 -lrt_host -lrt_b200 -Wl,-rpath,'$ORIGIN/../raytracing_b200' -o examples/headless_render
- *   examples/headless_render assets/CornellBox.obj assets/ibl/CGSkies_0036_free.hdr 1920 1080 64 out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1] [env=1] [lights=WA,WE,WV]
+ *   examples/headless_render assets/CornellBox.obj assets/ibl/CGSkies_0036_free.hdr 1920 1080 64 out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1] [env=1] [lights=WA,WE,WV] [--animate N]
  *
  * The optional device list spreads the frame over several GPUs of the node behind the same Render / Integrator objects
  * ("all" = every CUDA device; the image is partitioned by scanline inside the library, rt_create_multi).
@@ -17,6 +17,9 @@
  * emitters=1 turns on emitter sampling (Render::SetEmitterSampling: next-event estimation on the emissive triangles, with MIS).
  * env=1 turns on environment sampling (Render::SetEnvironmentSampling: next-event estimation on the environment map, with MIS).
  * lights=WA,WE,WV sets the weights of the light kind drawn at each vertex (Render::SetLightSelection: analytic, emitters, environment).
+ * --animate N renders N frames of `samples` samples each; before every frame after the first, the triangles of one material (that of
+ * the first triangle in leaf order, a stand-in for "one mesh") move along +z, CameraController's up axis, by 1 % of the scene's z extent (Render::UpdateTriangles: the BVH
+ * is refit on the device, no rebuild) and the accumulation starts over.  The last frame is written.
  *
  * Needs an H100 (there is no CPU fallback: Render's constructor throws without a CUDA device).
  */
@@ -33,7 +36,7 @@
 
 int main(int argc, char** argv)
 {
-    if (argc < 7) { std::fprintf(stderr, "usage: %s scene.obj env.hdr width height samples out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1] [env=1] [lights=WA,WE,WV]\n", argv[0]); return 2; }
+    if (argc < 7) { std::fprintf(stderr, "usage: %s scene.obj env.hdr width height samples out.pfm [all|d0,d1,...] [max_error=E] [denoise=ITER,SC,SN,SZ] [emitters=1] [env=1] [lights=WA,WE,WV] [--animate N]\n", argv[0]); return 2; }
     const unsigned width = (unsigned)std::atoi(argv[3]), height = (unsigned)std::atoi(argv[4]), samples = (unsigned)std::atoi(argv[5]);
     float max_error = 0.0f;                                                                         // 0: every pixel takes every sample
     const char* device_arg = nullptr;
@@ -42,9 +45,14 @@ int main(int argc, char** argv)
     bool emitters = false;                                                                          // emitter sampling off
     bool env = false;                                                                               // environment sampling off
     float light_w[3] = { 0.0f, 0.0f, 0.0f };                                                        // 0: the default weights
+    unsigned frames = 1;                                                                            // --animate N
     for (int i = 7; i < argc; ++i)
     {
-        if (std::string(argv[i]).rfind("max_error=", 0) == 0) max_error = (float)std::atof(argv[i] + 10);
+        if (std::string(argv[i]) == "--animate")
+        {
+            if (i + 1 >= argc || (frames = (unsigned)std::atoi(argv[++i])) == 0) { std::fprintf(stderr, "--animate takes a frame count >= 1\n"); return 2; }
+        }
+        else if (std::string(argv[i]).rfind("max_error=", 0) == 0) max_error = (float)std::atof(argv[i] + 10);
         else if (std::string(argv[i]).rfind("emitters=", 0) == 0) emitters = std::atoi(argv[i] + 9) != 0;
         else if (std::string(argv[i]).rfind("env=", 0) == 0) env = std::atoi(argv[i] + 4) != 0;
         else if (std::string(argv[i]).rfind("lights=", 0) == 0)
@@ -98,6 +106,23 @@ int main(int argc, char** argv)
         {
             render.SetSamplesPerFrame(samples);
             render.RenderFrame();                                                                  // every sample in one call, accumulated
+            if (frames > 1)
+            {   // one mesh (the triangles of the first triangle's material) moves along +z, the up axis of CameraController's
+                // camera, by 1 % of the scene's z extent per frame
+                std::vector<rt_host::Triangle> tris = scene.GetTriangles();                         // leaf order (Render built the BVH)
+                float lo = tris[0].v1.position.z, hi = lo;
+                for (auto const& t : tris) for (auto const* v : { &t.v1, &t.v2, &t.v3 }) { lo = std::min(lo, v->position.z); hi = std::max(hi, v->position.z); }
+                const float step = 0.01f * (hi - lo);
+                for (unsigned frame = 1; frame < frames; ++frame)
+                {
+                    for (auto& t : tris)
+                        if (t.mtlIndex == tris[0].mtlIndex) { t.v1.position.z += step; t.v2.position.z += step; t.v3.position.z += step; }
+                    render.UpdateTriangles(tris.data(), tris.size());
+                    render.NotifyCameraChanged();                                                  // start the accumulation over
+                    render.RenderFrame();
+                }
+            }
+            if (frames > 1) std::printf("animated %u frames of %u samples\n", frames, samples);
         }
         std::FILE* f = std::fopen(argv[6], "wb");
         if (!f) { std::perror(argv[6]); return 1; }

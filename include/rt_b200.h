@@ -381,6 +381,42 @@ int rt_set_spatial_denoiser(rt_ctx* ctx, uint32_t iterations, float sigma_color,
  * accumulation, and works with either option alone. */
 int rt_set_light_selection(rt_ctx* ctx, float analytic, float emitters, float environment);
 
+/* ---- geometry updates (new capability): animated geometry without a BVH rebuild ------------------------------------------------
+ * triangles[i] replaces uploaded triangle i, in the leaf order rt_upload_scene received; n_triangles must equal the upload's count.
+ * Positions, normals and texcoords are taken from the new array; mtlIndex and the padding words are not read (materials and the
+ * emitter list stay those of the upload).  Every derived record becomes what rt_upload_scene derives from the new array
+ * (rt_bvh_layout.h): wtris p1 / e1 / e2, tri_shade, tris_ref (the RtFloat3 .w words included); the end-of-leaf flags are kept.
+ * The BVH keeps its topology and is refit: min(a, b) = (b < a) ? b : a and max(a, b) = (a < b) ? b : a (std::min / std::max as the
+ * reference's Bounds3 uses them), per component.  A leaf box starts at min = FLT_MAX, max = -FLT_MAX and folds, for each of its
+ * triangles in leaf order, tb = Union(Bounds3(p1, p2), p3) (Triangle::GetBounds) by box = Union(box, tb); an interior box is
+ * Union(first child, second child).  The same boxes go into the nodes (xyz of bounds_min / bounds_max; their .w words, the offsets,
+ * counts, split axes and padding are kept) and into the child slots of the parent's traversal record.  With unchanged positions
+ * the boxes equal the builder's as float values (it folds over primitives rather than children, so only the sign of a zero can
+ * differ, which no comparison of the traversal can tell apart).  Non-finite coordinates are not rejected (rt_upload_scene does not
+ * reject them either); the comparisons above define their boxes too.
+ * Ordering: the update is enqueued on the render stream after everything submitted before it (a shadow pass deferred by
+ * RT_OPT_OVERLAP 2 is launched first, the second stream of RT_OPT_OVERLAP 1 is joined) and is asynchronous; the next frame sees the
+ * new geometry.  The buffers keep their sizes and addresses, so a captured frame graph stays valid.  The accumulation is kept, as
+ * for a camera move: call rt_reset.  Motion vectors stay camera-only (as in the reference), so the temporal denoiser gets no help
+ * from an update.  The sort-key origin of the sorted shading pass stays the upload's root-box centre (ray order, not results).
+ * rt_update_triangles reads the caller's array before it returns, through a pinned staging buffer of at most 2 x 32 MB (allocated
+ * at the first call) whose copies overlap the record kernel.  rt_update_triangles_device reads `device_triangles` (RtTriangle
+ * layout, 16-byte aligned device memory of the context's device, else RT_ERR_INVALID_ARGUMENT) on the render stream: the caller
+ * orders its producer before the call (rt_stream_handle) and keeps the buffer unchanged until the next blocking call.
+ * Emitter sampling: while it is on, the emitter table's areas are rebuilt from the new positions (read back from the device), which
+ * makes the call block; otherwise that happens when the option is turned on.  The environment table and the analytic lights are
+ * unaffected.  The first update builds a refit map (parent and record slot per node, the leaf list, an arrival counter per node:
+ * about 14 bytes per node, read from the device copy of the nodes, blocking) that lives until the next rt_upload_scene.
+ * Errors: RT_ERR_NOT_READY before an upload; RT_ERR_INVALID_ARGUMENT for a count mismatch or a null pointer; RT_ERR_UNSUPPORTED for
+ * rt_update_triangles_device on a multi-device context (rt_update_triangles fans out like rt_upload_scene).  The launches count
+ * under RT_K_MISC (RT_OPT_KERNEL_TIMING) and in rt_launch_count. */
+int rt_update_triangles(rt_ctx* ctx, const RtTriangle* triangles, uint64_t n_triangles);
+int rt_update_triangles_device(rt_ctx* ctx, const void* device_triangles, uint64_t n_triangles);
+/* Parity tap: the device's reference-layout nodes (n_nodes entries of the upload) and, if records != NULL, the traversal records
+ * (16 floats per interior record, rt_bvh_layout.h; one zero record for a single-leaf tree); *n_records is set whenever n_records
+ * != NULL (call with records == NULL to size the buffer).  Either pointer may be NULL.  Blocking.  Single-device contexts only. */
+int rt_read_bvh(rt_ctx* ctx, RtLinearBVHNode* nodes, float* records, uint64_t* n_records);
+
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);
 /* Hits of the rays currently in the incoming queue of `bounce` after rt_intersect(bounce): n = live rays;

@@ -36,7 +36,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_create_multi", "rt_device_count", "rt_gather_radiance", "rt_host_register", "rt_host_unregister", "rt_math_eval",
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
-           "rt_set_light_selection"]
+           "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh"]
 
 
 class RtSceneDesc(C.Structure):
@@ -120,6 +120,9 @@ def load_library():
     L.rt_read_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rt_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
     L.rt_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
+    L.rt_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+    L.rt_update_triangles_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+    L.rt_read_bvh.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -147,6 +150,7 @@ class Context:
         if world != 1:
             self._ck(self.lib.rt_set_partition(self.h, rank, world))
         self._keep = None
+        self._update_srcs = []              # (tensor, event on the render stream after its update): update_triangles
 
     def gather_radiance(self):
         self._ck(self.lib.rt_gather_radiance(self.h))
@@ -178,6 +182,7 @@ class Context:
         if self.h:
             self.lib.rt_destroy(self.h)
             self.h = None
+        self._update_srcs = []
 
     def __del__(self):
         try:
@@ -210,6 +215,7 @@ class Context:
         for i in range(4):
             d.scene_info[i] = int(info[i])
         self._ck(self.lib.rt_upload_scene(self.h, C.byref(d)))
+        self._n_nodes = a["nodes"].shape[0]
 
     def set_camera(self, cam):
         c = np.ascontiguousarray(cam, dtype=CAMERA_DT)
@@ -275,6 +281,39 @@ class Context:
         """Relative weights of the light kind drawn at each vertex while emitter or environment sampling is active
         (rt_set_light_selection; a kind's weight counts only while it is active); each finite and > 0."""
         self._ck(self.lib.rt_set_light_selection(self.h, float(analytic), float(emitters), float(environment)))
+
+    # ---- geometry updates
+    def update_triangles(self, tris):
+        """Replace the uploaded triangles (leaf order, same count) and refit the BVH on the device (rt_update_triangles*).
+        A TRIANGLE_DT numpy array goes through the host variant; a contiguous CUDA torch tensor (uint8 (n, 160) or float32
+        (n, 40)) is read on the render stream, which first waits for torch's current stream.  The context holds the tensor
+        until an event recorded on the render stream after the update has completed (checked at every later update, released
+        by destroy(), which drains the stream), so torch's allocator cannot hand its memory out while the update may still read
+        it, even if the caller drops the tensor at once.  (Tensor.record_stream is not used: the render stream is destroyed
+        with the context, and the allocator would later record an event on it.)  The accumulation is kept: call reset()."""
+        if isinstance(tris, np.ndarray):
+            t = np.ascontiguousarray(tris, dtype=TRIANGLE_DT)
+            self._ck(self.lib.rt_update_triangles(self.h, t.ctypes.data, t.shape[0]))
+            return
+        import torch
+        if not (isinstance(tris, torch.Tensor) and tris.is_cuda and tris.is_contiguous() and tris.dim() == 2 and
+                ((tris.dtype == torch.uint8 and tris.shape[1] == 160) or (tris.dtype == torch.float32 and tris.shape[1] == 40))):
+            raise TypeError("update_triangles: a TRIANGLE_DT array, or a contiguous CUDA tensor uint8 (n, 160) / float32 (n, 40)")
+        render = torch.cuda.ExternalStream(self.stream_handle(), device=tris.device)
+        render.wait_stream(torch.cuda.current_stream(tris.device))
+        self._ck(self.lib.rt_update_triangles_device(self.h, C.c_void_p(tris.data_ptr()), tris.shape[0]))
+        read = torch.cuda.Event()
+        read.record(render)
+        self._update_srcs = [(x, e) for x, e in self._update_srcs if not e.query()] + [(tris, read)]
+
+    def read_bvh(self):
+        """-> (nodes: NODE_DT[n_nodes] as the device holds them, records: float32 [n_records, 16] traversal records)."""
+        nodes = np.zeros(self._n_nodes, dtype=NODE_DT)
+        n = C.c_uint64()
+        self._ck(self.lib.rt_read_bvh(self.h, None, None, C.byref(n)))
+        rec = np.zeros((n.value, 16), dtype="<f4")
+        self._ck(self.lib.rt_read_bvh(self.h, nodes.ctypes.data, rec.ctypes.data, C.byref(n)))
+        return nodes, rec
 
     def integrate_stepwise(self, max_bounces):
         """The schedule of Integrator::Integrate (integrator.cpp:35-51), one call per reference virtual."""

@@ -56,6 +56,31 @@ struct WideLayout
 
 inline float int_bits(int v) { float f; memcpy(&f, &v, 4); return f; }
 
+// Record numbering of the interior nodes (interior_order: the depth-first order of build_layout's walk): breadth-first for the
+// first top_n, depth-first for the others.  Returns top_n.
+inline uint32_t number_records(const RtLinearBVHNode* nodes, uint64_t n_nodes, const std::vector<uint32_t>& interior_order,
+                               std::vector<int>& wide_index)
+{
+    const uint32_t n_interior = (uint32_t)interior_order.size();
+    const uint32_t top_n = n_interior < RT_BVH_TOP_RECORDS ? n_interior : RT_BVH_TOP_RECORDS;
+    std::vector<uint32_t> bfs;                     // binary node indices of interior nodes in BFS order (prefix only)
+    bfs.reserve(top_n);
+    if (n_interior > 0) bfs.push_back(0u);
+    for (size_t head = 0; head < bfs.size() && bfs.size() < top_n; ++head)
+    {
+        const RtLinearBVHNode& n = nodes[bfs[head]];
+        const uint32_t kids[2] = { bfs[head] + 1u, n.offset };
+        for (uint32_t k : kids)
+            if ((nodes[k].num_primitives_axis >> 16) == 0 && bfs.size() < top_n) bfs.push_back(k);
+    }
+    std::vector<uint8_t> in_top(n_nodes, 0);
+    for (uint32_t b : bfs) in_top[b] = 1;
+    int next = 0;
+    for (uint32_t b : bfs) wide_index[b] = next++;
+    for (uint32_t node : interior_order) if (!in_top[node]) wide_index[node] = next++;
+    return (uint32_t)bfs.size();
+}
+
 inline bool build_layout(const RtLinearBVHNode* nodes, uint64_t n_nodes, const RtTriangle* tris, uint64_t n_tris,
                          WideLayout& out, std::string& err)
 {
@@ -100,25 +125,7 @@ inline bool build_layout(const RtLinearBVHNode* nodes, uint64_t n_nodes, const R
     // the reference kernel's private stack holds 64 entries (trace_bvh.cl:142)
     if (max_depth > 64) { err = "BVH deeper than the 64-entry traversal stack of trace_bvh.cl:142"; return false; }
     out.max_depth = max_depth;
-    {   // renumber: breadth-first for the first top_n interior nodes, depth-first (the order found above) for the others
-        const uint32_t top_n = (uint32_t)n_interior < RT_BVH_TOP_RECORDS ? (uint32_t)n_interior : RT_BVH_TOP_RECORDS;
-        std::vector<uint32_t> bfs;                     // binary node indices of interior nodes in BFS order (prefix only)
-        bfs.reserve(top_n);
-        if (n_interior > 0) bfs.push_back(0u);
-        for (size_t head = 0; head < bfs.size() && bfs.size() < top_n; ++head)
-        {
-            const RtLinearBVHNode& n = nodes[bfs[head]];
-            const uint32_t kids[2] = { bfs[head] + 1u, n.offset };
-            for (uint32_t k : kids)
-                if ((nodes[k].num_primitives_axis >> 16) == 0 && bfs.size() < top_n) bfs.push_back(k);
-        }
-        std::vector<uint8_t> in_top(n_nodes, 0);
-        for (uint32_t b : bfs) in_top[b] = 1;
-        int next = 0;
-        for (uint32_t b : bfs) wide_index[b] = next++;
-        for (uint32_t node : interior_order) if (!in_top[node]) wide_index[node] = next++;
-        out.top_n = (uint32_t)bfs.size();
-    }
+    out.top_n = number_records(nodes, n_nodes, interior_order, wide_index);
 
     auto ref_of = [&](uint32_t child) -> int {
         const RtLinearBVHNode& c = nodes[child];
@@ -155,6 +162,36 @@ inline bool build_layout(const RtLinearBVHNode* nodes, uint64_t n_nodes, const R
         out.tris[i * 3 + 2] = F4{ e2z, fl, 0.0f, 0.0f };
     }
     return true;
+}
+
+// Refit map of rt_update_triangles, from a node array build_layout has accepted.  For every node reachable from the root:
+// link[n] = (parent node, parent's record * 2 + 0 for its first child / + 1 for its second), RT_REFIT_NONE twice for the root;
+// leaves: the reachable leaves.  Unreachable nodes keep RT_REFIT_NONE and are never refit.
+#define RT_REFIT_NONE 0xFFFFFFFFu
+struct RefitMap { std::vector<uint32_t> link, leaves; };
+
+inline void build_refit_map(const RtLinearBVHNode* nodes, uint64_t n_nodes, RefitMap& m)
+{
+    m.link.assign((size_t)n_nodes * 2, RT_REFIT_NONE);
+    m.leaves.clear();
+    std::vector<uint32_t> interior_order, stack{ 0u };
+    while (!stack.empty())
+    {   // build_layout's walk: the first child is visited first
+        const uint32_t node = stack.back(); stack.pop_back();
+        const RtLinearBVHNode& n = nodes[node];
+        if ((n.num_primitives_axis >> 16) > 0) { m.leaves.push_back(node); continue; }
+        interior_order.push_back(node);
+        stack.push_back(n.offset);
+        stack.push_back(node + 1);
+    }
+    std::vector<int> wide_index(n_nodes, -1);
+    number_records(nodes, n_nodes, interior_order, wide_index);
+    for (uint32_t p : interior_order)
+    {
+        const uint32_t r = (uint32_t)wide_index[p] * 2u;
+        m.link[(size_t)(p + 1) * 2] = p;            m.link[(size_t)(p + 1) * 2 + 1] = r;
+        m.link[(size_t)nodes[p].offset * 2] = p;    m.link[(size_t)nodes[p].offset * 2 + 1] = r + 1u;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------

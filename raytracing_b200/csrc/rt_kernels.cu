@@ -42,6 +42,7 @@
 #include "rt_device.cuh"
 #include "rt_emitters.h"
 #include "rt_envmap.h"
+#include "rt_refit.cuh"
 
 using namespace rt;
 
@@ -1113,6 +1114,13 @@ struct rt_ctx
     DevScene scene = {};
     float4 scene_mid = {};                         // centre of the root box: the origin half of k_shade_queues' sort key
     std::vector<void*> scene_allocs;
+    uint64_t n_tris = 0, n_nodes = 0;              // counts of the upload
+    // geometry updates (rt_update_triangles): the refit map (built at the first update, freed by the next upload) and the host
+    // variant's staging, two halves of pinned and of device memory (allocated at the first host update)
+    uint2* refit_link = nullptr; uint32_t* refit_leaves = nullptr; uint32_t* refit_arrivals = nullptr; uint32_t refit_n_leaves = 0;
+    char* stage_host = nullptr; char* stage_dev = nullptr; size_t stage_half = 0;
+    cudaEvent_t stage_copied[2] = { nullptr, nullptr };
+    bool emit_moved = false;                       // emit_tris' positions predate an update: refresh_lights reads them from tris_ref
     RtCamera camera = {};
     RayGenConsts raygen = {};
 
@@ -1516,6 +1524,16 @@ void free_aov_buffers(rt_ctx* c)
     c->aov_ready = false;
 }   // 8 CTAs x 256 threads = full occupancy target per SM
 
+// the refit map and the staging of rt_update_triangles (the caller has drained the stream)
+void free_refit(rt_ctx* c)
+{
+    cudaFree(c->refit_link); cudaFree(c->refit_leaves); cudaFree(c->refit_arrivals);
+    c->refit_link = nullptr; c->refit_leaves = nullptr; c->refit_arrivals = nullptr; c->refit_n_leaves = 0;
+    cudaFreeHost(c->stage_host); cudaFree(c->stage_dev);
+    c->stage_host = nullptr; c->stage_dev = nullptr; c->stage_half = 0;
+    for (cudaEvent_t& e : c->stage_copied) { if (e) cudaEventDestroy(e); e = nullptr; }
+}
+
 } // namespace
 
 extern "C" {
@@ -1587,6 +1605,7 @@ int rt_destroy(rt_ctx* c)
     for (void* p : c->emit_allocs) cudaFree(p);
     for (void* p : c->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void* p : c->scene_allocs) cudaFree(p);
+    free_refit(c);
     for (auto& t : c->timed) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
     for (auto e : c->event_pool) cudaEventDestroy(e);
     if (c->stream) cudaStreamDestroy(c->stream);
@@ -1630,6 +1649,32 @@ static int refresh_lights(rt_ctx* c)
     ++c->config_gen;
     if ((!c->emitter_sampling && !c->env_sampling) || !c->scene_ready) return RT_OK;
     DevScene& ds = c->scene;
+    if (c->emitter_sampling && c->emit_moved && !c->emit_idx.empty())
+    {   // rt_update_triangles moved the geometry: the emitters' positions (their areas) are read back from tris_ref; their
+        // materials stay those of the upload
+        const size_t n = c->emit_idx.size(), pos_at = (n * 4 + 15) / 16 * 16;
+        std::vector<float4> pos(n * 3);
+        void* d = nullptr;
+        RT_CUDA(c, cudaMalloc(&d, pos_at + n * 48));
+        cudaError_t e = cudaMemcpyAsync(d, c->emit_idx.data(), n * 4, cudaMemcpyHostToDevice, c->stream);
+        if (e == cudaSuccess)
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_gather_positions<<<grid_for((uint32_t)n), 256, 0, c->stream>>>(ds.tris_ref, (const uint32_t*)d, (uint32_t)n, (float4*)((char*)d + pos_at));
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(pos.data(), (char*)d + pos_at, n * 48, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        cudaFree(d);
+        if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "reading the emitters' positions back failed: %s", cudaGetErrorString(e));
+        for (size_t i = 0; i < n; ++i)
+        {
+            memcpy(&c->emit_tris[i].v1.position, &pos[i * 3 + 0], 16);
+            memcpy(&c->emit_tris[i].v2.position, &pos[i * 3 + 1], 16);
+            memcpy(&c->emit_tris[i].v3.position, &pos[i * 3 + 2], 16);
+        }
+        c->emit_moved = false;
+    }
     auto tri_of = [&](uint64_t i) -> const RtTriangle& { return c->emit_tris[i]; };
     rtemit::Table et;
     if (c->emitter_sampling)
@@ -1722,6 +1767,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
     for (void* p : c->scene_allocs) cudaFree(p);
     c->scene_allocs.clear();
+    free_refit(c);
     c->scene_ready = false;
     clear_light_tables(c);
 
@@ -1784,10 +1830,129 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     if (n_emit) { c->emit_mats.assign(s->materials, s->materials + s->n_materials); c->emit_lights.assign(s->lights, s->lights + s->n_lights); }
     else { c->emit_mats.clear(); c->emit_lights.clear(); }
     c->emit_n_tris = s->n_triangles;
+    c->emit_moved = false;
+    c->n_tris = s->n_triangles; c->n_nodes = s->n_nodes;
     c->analytic_lit = rtenv::analytic_lit(s->lights, s->scene_info.analytic_light_count);
     c->scene_ready = true;
     ++c->config_gen;
     return refresh_lights(c);
+}
+
+// ---- geometry updates: rt_update_triangles[_device], rt_read_bvh (include/rt_b200.h)
+
+// The checks both variants share, then the refit map (built from the device copy of the upload's nodes at the first update:
+// a refit rewrites only their boxes) and the ordering after earlier work.
+static int begin_update(rt_ctx* c, const void* triangles, uint64_t n, const char* what)
+{
+    if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "%s: rt_upload_scene has not been called", what);
+    if (!triangles) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: null triangles", what);
+    if (n != c->n_tris) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: %llu triangles, the upload has %llu", what, (unsigned long long)n, (unsigned long long)c->n_tris);
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the geometry this call rewrites
+    if (c->refit_link) return RT_OK;
+    std::vector<RtLinearBVHNode> nodes(c->n_nodes);
+    RT_CUDA(c, cudaMemcpyAsync(nodes.data(), c->scene.nodes_ref, c->n_nodes * sizeof(RtLinearBVHNode), cudaMemcpyDeviceToHost, c->stream));
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    rtbvh::RefitMap m;
+    rtbvh::build_refit_map(nodes.data(), c->n_nodes, m);
+    auto fail = [&](cudaError_t e) { free_refit(c); RT_FAIL(c, RT_ERR_CUDA, "%s: refit map: %s", what, cudaGetErrorString(e)); };
+    cudaError_t e;
+    if ((e = cudaMalloc(&c->refit_link, m.link.size() * 4)) != cudaSuccess || (e = cudaMalloc(&c->refit_leaves, m.leaves.size() * 4)) != cudaSuccess ||
+        (e = cudaMalloc(&c->refit_arrivals, c->n_nodes * 4)) != cudaSuccess ||
+        (e = cudaMemcpy(c->refit_link, m.link.data(), m.link.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess ||
+        (e = cudaMemcpy(c->refit_leaves, m.leaves.data(), m.leaves.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess)
+        return fail(e);
+    c->refit_n_leaves = (uint32_t)m.leaves.size();
+    return RT_OK;
+}
+
+static int launch_refit_records(rt_ctx* c, const void* src, uint32_t first, uint32_t n)
+{
+    DevScene& ds = c->scene;
+    TimedLaunch t(c, RT_K_MISC);
+    k_refit_records<<<grid_for(n), 256, 0, c->stream>>>((const float4*)src, first, n, (float4*)ds.tris_ref, (float4*)ds.wtris, (float4*)ds.tri_shade);
+    return post_launch(c, "k_refit_records");
+}
+
+// The refit, then the emitter table of the moved geometry.  The two refit kernels are plain launches and never execute
+// griddepcontrol.launch_dependents: a traversal kernel launched with programmatic dependent launch stages the BVH before its
+// pdl_wait() (rt_traverse.cuh), so an early trigger would let the next frame stage stale boxes.
+static int finish_update(rt_ctx* c)
+{
+    RT_CUDA(c, cudaMemsetAsync(c->refit_arrivals, 0, c->n_nodes * 4, c->stream));
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        k_refit<<<grid_for(c->refit_n_leaves), 256, 0, c->stream>>>(c->refit_leaves, c->refit_n_leaves, c->refit_link, c->refit_arrivals,
+                                                                     (float*)c->scene.nodes_ref, c->scene.tris_ref, (float*)c->scene.wnodes);
+        int rc = post_launch(c, "k_refit"); if (rc) return rc;
+    }
+    // scene_mid, the origin of k_shade_queues' sort key, stays that of the upload: it orders the continuation rays, which
+    // changes no result.  The buffers keep their addresses, so a captured frame graph stays valid.
+    if (!c->emit_idx.empty()) c->emit_moved = true;
+    return (c->emitter_sampling && !c->emit_idx.empty()) ? refresh_lights(c) : RT_OK;
+}
+
+int rt_update_triangles(rt_ctx* c, const RtTriangle* triangles, uint64_t n)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_update_triangles(k, triangles, n));
+    { int rc = begin_update(c, triangles, n, "rt_update_triangles"); if (rc) return rc; }
+    if (!c->stage_host)
+    {   // two halves of at most 32 MB each: the host copy into one half overlaps the upload and kernel of the other
+        const size_t half = std::min<size_t>((size_t)n * sizeof(RtTriangle), (size_t)32 << 20) / sizeof(RtTriangle) * sizeof(RtTriangle);
+        cudaError_t e;
+        if ((e = cudaMallocHost(&c->stage_host, 2 * half)) != cudaSuccess || (e = cudaMalloc(&c->stage_dev, 2 * half)) != cudaSuccess ||
+            (e = cudaEventCreateWithFlags(&c->stage_copied[0], cudaEventDisableTiming)) != cudaSuccess ||
+            (e = cudaEventCreateWithFlags(&c->stage_copied[1], cudaEventDisableTiming)) != cudaSuccess)
+        {
+            cudaFreeHost(c->stage_host); cudaFree(c->stage_dev); c->stage_host = nullptr; c->stage_dev = nullptr;
+            for (cudaEvent_t& ev : c->stage_copied) { if (ev) cudaEventDestroy(ev); ev = nullptr; }
+            RT_FAIL(c, RT_ERR_CUDA, "rt_update_triangles: staging buffers: %s", cudaGetErrorString(e));
+        }
+        c->stage_half = half;
+    }
+    const uint64_t per_chunk = c->stage_half / sizeof(RtTriangle);
+    for (uint64_t first = 0, k = 0; first < n; first += per_chunk, k ^= 1)
+    {
+        const uint32_t m = (uint32_t)std::min<uint64_t>(per_chunk, n - first);
+        char* h = c->stage_host + k * c->stage_half; char* d = c->stage_dev + k * c->stage_half;
+        RT_CUDA(c, cudaEventSynchronize(c->stage_copied[k]));          // the copy out of this half two chunks ago is done
+        memcpy(h, triangles + first, (size_t)m * sizeof(RtTriangle));
+        RT_CUDA(c, cudaMemcpyAsync(d, h, (size_t)m * sizeof(RtTriangle), cudaMemcpyHostToDevice, c->stream));
+        RT_CUDA(c, cudaEventRecord(c->stage_copied[k], c->stream));
+        int rc = launch_refit_records(c, d, (uint32_t)first, m); if (rc) return rc;
+    }
+    return finish_update(c);
+}
+
+int rt_update_triangles_device(rt_ctx* c, const void* triangles, uint64_t n)
+{
+    RT_CHECK_CTX(c);
+    if (!c->children.empty())
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_update_triangles_device: a multi-device context: use rt_update_triangles (device memory belongs to one device)");
+    if (triangles)
+    {
+        cudaPointerAttributes a = {};
+        if (cudaPointerGetAttributes(&a, triangles) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+        if (a.type != cudaMemoryTypeDevice || a.device != c->device || ((uintptr_t)triangles & 15u))
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_update_triangles_device: not 16-byte aligned device memory of device %d", c->device);
+    }
+    { int rc = begin_update(c, triangles, n, "rt_update_triangles_device"); if (rc) return rc; }
+    { int rc = launch_refit_records(c, triangles, 0, (uint32_t)n); if (rc) return rc; }
+    return finish_update(c);
+}
+
+int rt_read_bvh(rt_ctx* c, RtLinearBVHNode* nodes, float* records, uint64_t* n_records)
+{
+    RT_CHECK_CTX(c); RT_NOT_ON_GROUP(c, "rt_read_bvh");
+    if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_read_bvh: rt_upload_scene has not been called");
+    if (records && !n_records) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_bvh: records without n_records");
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }
+    if (nodes) RT_CUDA(c, cudaMemcpyAsync(nodes, c->scene.nodes_ref, c->n_nodes * sizeof(RtLinearBVHNode), cudaMemcpyDeviceToHost, c->stream));
+    if (records) RT_CUDA(c, cudaMemcpyAsync(records, c->scene.wnodes, (size_t)c->scene.wnodes_f4 * 16, cudaMemcpyDeviceToHost, c->stream));
+    if (n_records) *n_records = c->scene.wnodes_f4 / 4;
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    return RT_OK;
 }
 
 int rt_set_camera(rt_ctx* c, const RtCamera* cam)

@@ -145,6 +145,11 @@ void CUDAPathTraceIntegrator::SetEnvironmentSampling(bool on)
     Check(rt_set_option(ctx_, RT_OPT_ENV_SAMPLING, on ? 1u : 0u), "SetEnvironmentSampling");
 }
 
+void CUDAPathTraceIntegrator::UpdateTriangles(const Triangle* triangles, size_t count)
+{
+    Check(rt_update_triangles(ctx_, triangles, count), "UpdateTriangles");
+}
+
 void CUDAPathTraceIntegrator::SetLightSelection(float analytic, float emitters, float environment)
 {
     Check(rt_set_light_selection(ctx_, analytic, emitters, environment), "SetLightSelection");

@@ -93,6 +93,10 @@ public:
     void SetEnvironmentSampling(bool on);
     // light-kind weights (rt_set_light_selection): analytic, emitters, environment, each finite and > 0.  No reset, as above.
     void SetLightSelection(float analytic, float emitters, float environment);
+    // geometry update (rt_update_triangles): new positions, normals and texcoords for the uploaded triangles (leaf order, same count;
+    // materials are kept); the BVH is refit on the device.  No reset: like a camera move, whether the old samples are kept is the
+    // caller's choice (RequestReset() starts over; an animation that keeps them gets motion blur).
+    void UpdateTriangles(const Triangle* triangles, size_t count);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

@@ -204,6 +204,11 @@ int rth_render_set_light_selection(void* h, float analytic, float emitters, floa
     try { ((RenderHandle*)h)->render->SetLightSelection(analytic, emitters, environment); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_update_triangles(void* h, const RtTriangle* triangles, size_t count)
+{
+    try { ((RenderHandle*)h)->render->UpdateTriangles(reinterpret_cast<const Triangle*>(triangles), count); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_active_pixels(void* h, std::uint32_t* n)
 {
     try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

@@ -53,6 +53,9 @@ public:
     // environment sampling and light-kind weights (CUDAPathTraceIntegrator): apply from the next RenderFrame(), keep the accumulation
     void SetEnvironmentSampling(bool on) { Cuda().SetEnvironmentSampling(on); }
     void SetLightSelection(float analytic, float emitters, float environment) { Cuda().SetLightSelection(analytic, emitters, environment); }
+    // geometry update (CUDAPathTraceIntegrator::UpdateTriangles): the scene's triangles in leaf order, moved; the next RenderFrame()
+    // renders them into the same accumulation unless the caller calls NotifyCameraChanged()
+    void UpdateTriangles(const Triangle* triangles, size_t count) { Cuda().UpdateTriangles(triangles, count); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

@@ -48,6 +48,7 @@ def load_library():
     L.rth_render_set_emitter_sampling.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_environment_sampling.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
+    L.rth_render_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
@@ -238,6 +239,13 @@ class HostRender:
     def set_light_selection(self, analytic=1.0, emitters=1.0, environment=1.0):
         """Render::SetLightSelection: relative weights of the light kind drawn at each vertex; applies from the next render_frame()."""
         if self.L.rth_render_set_light_selection(self.h, float(analytic), float(emitters), float(environment)) != 0:
+            raise _err(self.L)
+
+    def update_triangles(self, triangles):
+        """Render::UpdateTriangles: the scene's triangles in leaf order with new positions, normals and texcoords; the BVH is refit
+        on the device.  Keeps the accumulation (request_reset() starts over)."""
+        t = np.ascontiguousarray(triangles, dtype=TRIANGLE_DT)
+        if self.L.rth_render_update_triangles(self.h, t.ctypes.data, t.shape[0]) != 0:
             raise _err(self.L)
 
     def active_pixels(self):
