@@ -412,10 +412,54 @@ int rt_set_light_selection(rt_ctx* ctx, float analytic, float emitters, float en
  * under RT_K_MISC (RT_OPT_KERNEL_TIMING) and in rt_launch_count. */
 int rt_update_triangles(rt_ctx* ctx, const RtTriangle* triangles, uint64_t n_triangles);
 int rt_update_triangles_device(rt_ctx* ctx, const void* device_triangles, uint64_t n_triangles);
-/* Parity tap: the device's reference-layout nodes (n_nodes entries of the upload) and, if records != NULL, the traversal records
+/* Parity tap: the device's reference-layout nodes (n_nodes entries of the current tree: the upload's, or 2n - 1 after
+ * rt_rebuild_bvh) and, if records != NULL, the traversal records
  * (16 floats per interior record, rt_bvh_layout.h; one zero record for a single-leaf tree); *n_records is set whenever n_records
  * != NULL (call with records == NULL to size the buffer).  Either pointer may be NULL.  Blocking.  Single-device contexts only. */
 int rt_read_bvh(rt_ctx* ctx, RtLinearBVHNode* nodes, float* records, uint64_t* n_records);
+
+/* ---- BVH rebuild (new capability): a fresh tree over the current triangles, built on the device ---------------------------------
+ * Replaces the BVH by a linear BVH (one triangle per leaf, in Morton order) over the device copy of the positions: the upload's
+ * triangles or those of the last rt_update_triangles*.  For geometry that has deformed far enough that a refit tree traces slowly
+ * (DESIGN.md section 4 measures where that happens); nothing is copied from or to the host.  The rule, with n triangles and every
+ * operation in float without contraction, in the order written:
+ *  1. Key point s = (p1 + p2) + p3 per component.  The quantization box lo / hi of an axis is the min / max over the finite s of
+ *     that axis (min and max are exact, so only the sign of a zero depends on the reduction order, which changes no code).
+ *  2. Per axis: k = 1024.0f / (hi - lo) if hi > lo, else 0 (also when no s of the axis is finite); for a finite s, x = (s - lo) * k
+ *     and q = 1023 if x >= 1023, trunc(x) if x > 0, else 0 (so a NaN x gives 0); a non-finite s gives q = 0.
+ *  3. Code: bit j of qx goes to bit 3j + 2, of qy to 3j + 1, of qz to 3j (30 bits).  Key = (uint64(code) << 32) | triangle id; the
+ *     keys are distinct, so their ascending order is unique.
+ *  4. Topology: the binary radix tree of the sorted keys.  A range [a, b] of sorted keys with a < b splits after the unique i at
+ *     which the highest bit h where key[a] and key[b] differ flips; the first child holds the lower keys.  Split axis: with
+ *     m = h - 32, 2 - (m mod 3) if h >= 32, else 0 (equal codes, split by id).  Each level uses up at least one of the 30 + 31 key
+ *     bits, so the depth is at most 62 levels (n < 2^31, the upload's limit), under the 64-entry traversal stack: nothing checks
+ *     it at run time.
+ *  5. Nodes in the reference layout, depth-first preorder (first child = node + 1, second child = `offset`): a leaf has offset =
+ *     its triangle id and num_primitives_axis = 1 << 16; an interior node has offset = its second child and num_primitives_axis =
+ *     its split axis; the .w words and the padding are 0; n = 1 gives a single leaf.  Triangles are not reordered, so primitive
+ *     ids, emissive_indices, the leaf order rt_update_triangles expects and every AOV keep their meaning.  The boxes follow the
+ *     refit rule of the geometry-update block exactly.
+ *  6. The derived records are what rt_upload_scene derives from these nodes (rt_bvh_layout.h build_layout): the traversal
+ *     records in its order (the first min(n - 1, 1024) interior nodes breadth-first, then the rest depth-first), the root
+ *     reference and the breadth-first prefix length, and the wtris end-of-leaf flags, now all 1.  tris_ref, tri_shade and the
+ *     materials are untouched.
+ * Frames after a rebuild are those of the same triangles with these nodes uploaded; against the previous tree, results can differ
+ * only where two triangles tie in t (the closest-hit traversal keeps the first found) or where a ray meets a triangle with a
+ * non-finite coordinate (its test can report t = NaN, and what follows depends on the visiting order with any tree).  The accumulation is kept: call rt_reset
+ * when the geometry moved.  The rebuild also builds the refit map, so a later rt_update_triangles* refits the rebuilt topology
+ * without its blocking map build; rt_upload_scene returns to the uploaded tree.  State derived from the tree (shared-memory
+ * staging of small trees, the RT_OPT_TOP_SMEM prefix) follows the new tree; the sort-key origin of the sorted shading pass stays
+ * the upload's root-box centre, as after an update.  The light tables are unaffected (ids and positions do not change).
+ * Ordering: enqueued on the render stream like an update (a deferred shadow pass is launched first, the second stream is joined).
+ * The first rebuild after an upload replaces the nodes, records and refit map (2n - 1 nodes, max(n - 1, 1) records) and allocates
+ * the build temporaries: it blocks, and the frame graph is re-captured.  Later rebuilds reuse all of them in place: they are
+ * asynchronous and a captured frame graph stays valid.
+ * Device memory while a rebuilt tree is live: nodes 48 B x (2n - 1) and records 64 B x (n - 1) in place of the upload's, the refit
+ * map 12 B x (2n - 1) + 4 B x n, and temporaries of 32 B per triangle plus the radix sort's scratch.
+ * n_nodes, if not NULL, is set to the new node count 2n - 1.  Multi-device contexts fan out: each device builds the same tree.
+ * Errors: RT_ERR_NOT_READY before an upload.  The launches count under RT_K_MISC (RT_OPT_KERNEL_TIMING) and in rt_launch_count
+ * (the radix sort counts as one). */
+int rt_rebuild_bvh(rt_ctx* ctx, uint64_t* n_nodes);
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

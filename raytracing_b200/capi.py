@@ -36,7 +36,8 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_create_multi", "rt_device_count", "rt_gather_radiance", "rt_host_register", "rt_host_unregister", "rt_math_eval",
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
-           "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh"]
+           "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh",
+           "rt_rebuild_bvh"]
 
 
 class RtSceneDesc(C.Structure):
@@ -123,6 +124,7 @@ def load_library():
     L.rt_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     L.rt_update_triangles_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     L.rt_read_bvh.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+    L.rt_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -305,6 +307,14 @@ class Context:
         read = torch.cuda.Event()
         read.record(render)
         self._update_srcs = [(x, e) for x, e in self._update_srcs if not e.query()] + [(tris, read)]
+
+    def rebuild_bvh(self):
+        """Replace the BVH by a linear BVH over the current triangles, built on the device (rt_rebuild_bvh); -> the new node count
+        (2n - 1).  The triangles keep their ids; the accumulation is kept: call reset() if the geometry moved."""
+        n = C.c_uint64()
+        self._ck(self.lib.rt_rebuild_bvh(self.h, C.byref(n)))
+        self._n_nodes = n.value
+        return n.value
 
     def read_bvh(self):
         """-> (nodes: NODE_DT[n_nodes] as the device holds them, records: float32 [n_records, 16] traversal records)."""

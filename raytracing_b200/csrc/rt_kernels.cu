@@ -43,6 +43,7 @@
 #include "rt_emitters.h"
 #include "rt_envmap.h"
 #include "rt_refit.cuh"
+#include "rt_lbvh.cuh"
 
 using namespace rt;
 
@@ -1121,6 +1122,17 @@ struct rt_ctx
     char* stage_host = nullptr; char* stage_dev = nullptr; size_t stage_half = 0;
     cudaEvent_t stage_copied[2] = { nullptr, nullptr };
     bool emit_moved = false;                       // emit_tris' positions predate an update: refresh_lights reads them from tris_ref
+    // rt_rebuild_bvh: the build temporaries of the linear BVH (allocated with its nodes and records at the first rebuild after an
+    // upload, in scene_allocs; live = scene.nodes_ref / wnodes and the refit map hold a rebuilt tree's 2n - 1 nodes)
+    struct Lbvh
+    {
+        bool live = false;
+        uint32_t* bounds = nullptr;                // 6 words: the key-point box of k_lbvh_bounds
+        uint32_t* codes[2] = { nullptr, nullptr }; uint32_t* ids[2] = { nullptr, nullptr };   // the sort's double buffers
+        uint4* inner = nullptr;                    // per internal node: first leaf, last leaf, split, axis
+        uint2* top = nullptr;                      // the breadth-first top records by preorder (k_lbvh_top)
+        void* sort_tmp = nullptr; size_t sort_bytes = 0;
+    } lbvh;
     RtCamera camera = {};
     RayGenConsts raygen = {};
 
@@ -1524,11 +1536,17 @@ void free_aov_buffers(rt_ctx* c)
     c->aov_ready = false;
 }   // 8 CTAs x 256 threads = full occupancy target per SM
 
-// the refit map and the staging of rt_update_triangles (the caller has drained the stream)
-void free_refit(rt_ctx* c)
+// the refit map of rt_update_triangles (the caller has drained the stream)
+void free_refit_map(rt_ctx* c)
 {
     cudaFree(c->refit_link); cudaFree(c->refit_leaves); cudaFree(c->refit_arrivals);
     c->refit_link = nullptr; c->refit_leaves = nullptr; c->refit_arrivals = nullptr; c->refit_n_leaves = 0;
+}
+
+// the refit map and the staging of rt_update_triangles (the caller has drained the stream)
+void free_refit(rt_ctx* c)
+{
+    free_refit_map(c);
     cudaFreeHost(c->stage_host); cudaFree(c->stage_dev);
     c->stage_host = nullptr; c->stage_dev = nullptr; c->stage_half = 0;
     for (cudaEvent_t& e : c->stage_copied) { if (e) cudaEventDestroy(e); e = nullptr; }
@@ -1768,6 +1786,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     for (void* p : c->scene_allocs) cudaFree(p);
     c->scene_allocs.clear();
     free_refit(c);
+    c->lbvh = rt_ctx::Lbvh();
     c->scene_ready = false;
     clear_light_tables(c);
 
@@ -1952,6 +1971,136 @@ int rt_read_bvh(rt_ctx* c, RtLinearBVHNode* nodes, float* records, uint64_t* n_r
     if (records) RT_CUDA(c, cudaMemcpyAsync(records, c->scene.wnodes, (size_t)c->scene.wnodes_f4 * 16, cudaMemcpyDeviceToHost, c->stream));
     if (n_records) *n_records = c->scene.wnodes_f4 / 4;
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    return RT_OK;
+}
+
+// ---- BVH rebuild: rt_rebuild_bvh (include/rt_b200.h, kernels in rt_lbvh.cuh)
+
+// The first rebuild after an upload: the nodes, records and refit map of a tree of 2n - 1 nodes replace the upload's (which a
+// frame in flight may still read: blocking), and the build temporaries are allocated.  Everything is allocated before anything
+// is freed, so a failure leaves the uploaded tree in place.
+static int alloc_lbvh(rt_ctx* c)
+{
+    const size_t n = c->n_tris, nn = 2 * n - 1, n_rec = n > 1 ? n - 1 : 1;
+    std::vector<void*> got;
+    cudaError_t e = cudaSuccess;
+    auto get = [&](size_t bytes) -> void* {
+        void* d = nullptr;
+        if (e == cudaSuccess && (e = cudaMalloc(&d, bytes)) == cudaSuccess) got.push_back(d);
+        return d;
+    };
+    rt_ctx::Lbvh L;
+    L.live = true;
+    void* nodes = get(nn * sizeof(RtLinearBVHNode)); void* wnodes = get(n_rec * 64);
+    void* link = get(nn * 8); void* leaves = get(n * 4); void* arrivals = get(nn * 4);
+    L.bounds = (uint32_t*)get(6 * 4); L.top = (uint2*)get(RT_BVH_TOP_RECORDS * 8); L.inner = (uint4*)get(n_rec * 16);
+    for (int k = 0; k < 2; ++k) { L.codes[k] = (uint32_t*)get(n * 4); L.ids[k] = (uint32_t*)get(n * 4); }
+    if (e == cudaSuccess)
+    {
+        cub::DoubleBuffer<uint32_t> keys(L.codes[0], L.codes[1]), vals(L.ids[0], L.ids[1]);
+        e = cub::DeviceRadixSort::SortPairs(nullptr, L.sort_bytes, keys, vals, (int)n, 0, 30, c->stream);
+        L.sort_tmp = get(L.sort_bytes ? L.sort_bytes : 16);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess)
+    {
+        for (void* p : got) cudaFree(p);
+        RT_FAIL(c, RT_ERR_CUDA, "rt_rebuild_bvh: allocating the rebuilt tree: %s", cudaGetErrorString(e));
+    }
+    DevScene& ds = c->scene;
+    for (const void* old : { (const void*)ds.nodes_ref, (const void*)ds.wnodes })
+    {
+        auto it = std::find(c->scene_allocs.begin(), c->scene_allocs.end(), old);
+        if (it != c->scene_allocs.end()) { cudaFree(*it); c->scene_allocs.erase(it); }
+    }
+    free_refit_map(c);
+    ds.nodes_ref = (const float4*)nodes; ds.wnodes = (const float4*)wnodes;
+    c->refit_link = (uint2*)link; c->refit_leaves = (uint32_t*)leaves; c->refit_arrivals = (uint32_t*)arrivals;
+    for (void* p : got)
+        if (p != link && p != leaves && p != arrivals) c->scene_allocs.push_back(p);
+    c->lbvh = L;
+    ++c->config_gen;                                   // new buffers and sizes: the frame graph is re-captured
+    return RT_OK;
+}
+
+int rt_rebuild_bvh(rt_ctx* c, uint64_t* n_nodes)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_rebuild_bvh(k, n_nodes));
+    if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_rebuild_bvh: rt_upload_scene has not been called");
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the tree this call rewrites
+    if (!c->lbvh.live) { int rc = alloc_lbvh(c); if (rc) return rc; }
+    rt_ctx::Lbvh& L = c->lbvh;
+    DevScene& ds = c->scene;
+    const uint32_t n = (uint32_t)c->n_tris, n_inner = n - 1;
+    const uint32_t top_n = n_inner < RT_BVH_TOP_RECORDS ? n_inner : RT_BVH_TOP_RECORDS;
+    float4* nodes = (float4*)ds.nodes_ref; float4* wnodes = (float4*)ds.wnodes; float4* wtris = (float4*)ds.wtris;
+    // Every launch below is a plain launch (none triggers dependent launches early), like the refit's: the next frame's
+    // traversal kernel, even one launched with programmatic dependent launch, sees the finished tree.
+    if (n == 1)
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        k_lbvh_single<<<1, 1, 0, c->stream>>>(nodes, wnodes, wtris, c->refit_link, c->refit_leaves);
+        int rc = post_launch(c, "k_lbvh_single"); if (rc) return rc;
+    }
+    else
+    {
+        RT_CUDA(c, cudaMemsetAsync(L.bounds, 0, 6 * 4, c->stream));
+        int rc;
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            const uint32_t g = std::min<uint32_t>(grid_for(n).x, (uint32_t)c->num_sms * 8u);
+            k_lbvh_bounds<<<g, 256, 0, c->stream>>>(ds.tris_ref, n, L.bounds);
+            if ((rc = post_launch(c, "k_lbvh_bounds"))) return rc;
+        }
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_keys<<<grid_for(n), 256, 0, c->stream>>>(ds.tris_ref, n, L.bounds, L.codes[0], L.ids[0], wtris);
+            if ((rc = post_launch(c, "k_lbvh_keys"))) return rc;
+        }
+        // a stable sort of the 30-bit codes with the ids (ascending) as values orders the keys (code << 32) | id
+        cub::DoubleBuffer<uint32_t> keys(L.codes[0], L.codes[1]), vals(L.ids[0], L.ids[1]);
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            size_t bytes = L.sort_bytes;
+            RT_CUDA(c, cub::DeviceRadixSort::SortPairs(L.sort_tmp, bytes, keys, vals, (int)n, 0, 30, c->stream));
+            if ((rc = post_launch(c, "DeviceRadixSort"))) return rc;
+        }
+        const uint32_t* codes = keys.Current(); const uint32_t* ids = vals.Current();
+        uint32_t* parent = keys.Alternate(); uint32_t* ipre = vals.Alternate();       // the sort's inputs are dead
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_karras<<<grid_for(n_inner), 256, 0, c->stream>>>(codes, ids, n, L.inner, parent);
+            if ((rc = post_launch(c, "k_lbvh_karras"))) return rc;
+        }
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_number<<<grid_for(n_inner), 256, 0, c->stream>>>(L.inner, parent, n_inner, ipre);
+            if ((rc = post_launch(c, "k_lbvh_number"))) return rc;
+        }
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_top<<<1, 1024, 0, c->stream>>>(L.inner, ipre, top_n, L.top);
+            if ((rc = post_launch(c, "k_lbvh_top"))) return rc;
+        }
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_write<<<grid_for(n_inner), 256, 0, c->stream>>>(L.inner, ipre, ids, L.top, top_n, n_inner, nodes, wnodes,
+                                                                   c->refit_link, c->refit_leaves);
+            if ((rc = post_launch(c, "k_lbvh_write"))) return rc;
+        }
+    }
+    // the boxes: the refit of the new topology (k_refit keeps the box rule in one place)
+    c->n_nodes = 2ull * n - 1; c->refit_n_leaves = n;
+    ds.wnodes_f4 = 4 * (n_inner ? n_inner : 1); ds.top_n = top_n; ds.root_ref = n == 1 ? ~0 : 0;
+    RT_CUDA(c, cudaMemsetAsync(c->refit_arrivals, 0, c->n_nodes * 4, c->stream));
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        k_refit<<<grid_for(n), 256, 0, c->stream>>>(c->refit_leaves, n, c->refit_link, c->refit_arrivals, (float*)nodes, ds.tris_ref,
+                                                    (float*)wnodes);
+        int rc = post_launch(c, "k_refit"); if (rc) return rc;
+    }
+    if (n_nodes) *n_nodes = c->n_nodes;
     return RT_OK;
 }
 

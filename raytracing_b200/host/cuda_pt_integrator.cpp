@@ -150,6 +150,13 @@ void CUDAPathTraceIntegrator::UpdateTriangles(const Triangle* triangles, size_t 
     Check(rt_update_triangles(ctx_, triangles, count), "UpdateTriangles");
 }
 
+std::uint64_t CUDAPathTraceIntegrator::RebuildBvh()
+{
+    std::uint64_t n_nodes = 0;
+    Check(rt_rebuild_bvh(ctx_, &n_nodes), "RebuildBvh");
+    return n_nodes;
+}
+
 void CUDAPathTraceIntegrator::SetLightSelection(float analytic, float emitters, float environment)
 {
     Check(rt_set_light_selection(ctx_, analytic, emitters, environment), "SetLightSelection");

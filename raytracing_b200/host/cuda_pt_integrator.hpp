@@ -97,6 +97,9 @@ public:
     // materials are kept); the BVH is refit on the device.  No reset: like a camera move, whether the old samples are kept is the
     // caller's choice (RequestReset() starts over; an animation that keeps them gets motion blur).
     void UpdateTriangles(const Triangle* triangles, size_t count);
+    // BVH rebuild (rt_rebuild_bvh): replaces the tree by a linear BVH over the current triangles, built on the device, when a refit
+    // no longer traces well; returns the new node count (2n - 1).  Triangle ids do not change.  No reset, as above.
+    std::uint64_t RebuildBvh();
     rt_ctx* Context() const { return ctx_; }
 
 protected:

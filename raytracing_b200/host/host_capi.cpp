@@ -209,6 +209,11 @@ int rth_render_update_triangles(void* h, const RtTriangle* triangles, size_t cou
     try { ((RenderHandle*)h)->render->UpdateTriangles(reinterpret_cast<const Triangle*>(triangles), count); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_rebuild_bvh(void* h, std::uint64_t* n_nodes)
+{
+    try { *n_nodes = ((RenderHandle*)h)->render->RebuildBvh(); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_active_pixels(void* h, std::uint32_t* n)
 {
     try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

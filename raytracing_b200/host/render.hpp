@@ -56,6 +56,9 @@ public:
     // geometry update (CUDAPathTraceIntegrator::UpdateTriangles): the scene's triangles in leaf order, moved; the next RenderFrame()
     // renders them into the same accumulation unless the caller calls NotifyCameraChanged()
     void UpdateTriangles(const Triangle* triangles, size_t count) { Cuda().UpdateTriangles(triangles, count); }
+    // BVH rebuild (CUDAPathTraceIntegrator::RebuildBvh): a device-built tree over the current triangles; returns its node count.
+    // Keeps the accumulation, as above
+    std::uint64_t RebuildBvh() { return Cuda().RebuildBvh(); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

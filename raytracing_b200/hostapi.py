@@ -49,6 +49,7 @@ def load_library():
     L.rth_render_set_environment_sampling.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
     L.rth_render_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.rth_render_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
@@ -247,6 +248,14 @@ class HostRender:
         t = np.ascontiguousarray(triangles, dtype=TRIANGLE_DT)
         if self.L.rth_render_update_triangles(self.h, t.ctypes.data, t.shape[0]) != 0:
             raise _err(self.L)
+
+    def rebuild_bvh(self):
+        """Render::RebuildBvh: a linear BVH over the current triangles, built on the device; -> the new node count (2n - 1).
+        Keeps the accumulation (request_reset() starts over)."""
+        n = C.c_uint64()
+        if self.L.rth_render_rebuild_bvh(self.h, C.byref(n)) != 0:
+            raise _err(self.L)
+        return n.value
 
     def active_pixels(self):
         """Render::ActivePixels: pixels that trace the next sample."""
