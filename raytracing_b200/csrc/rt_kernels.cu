@@ -44,6 +44,7 @@
 #include "rt_envmap.h"
 #include "rt_refit.cuh"
 #include "rt_lbvh.cuh"
+#include "rt_owned.h"
 
 using namespace rt;
 
@@ -1048,9 +1049,9 @@ struct rt_ctx
     std::vector<rt_ctx*> children;
     int present = 0;                               // RT_OPT_PRESENT (groups): 0 parallel read-back, 1 gather to device 0 over NVLink
     float4* gather_buf = nullptr; size_t gather_stride_f4 = 0;   // device 0: the gathered radiance slabs (rt_gather_radiance)
-    std::vector<cudaEvent_t> gather_events;
+    std::vector<Owned<cudaEvent_t>> gather_events;
     uint32_t width = 0, height = 0, rank = 0, world = 1, n_local = 0, local_rows = 0;
-    cudaStream_t stream = nullptr;
+    Owned<cudaStream_t> stream;
     int num_sms = 0;
     std::string error;
 
@@ -1067,8 +1068,8 @@ struct rt_ctx
     int use_graph = 1;
     uint64_t config_gen = 1, graph_gen = 0;     // config_gen changes whenever a launch argument other than FrameDyn may change
     uint32_t graph_max_bounces = 0;
-    cudaGraph_t graph = nullptr;                // kept alive: node handles used for parameter updates belong to it
-    cudaGraphExec_t graph_exec = nullptr;
+    Owned<cudaGraph_t> graph;                   // kept alive: node handles used for parameter updates belong to it
+    Owned<cudaGraphExec_t> graph_exec;
     cudaGraphNode_t graph_set_frame_node = nullptr;
     void* graph_set_frame_func = nullptr;
     uint64_t graph_launches = 0;
@@ -1076,14 +1077,14 @@ struct rt_ctx
     int overlap = 2;               // RT_OPT_OVERLAP
     bool shadow_deferred = false;  // overlap 2: rt_shadow_accumulate(shadow_deferred_bounce) has been requested but not launched yet
     uint32_t shadow_deferred_bounce = 0;
-    cudaStream_t shadow_stream = nullptr;
-    cudaEvent_t ev_shaded = nullptr, ev_shadowed = nullptr;
+    Owned<cudaStream_t> shadow_stream;
+    Owned<cudaEvent_t> ev_shaded, ev_shadowed;
     bool shadow_pending = false;
     // pipelined read-back (rt_resolve_async): second resolve buffer, copy stream, events
     float4* resolved2 = nullptr;
     float4* resolved_full[2] = { nullptr, nullptr };   // whole-frame resolve targets of rt_resolve_gathered
-    cudaStream_t copy_stream = nullptr;
-    cudaEvent_t resolve_done[2] = { nullptr, nullptr }, copy_done[2] = { nullptr, nullptr };
+    Owned<cudaStream_t> copy_stream;
+    Owned<cudaEvent_t> resolve_done[2], copy_done[2];
     bool copy_pending[2] = { false, false };
     uint32_t async_index = 0;
     // AOV + denoiser buffers (allocated on first use)
@@ -1100,30 +1101,27 @@ struct rt_ctx
     // fused gather (rt_set_gather_target): this rank's slab and flag in the presenting device's memory, frames signalled so far
     float4* gather_slab = nullptr; uint32_t* gather_flag = nullptr; uint32_t gather_frame = 0;
     uint32_t gather_sample = 0xFFFFFFFFu;          // sample_count after the last frame that was pushed
-    void* own_gather = nullptr; size_t own_gather_stride = 0;      // the buffer this context allocated (rt_gather_buffer)
-    std::vector<void*> ipc_opened;
+    char* own_gather = nullptr; size_t own_gather_stride = 0;      // the buffer this context allocated (rt_gather_buffer)
     int grid_div = 1;              // contexts that share this device (rt_create_multi lists a device k times): each launches 1/k of the resident CTAs
     int frame_threads = 0;         // RT_OPT_FRAME_THREADS: threads per CTA of k_frame (0 = by partition size)
     size_t n_alloc = 0;            // entries of every per-pixel queue: n_local + one group of 32 per CTA that can be resident (k_frame's regions)
     int* d_bn = nullptr;           // sobol | scrambling | ranking (rt_upload_sampler_tables)
     struct Occupancy { const void* kernel; int threads; size_t smem; int per_sm; };
     std::vector<Occupancy> occupancy;   // resident CTAs per SM of each persistent kernel (resident_per_sm)
-    void* scratch = nullptr; size_t scratch_bytes = 0;
+    char* scratch = nullptr; size_t scratch_bytes = 0;
 
     // scene
     bool scene_ready = false, camera_ready = false;
     DevScene scene = {};
     float4 scene_mid = {};                         // centre of the root box: the origin half of k_shade_queues' sort key
-    std::vector<void*> scene_allocs;
     uint64_t n_tris = 0, n_nodes = 0;              // counts of the upload
     // geometry updates (rt_update_triangles): the refit map (built at the first update, freed by the next upload) and the host
     // variant's staging, two halves of pinned and of device memory (allocated at the first host update)
     uint2* refit_link = nullptr; uint32_t* refit_leaves = nullptr; uint32_t* refit_arrivals = nullptr; uint32_t refit_n_leaves = 0;
-    char* stage_host = nullptr; char* stage_dev = nullptr; size_t stage_half = 0;
-    cudaEvent_t stage_copied[2] = { nullptr, nullptr };
+    struct Staging { DevAllocs mem; char* host = nullptr; char* dev = nullptr; size_t half = 0; Owned<cudaEvent_t> copied[2]; };
     bool emit_moved = false;                       // emit_tris' positions predate an update: refresh_lights reads them from tris_ref
     // rt_rebuild_bvh: the build temporaries of the linear BVH (allocated with its nodes and records at the first rebuild after an
-    // upload, in scene_allocs; live = scene.nodes_ref / wnodes and the refit map hold a rebuilt tree's 2n - 1 nodes)
+    // upload, in tree_mem; live = scene.nodes_ref / wnodes and the refit map hold a rebuilt tree's 2n - 1 nodes)
     struct Lbvh
     {
         bool live = false;
@@ -1131,7 +1129,7 @@ struct rt_ctx
         uint32_t* codes[2] = { nullptr, nullptr }; uint32_t* ids[2] = { nullptr, nullptr };   // the sort's double buffers
         uint4* inner = nullptr;                    // per internal node: first leaf, last leaf, split, axis
         uint2* top = nullptr;                      // the breadth-first top records by preorder (k_lbvh_top)
-        void* sort_tmp = nullptr; size_t sort_bytes = 0;
+        char* sort_tmp = nullptr; size_t sort_bytes = 0;
     } lbvh;
     RtCamera camera = {};
     RayGenConsts raygen = {};
@@ -1152,7 +1150,6 @@ struct rt_ctx
     std::vector<RtPackedMaterial> emit_mats;
     std::vector<RtLight> emit_lights;
     uint64_t emit_n_tris = 0;
-    std::vector<void*> emit_allocs;                // the device emitter and environment tables
     // environment sampling (RT_OPT_ENV_SAMPLING, its table scene.env_* built from the device image) and the light-kind weights
     // (rt_set_light_selection; analytic_lit: an analytic light of the upload has non-zero radiance)
     int env_sampling = 0;
@@ -1172,11 +1169,25 @@ struct rt_ctx
     uint64_t launches = 0;
 
     // kernel timing
-    struct Timed { cudaEvent_t a, b; int cls; };
+    struct Timed { Owned<cudaEvent_t> a, b; int cls; };
     std::vector<Timed> timed;
-    std::vector<cudaEvent_t> event_pool;
+    std::vector<Owned<cudaEvent_t>> event_pool;
     float ms[RT_K_CLASS_COUNT] = {};
     uint32_t nlaunch[RT_K_CLASS_COUNT] = {};
+
+    // The device memory, one group per lifetime.  Declared last, so freed before the streams and events that order work on it.
+    DevAllocs ctx_mem;             // counters, counters_sum, d_dyn, d_bn, resolved_full: the context's
+    DevAllocs scratch_mem;         // scratch, replaced when it has to grow
+    DevAllocs gather_mem;          // own_gather (rt_gather_buffer), or a multi-device context's gather_buf
+    DevAllocs frame_mem;           // q, radiance, resolved, resolved2: the partition's
+    DevAllocs aov_mem;             // aov_*, prev_radiance, prev_depth: from the first use to the next partition
+    DevAllocs sd_mem;              // sd_col, sd_guide: while the spatial denoiser is on
+    DevAllocs ad_mem;              // ad: while adaptive sampling is on
+    DevAllocs scene_mem;           // the upload's arrays but the tree
+    DevAllocs tree_mem;            // scene.nodes_ref, scene.wnodes, the refit map, lbvh's temporaries
+    Staging stage;                 // rt_update_triangles' staging
+    DevAllocs light_mem;           // the emitter and environment tables
+    std::vector<std::unique_ptr<void, IpcClose>> ipc_opened;
 };
 
 static std::string g_create_error;
@@ -1225,20 +1236,20 @@ namespace
 
 struct TimedLaunch
 {
-    rt_ctx* c; int cls; cudaEvent_t a = nullptr, b = nullptr; cudaStream_t st;
+    rt_ctx* c; int cls; Owned<cudaEvent_t> a, b; cudaStream_t st;
     TimedLaunch(rt_ctx* ctx, int k, cudaStream_t stream = nullptr) : c(ctx), cls(k), st(stream ? stream : ctx->stream)
     {
         ++c->launches;
         if (!c->kernel_timing) return;
-        auto get = [&]() { cudaEvent_t e; if (!c->event_pool.empty()) { e = c->event_pool.back(); c->event_pool.pop_back(); } else cudaEventCreate(&e); return e; };
-        a = get(); b = get();
+        auto get = [&](Owned<cudaEvent_t>& e) { if (!c->event_pool.empty()) { e = std::move(c->event_pool.back()); c->event_pool.pop_back(); } else make_event(e, cudaEventDefault); };
+        get(a); get(b);
         cudaEventRecord(a, st);
     }
     ~TimedLaunch()
     {
         if (!a) return;
         cudaEventRecord(b, st);
-        c->timed.push_back({ a, b, cls });
+        c->timed.push_back({ std::move(a), std::move(b), cls });
     }
 };
 
@@ -1284,29 +1295,22 @@ FrameParams frame_params(const rt_ctx* c)
     return p;
 }
 
+// The frame group exists unless the last rt_set_partition could not allocate it.
+int frame_buffers_ready(rt_ctx* c)
+{
+    if (!c->radiance) RT_FAIL(c, RT_ERR_NOT_READY, "frame buffers could not be allocated: call rt_set_partition again");
+    return RT_OK;
+}
+
 int require_ready(rt_ctx* c)
 {
     if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_upload_scene has not been called");
     if (!c->camera_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_set_camera has not been called");
-    return RT_OK;
+    return frame_buffers_ready(c);
 }
 
-void free_aov_buffers(rt_ctx* c);
 bool aov_wanted(const rt_ctx* c);
 int ensure_aov_buffers(rt_ctx* c);
-
-// the per-pixel buffers: queues, radiance, resolve targets, AOVs
-void free_frame_buffers(rt_ctx* c)
-{
-    auto freep = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
-    for (int i = 0; i < 2; ++i) { freep(c->q.A[i]); freep(c->q.B[i]); freep(c->q.C[i]); }
-    freep(c->q.sA); freep(c->q.sB); freep(c->q.sC); freep(c->q.hits); freep(c->q.shadow_flags);
-    freep(c->q.hitq); freep(c->q.missq);
-    freep(c->radiance); freep(c->resolved); freep(c->resolved2);
-    freep(c->sd_col[0]); freep(c->sd_col[1]); freep(c->sd_guide);
-    free_aov_buffers(c);
-    freep(c->ad.count); freep(c->ad.y_prev); freep(c->ad.q); freep(c->ad.list); freep(c->ad.tile); freep(c->ad.ctl);
-}
 
 // ---- adaptive sampling: the active setting is on / either setting is on (what the refused combinations check)
 bool adaptive_on(const rt_ctx* c) { return c->ad_error > 0.0f; }
@@ -1315,25 +1319,22 @@ uint32_t adaptive_tiles(const rt_ctx* c) { return std::max((c->n_local + RT_AD_T
 
 // The per-pixel state for the current partition (allocated on first use) reset to: every local pixel active, counts and
 // estimators zero.
-void free_adaptive(rt_ctx* c);
-
 int reset_adaptive(rt_ctx* c)
 {
     const size_t n = std::max(c->n_local, 1u), tiles = adaptive_tiles(c);
-    // each buffer on its own: after a failed allocation the next call allocates only what is missing (free_adaptive frees all)
-    auto alloc = [&](auto*& ptr, size_t bytes) -> int {
-        if (ptr) return RT_OK;
+    if (!c->ad.count)
+    {
         ++c->config_gen;
-        RT_CUDA(c, cudaMalloc(&ptr, bytes));
-        return RT_OK;
-    };
-    int rc;
-    if ((rc = alloc(c->ad.count, n * 4)) || (rc = alloc(c->ad.y_prev, n * 4)) || (rc = alloc(c->ad.q, n * 8)) || (rc = alloc(c->ad.list, n * 4)) ||
-        (rc = alloc(c->ad.tile, tiles * 8)) || (rc = alloc(c->ad.ctl, sizeof(AdaptiveCtl))))
-    {   // the frames run with the feature off until a later rt_reset succeeds (the requested setting stays)
-        free_adaptive(c);
-        c->ad_error = 0.0f; c->ad_min = 0;
-        return rc;
+        DevAllocs g;
+        AdaptiveState a = {};
+        cudaError_t e;
+        if ((e = g.alloc(a.count, n)) || (e = g.alloc(a.y_prev, n)) || (e = g.alloc(a.q, n)) || (e = g.alloc(a.list, n)) ||
+            (e = g.alloc(a.tile, tiles)) || (e = g.alloc(a.ctl, 1)))
+        {   // the frames run with the feature off until a later rt_reset succeeds (the requested setting stays)
+            c->ad_error = 0.0f; c->ad_min = 0;
+            RT_FAIL(c, RT_ERR_CUDA, "allocating the adaptive-sampling state failed: %s", cudaGetErrorString(e));
+        }
+        c->ad_mem = std::move(g); c->ad = a;
     }
     RT_CUDA(c, cudaMemsetAsync(c->ad.count, 0, n * 4, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->ad.y_prev, 0, n * 4, c->stream));
     RT_CUDA(c, cudaMemsetAsync(c->ad.q, 0, n * 8, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->ad.tile, 0, tiles * 8, c->stream));
@@ -1341,15 +1342,6 @@ int reset_adaptive(rt_ctx* c)
     TimedLaunch t(c, RT_K_MISC);
     k_adaptive_init<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->ad, c->n_local);
     return post_launch(c, "k_adaptive_init");
-}
-
-void free_adaptive(rt_ctx* c)
-{
-    if (!c->ad.count && !c->ad.y_prev && !c->ad.q && !c->ad.list && !c->ad.tile && !c->ad.ctl) return;
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    cudaFree(c->ad.count); cudaFree(c->ad.y_prev); cudaFree(c->ad.q); cudaFree(c->ad.list); cudaFree(c->ad.tile); cudaFree(c->ad.ctl);
-    c->ad = AdaptiveState{};
-    ++c->config_gen;
 }
 
 // the convergence update that closes a sample (rt_advance_sample_count, after k_frame, and a node of the per-phase frame graph)
@@ -1367,20 +1359,25 @@ int alloc_frame_buffers(rt_ctx* c)
     if (c->copy_stream) cudaStreamSynchronize(c->copy_stream); // a pipelined read-back may still be reading the resolve buffers
     c->shadow_pending = false; c->shadow_deferred = false;     // the frame in flight (if any) is abandoned with its buffers
     ++c->config_gen;
-    free_frame_buffers(c);
+    // the per-pixel buffers go before the new ones are allocated, so that the peak does not hold both
+    c->frame_mem.clear(); c->sd_mem.clear(); c->aov_mem.clear(); c->ad_mem.clear();
+    c->q = {}; c->radiance = c->resolved = c->resolved2 = nullptr; c->sd_col[0] = c->sd_col[1] = c->sd_guide = nullptr;
+    c->aov_albedo = c->aov_normal = c->prev_radiance = nullptr; c->aov_depth = c->prev_depth = nullptr; c->aov_velocity = nullptr;
+    c->ad = {}; c->aov_ready = false;
     c->local_rows = (c->height > c->rank) ? (c->height - c->rank + c->world - 1) / c->world : 0;
     c->n_local = c->local_rows * c->width;
     // k_frame gives every resident CTA its own region of each queue, rounded up to whole groups of 32 slots
     size_t n = (size_t)c->n_local + 32u + (size_t)c->num_sms * 32u * 32u;       // up to 32 resident CTAs per SM
     c->n_alloc = n;
-    for (int i = 0; i < 2; ++i)
-    {
-        RT_CUDA(c, cudaMalloc(&c->q.A[i], n * 16)); RT_CUDA(c, cudaMalloc(&c->q.B[i], n * 16)); RT_CUDA(c, cudaMalloc(&c->q.C[i], n * 16));
-    }
-    RT_CUDA(c, cudaMalloc(&c->q.sA, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.sB, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.sC, n * 16));
-    RT_CUDA(c, cudaMalloc(&c->q.hits, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.shadow_flags, n * 4));
-    RT_CUDA(c, cudaMalloc(&c->q.hitq, n * 16)); RT_CUDA(c, cudaMalloc(&c->q.missq, n * 4));
-    RT_CUDA(c, cudaMalloc(&c->radiance, n * 16)); RT_CUDA(c, cudaMalloc(&c->resolved, n * 16));
+    DevAllocs g;
+    Queues q = {};
+    float4 *radiance = nullptr, *resolved = nullptr;
+    cudaError_t e = cudaSuccess;
+    auto get = [&](auto*& view) { if (e == cudaSuccess) e = g.alloc(view, n); };
+    for (int i = 0; i < 2; ++i) { get(q.A[i]); get(q.B[i]); get(q.C[i]); }
+    get(q.sA); get(q.sB); get(q.sC); get(q.hits); get(q.shadow_flags); get(q.hitq); get(q.missq); get(radiance); get(resolved);
+    if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "allocating the frame buffers failed: %s", cudaGetErrorString(e));
+    c->frame_mem = std::move(g); c->q = q; c->radiance = radiance; c->resolved = resolved;
     RT_CUDA(c, cudaMemsetAsync(c->radiance, 0, n * 16, c->stream));
     c->copy_pending[0] = c->copy_pending[1] = false;          // both streams were drained above
     if (adaptive_on(c)) { int rc = reset_adaptive(c); if (rc) return rc; }   // every pixel of the new partition active again
@@ -1518,38 +1515,27 @@ int ensure_aov_buffers(rt_ctx* c)
     ++c->config_gen;
     c->aov_ready = false;
     size_t n = c->n_local ? c->n_local : 1;
-    RT_CUDA(c, cudaMalloc(&c->aov_albedo, n * 16)); RT_CUDA(c, cudaMalloc(&c->aov_depth, n * 4));
-    RT_CUDA(c, cudaMalloc(&c->aov_normal, n * 16)); RT_CUDA(c, cudaMalloc(&c->aov_velocity, n * 8));
-    RT_CUDA(c, cudaMalloc(&c->prev_radiance, n * 16)); RT_CUDA(c, cudaMalloc(&c->prev_depth, n * 4));
+    DevAllocs g;
+    float4 *albedo = nullptr, *normal = nullptr, *prev_radiance = nullptr; float *depth = nullptr, *prev_depth = nullptr; float2* velocity = nullptr;
+    cudaError_t e;
+    if ((e = g.alloc(albedo, n)) || (e = g.alloc(depth, n)) || (e = g.alloc(normal, n)) || (e = g.alloc(velocity, n)) ||
+        (e = g.alloc(prev_radiance, n)) || (e = g.alloc(prev_depth, n)))
+        RT_FAIL(c, RT_ERR_CUDA, "allocating the AOV buffers failed: %s", cudaGetErrorString(e));
+    c->aov_mem = std::move(g); c->aov_albedo = albedo; c->aov_depth = depth; c->aov_normal = normal; c->aov_velocity = velocity;
+    c->prev_radiance = prev_radiance; c->prev_depth = prev_depth;
     RT_CUDA(c, cudaMemsetAsync(c->aov_albedo, 0, n * 16, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->aov_depth, 0, n * 4, c->stream));
     RT_CUDA(c, cudaMemsetAsync(c->aov_normal, 0, n * 16, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->aov_velocity, 0, n * 8, c->stream));
     RT_CUDA(c, cudaMemsetAsync(c->prev_radiance, 0, n * 16, c->stream)); RT_CUDA(c, cudaMemsetAsync(c->prev_depth, 0, n * 4, c->stream));
     return RT_OK;
 }
 
-void free_aov_buffers(rt_ctx* c)
+int ensure_scratch(rt_ctx* c, size_t bytes)
 {
-    cudaFree(c->aov_albedo); cudaFree(c->aov_depth); cudaFree(c->aov_normal); cudaFree(c->aov_velocity);
-    cudaFree(c->prev_radiance); cudaFree(c->prev_depth);
-    c->aov_albedo = nullptr; c->aov_depth = nullptr; c->aov_normal = nullptr; c->aov_velocity = nullptr;
-    c->prev_radiance = nullptr; c->prev_depth = nullptr;
-    c->aov_ready = false;
-}   // 8 CTAs x 256 threads = full occupancy target per SM
-
-// the refit map of rt_update_triangles (the caller has drained the stream)
-void free_refit_map(rt_ctx* c)
-{
-    cudaFree(c->refit_link); cudaFree(c->refit_leaves); cudaFree(c->refit_arrivals);
-    c->refit_link = nullptr; c->refit_leaves = nullptr; c->refit_arrivals = nullptr; c->refit_n_leaves = 0;
-}
-
-// the refit map and the staging of rt_update_triangles (the caller has drained the stream)
-void free_refit(rt_ctx* c)
-{
-    free_refit_map(c);
-    cudaFreeHost(c->stage_host); cudaFree(c->stage_dev);
-    c->stage_host = nullptr; c->stage_dev = nullptr; c->stage_half = 0;
-    for (cudaEvent_t& e : c->stage_copied) { if (e) cudaEventDestroy(e); e = nullptr; }
+    if (c->scratch_bytes >= bytes) return RT_OK;
+    c->scratch_mem.clear(); c->scratch = nullptr; c->scratch_bytes = 0;
+    RT_CUDA(c, c->scratch_mem.alloc(c->scratch, bytes));
+    c->scratch_bytes = bytes;
+    return RT_OK;
 }
 
 } // namespace
@@ -1573,9 +1559,9 @@ int rt_create(uint32_t width, uint32_t height, int device, rt_ctx** out_ctx)
         return RT_ERR_NO_DEVICE;
     }
     if (device < 0 || device >= ndev) { g_create_error = "rt_create: device index out of range"; return RT_ERR_INVALID_ARGUMENT; }
-    rt_ctx* c = new rt_ctx;
+    std::unique_ptr<rt_ctx> c(new rt_ctx);
     c->device = device; c->width = width; c->height = height;
-    auto fail = [&](const char* what, cudaError_t err) { g_create_error = std::string("rt_create: ") + what + ": " + cudaGetErrorString(err); delete c; return RT_ERR_CUDA; };
+    auto fail = [&](const char* what, cudaError_t err) { g_create_error = std::string("rt_create: ") + what + ": " + cudaGetErrorString(err); return RT_ERR_CUDA; };
     if ((e = cudaSetDevice(device)) != cudaSuccess) return fail("cudaSetDevice", e);
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail("cudaGetDeviceProperties", e);
@@ -1583,51 +1569,25 @@ int rt_create(uint32_t width, uint32_t height, int device, rt_ctx** out_ctx)
     if ((e = cudaFuncSetAttribute(k_shade_queues<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess ||
         (e = cudaFuncSetAttribute(k_shade_queues<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess)
         return fail("cudaFuncSetAttribute(k_shade_queues)", e);
-    if ((e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
-    if ((e = cudaMalloc(&c->counters, sizeof(DevCounters))) != cudaSuccess) return fail("cudaMalloc(counters)", e);
-    if ((e = cudaMalloc(&c->d_dyn, sizeof(FrameDyn))) != cudaSuccess) return fail("cudaMalloc(frame constants)", e);
+    if ((e = make_stream(c->stream)) != cudaSuccess) return fail("cudaStreamCreate", e);
+    if ((e = c->ctx_mem.alloc(c->counters, 1)) != cudaSuccess) return fail("cudaMalloc(counters)", e);
+    if ((e = c->ctx_mem.alloc(c->d_dyn, 1)) != cudaSuccess) return fail("cudaMalloc(frame constants)", e);
     cudaMemsetAsync(c->d_dyn, 0, sizeof(FrameDyn), c->stream);
     cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream);
-    int rc = alloc_frame_buffers(c);
-    if (rc != RT_OK) { g_create_error = c->error; rt_destroy(c); return rc; }
-    *out_ctx = c;
+    int rc = alloc_frame_buffers(c.get());
+    if (rc != RT_OK) { g_create_error = c->error; return rc; }
+    *out_ctx = c.release();
     return RT_OK;
 }
 
 int rt_destroy(rt_ctx* c)
 {
     if (!c) return RT_ERR_INVALID_ARGUMENT;
-    if (!c->children.empty())
-    {   // multi-device context: the gather buffer lives on the first child's device
-        cudaSetDevice(c->children[0]->device);
-        for (rt_ctx* k : c->children) if (k->stream) cudaStreamSynchronize(k->stream);
-        cudaFree(c->gather_buf);
-        for (cudaEvent_t e : c->gather_events) cudaEventDestroy(e);
-        for (rt_ctx* k : c->children) rt_destroy(k);
-        delete c;
-        return RT_OK;
-    }
-    cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    if (c->shadow_stream) cudaStreamSynchronize(c->shadow_stream);
-    free_frame_buffers(c);
-    cudaFree(c->counters); cudaFree(c->counters_sum); cudaFree(c->scratch); cudaFree(c->d_dyn); cudaFree(c->d_bn); cudaFree(c->resolved_full[0]); cudaFree(c->resolved_full[1]);
-    if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
-    if (c->graph) cudaGraphDestroy(c->graph);
-    if (c->shadow_stream) { cudaStreamSynchronize(c->shadow_stream); cudaStreamDestroy(c->shadow_stream); }
-    if (c->ev_shaded) cudaEventDestroy(c->ev_shaded);
-    if (c->ev_shadowed) cudaEventDestroy(c->ev_shadowed);
-    for (int i = 0; i < 2; ++i) { if (c->resolve_done[i]) cudaEventDestroy(c->resolve_done[i]); if (c->copy_done[i]) cudaEventDestroy(c->copy_done[i]); }
-    if (c->copy_stream) { cudaStreamSynchronize(c->copy_stream); cudaStreamDestroy(c->copy_stream); }
-    cudaFree(c->own_gather);
-    for (void* p : c->emit_allocs) cudaFree(p);
-    for (void* p : c->ipc_opened) cudaIpcCloseMemHandle(p);
-    for (void* p : c->scene_allocs) cudaFree(p);
-    free_refit(c);
-    for (auto& t : c->timed) { cudaEventDestroy(t.a); cudaEventDestroy(t.b); }
-    for (auto e : c->event_pool) cudaEventDestroy(e);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    for (rt_ctx* k : c->children) rt_destroy(k);
+    cudaSetDevice(c->device);            // a multi-device context's is its first child's, where the gather buffer lives
+    for (cudaStream_t s : { c->stream.get(), c->shadow_stream.get(), c->copy_stream.get() })
+        if (s) cudaStreamSynchronize(s);
+    delete c;                            // the owners free the buffers, then destroy the events and streams
     return RT_OK;
 }
 
@@ -1645,10 +1605,19 @@ int rt_set_partition(rt_ctx* c, uint32_t rank, uint32_t world)
     return alloc_frame_buffers(c);
 }
 
+// Copies `bytes` from the host into a new block of g (16 bytes for an empty array) and points *dst at it.
+static int upload_to(rt_ctx* c, DevAllocs& g, const void* src, size_t bytes, const void** dst)
+{
+    char* d = nullptr;
+    RT_CUDA(c, g.alloc(d, bytes ? bytes : 16));
+    if (bytes) RT_CUDA(c, cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
+    *dst = d;
+    return RT_OK;
+}
+
 static void clear_light_tables(rt_ctx* c)
 {
-    for (void* p : c->emit_allocs) cudaFree(p);
-    c->emit_allocs.clear();
+    c->light_mem.clear();
     DevScene& ds = c->scene;
     ds.emit_pdfA = nullptr; ds.emit_cdf = nullptr; ds.emit_list = nullptr; ds.n_emit = 0; ds.emit_pe = 0.0f;
     ds.env_marg = nullptr; ds.env_cond = nullptr; ds.env_pdf = nullptr; ds.light_pev = 0.0f; ds.no_analytic = 0;
@@ -1672,19 +1641,16 @@ static int refresh_lights(rt_ctx* c)
         // materials stay those of the upload
         const size_t n = c->emit_idx.size(), pos_at = (n * 4 + 15) / 16 * 16;
         std::vector<float4> pos(n * 3);
-        void* d = nullptr;
-        RT_CUDA(c, cudaMalloc(&d, pos_at + n * 48));
-        cudaError_t e = cudaMemcpyAsync(d, c->emit_idx.data(), n * 4, cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess)
+        { int rc = ensure_scratch(c, pos_at + n * 48); if (rc) return rc; }
+        char* d = c->scratch;
+        RT_CUDA(c, cudaMemcpyAsync(d, c->emit_idx.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
         {
             TimedLaunch t(c, RT_K_MISC);
-            k_gather_positions<<<grid_for((uint32_t)n), 256, 0, c->stream>>>(ds.tris_ref, (const uint32_t*)d, (uint32_t)n, (float4*)((char*)d + pos_at));
-            e = cudaGetLastError();
+            k_gather_positions<<<grid_for((uint32_t)n), 256, 0, c->stream>>>(ds.tris_ref, (const uint32_t*)d, (uint32_t)n, (float4*)(d + pos_at));
+            int rc = post_launch(c, "k_gather_positions"); if (rc) return rc;
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(pos.data(), (char*)d + pos_at, n * 48, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        cudaFree(d);
-        if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "reading the emitters' positions back failed: %s", cudaGetErrorString(e));
+        RT_CUDA(c, cudaMemcpyAsync(pos.data(), d + pos_at, n * 48, cudaMemcpyDeviceToHost, c->stream));
+        RT_CUDA(c, cudaStreamSynchronize(c->stream));
         for (size_t i = 0; i < n; ++i)
         {
             memcpy(&c->emit_tris[i].v1.position, &pos[i * 3 + 0], 16);
@@ -1709,32 +1675,27 @@ static int refresh_lights(rt_ctx* c)
     }
     if (!emit_active && !env_active) return RT_OK;
     const rtenv::Selection sel = rtenv::select(c->analytic_lit, emit_active, env_active, c->light_w[0], c->light_w[1], c->light_w[2]);
-    auto upload = [&](const void* src, size_t bytes, const void** dst) -> int {
-        void* d = nullptr;
-        RT_CUDA(c, cudaMalloc(&d, bytes));
-        c->emit_allocs.push_back(d);
-        RT_CUDA(c, cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
-        *dst = d;
-        return RT_OK;
-    };
+    DevAllocs g;
+    DevScene lt = ds;                                  // the tables take effect together, once every upload has succeeded
     int rc;
     if (emit_active)
     {
         rtemit::build(tri_of, c->emit_idx.data(), c->emit_idx.size(), c->emit_n_tris, c->emit_mats.data(), c->emit_lights.data(),
                       ds.light_count, c->white_furnace != 0, et, sel.p_e);
-        if ((rc = upload(et.pdfA.data(), et.pdfA.size() * 4, (const void**)&ds.emit_pdfA))) return rc;
-        if ((rc = upload(et.cdf.data(), et.cdf.size() * 4, (const void**)&ds.emit_cdf))) return rc;
-        if ((rc = upload(et.list.data(), et.list.size() * 4, (const void**)&ds.emit_list))) return rc;
-        ds.n_emit = (uint32_t)et.list.size(); ds.emit_pe = et.p_e;
+        if ((rc = upload_to(c, g, et.pdfA.data(), et.pdfA.size() * 4, (const void**)&lt.emit_pdfA))) return rc;
+        if ((rc = upload_to(c, g, et.cdf.data(), et.cdf.size() * 4, (const void**)&lt.emit_cdf))) return rc;
+        if ((rc = upload_to(c, g, et.list.data(), et.list.size() * 4, (const void**)&lt.emit_list))) return rc;
+        lt.n_emit = (uint32_t)et.list.size(); lt.emit_pe = et.p_e;
     }
     if (env_active)
     {
         rtenv::scale(vt, sel.p_v);
-        if ((rc = upload(vt.marg.data(), vt.marg.size() * 4, (const void**)&ds.env_marg))) return rc;
-        if ((rc = upload(vt.cond.data(), vt.cond.size() * 4, (const void**)&ds.env_cond))) return rc;
-        if ((rc = upload(vt.pdf.data(), vt.pdf.size() * 4, (const void**)&ds.env_pdf))) return rc;
+        if ((rc = upload_to(c, g, vt.marg.data(), vt.marg.size() * 4, (const void**)&lt.env_marg))) return rc;
+        if ((rc = upload_to(c, g, vt.cond.data(), vt.cond.size() * 4, (const void**)&lt.env_cond))) return rc;
+        if ((rc = upload_to(c, g, vt.pdf.data(), vt.pdf.size() * 4, (const void**)&lt.env_pdf))) return rc;
     }
-    ds.light_pev = sel.p_ev; ds.no_analytic = sel.no_analytic ? 1u : 0u;
+    lt.light_pev = sel.p_ev; lt.no_analytic = sel.no_analytic ? 1u : 0u;
+    c->light_mem = std::move(g); ds = lt;
     return RT_OK;
 }
 
@@ -1783,25 +1744,16 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = join_shadow(c); if (rc) return rc; }     // a shadow pass of an unfinished frame may still read the old scene
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
-    for (void* p : c->scene_allocs) cudaFree(p);
-    c->scene_allocs.clear();
-    free_refit(c);
+    c->scene_mem.clear(); c->tree_mem.clear(); c->stage = {};
+    c->refit_link = nullptr; c->refit_leaves = nullptr; c->refit_arrivals = nullptr; c->refit_n_leaves = 0;
     c->lbvh = rt_ctx::Lbvh();
     c->scene_ready = false;
     clear_light_tables(c);
 
-    auto upload = [&](const void* src, size_t bytes, const void** dst) -> int {
-        void* d = nullptr;
-        size_t alloc = bytes ? bytes : 16;
-        RT_CUDA(c, cudaMalloc(&d, alloc));
-        c->scene_allocs.push_back(d);
-        if (bytes) RT_CUDA(c, cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
-        *dst = d;
-        return RT_OK;
-    };
+    auto upload = [&](const void* src, size_t bytes, const void** dst) { return upload_to(c, c->scene_mem, src, bytes, dst); };
     int rc;
     DevScene& ds = c->scene;
-    if ((rc = upload(s->nodes, s->n_nodes * sizeof(RtLinearBVHNode), (const void**)&ds.nodes_ref))) return rc;
+    if ((rc = upload_to(c, c->tree_mem, s->nodes, s->n_nodes * sizeof(RtLinearBVHNode), (const void**)&ds.nodes_ref))) return rc;
     {
         std::vector<rtbvh::F4> rec;
         rtbvh::build_tri_shade(s->triangles, s->n_triangles, rec);
@@ -1830,7 +1782,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
         std::string err;
         if (!rtbvh::build_layout(s->nodes, s->n_nodes, s->triangles, s->n_triangles, wl, err))
             RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: malformed BVH: %s", err.c_str());
-        if ((rc = upload(wl.nodes.data(), wl.nodes.size() * 16, (const void**)&ds.wnodes))) return rc;
+        if ((rc = upload_to(c, c->tree_mem, wl.nodes.data(), wl.nodes.size() * 16, (const void**)&ds.wnodes))) return rc;
         if ((rc = upload(wl.tris.data(), wl.tris.size() * 16, (const void**)&ds.wtris))) return rc;
         ds.root_ref = wl.root_ref;
         ds.wnodes_f4 = (uint32_t)wl.nodes.size(); ds.wtris_f4 = (uint32_t)wl.tris.size();
@@ -1874,13 +1826,14 @@ static int begin_update(rt_ctx* c, const void* triangles, uint64_t n, const char
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
     rtbvh::RefitMap m;
     rtbvh::build_refit_map(nodes.data(), c->n_nodes, m);
-    auto fail = [&](cudaError_t e) { free_refit(c); RT_FAIL(c, RT_ERR_CUDA, "%s: refit map: %s", what, cudaGetErrorString(e)); };
+    DevAllocs g;
+    uint2* link = nullptr; uint32_t *leaves = nullptr, *arrivals = nullptr;
     cudaError_t e;
-    if ((e = cudaMalloc(&c->refit_link, m.link.size() * 4)) != cudaSuccess || (e = cudaMalloc(&c->refit_leaves, m.leaves.size() * 4)) != cudaSuccess ||
-        (e = cudaMalloc(&c->refit_arrivals, c->n_nodes * 4)) != cudaSuccess ||
-        (e = cudaMemcpy(c->refit_link, m.link.data(), m.link.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess ||
-        (e = cudaMemcpy(c->refit_leaves, m.leaves.data(), m.leaves.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess)
-        return fail(e);
+    if ((e = g.alloc(link, m.link.size() / 2)) || (e = g.alloc(leaves, m.leaves.size())) || (e = g.alloc(arrivals, c->n_nodes)) ||
+        (e = cudaMemcpy(link, m.link.data(), m.link.size() * 4, cudaMemcpyHostToDevice)) ||
+        (e = cudaMemcpy(leaves, m.leaves.data(), m.leaves.size() * 4, cudaMemcpyHostToDevice)))
+        RT_FAIL(c, RT_ERR_CUDA, "%s: refit map: %s", what, cudaGetErrorString(e));
+    c->tree_mem.adopt(std::move(g)); c->refit_link = link; c->refit_leaves = leaves; c->refit_arrivals = arrivals;
     c->refit_n_leaves = (uint32_t)m.leaves.size();
     return RT_OK;
 }
@@ -1915,29 +1868,26 @@ int rt_update_triangles(rt_ctx* c, const RtTriangle* triangles, uint64_t n)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_update_triangles(k, triangles, n));
     { int rc = begin_update(c, triangles, n, "rt_update_triangles"); if (rc) return rc; }
-    if (!c->stage_host)
+    rt_ctx::Staging& sg = c->stage;
+    if (!sg.host)
     {   // two halves of at most 32 MB each: the host copy into one half overlaps the upload and kernel of the other
-        const size_t half = std::min<size_t>((size_t)n * sizeof(RtTriangle), (size_t)32 << 20) / sizeof(RtTriangle) * sizeof(RtTriangle);
+        rt_ctx::Staging s;
+        s.half = std::min<size_t>((size_t)n * sizeof(RtTriangle), (size_t)32 << 20) / sizeof(RtTriangle) * sizeof(RtTriangle);
         cudaError_t e;
-        if ((e = cudaMallocHost(&c->stage_host, 2 * half)) != cudaSuccess || (e = cudaMalloc(&c->stage_dev, 2 * half)) != cudaSuccess ||
-            (e = cudaEventCreateWithFlags(&c->stage_copied[0], cudaEventDisableTiming)) != cudaSuccess ||
-            (e = cudaEventCreateWithFlags(&c->stage_copied[1], cudaEventDisableTiming)) != cudaSuccess)
-        {
-            cudaFreeHost(c->stage_host); cudaFree(c->stage_dev); c->stage_host = nullptr; c->stage_dev = nullptr;
-            for (cudaEvent_t& ev : c->stage_copied) { if (ev) cudaEventDestroy(ev); ev = nullptr; }
+        if ((e = s.mem.alloc(s.host, 2 * s.half, true)) || (e = s.mem.alloc(s.dev, 2 * s.half)) || (e = make_event(s.copied[0])) ||
+            (e = make_event(s.copied[1])))
             RT_FAIL(c, RT_ERR_CUDA, "rt_update_triangles: staging buffers: %s", cudaGetErrorString(e));
-        }
-        c->stage_half = half;
+        sg = std::move(s);
     }
-    const uint64_t per_chunk = c->stage_half / sizeof(RtTriangle);
+    const uint64_t per_chunk = sg.half / sizeof(RtTriangle);
     for (uint64_t first = 0, k = 0; first < n; first += per_chunk, k ^= 1)
     {
         const uint32_t m = (uint32_t)std::min<uint64_t>(per_chunk, n - first);
-        char* h = c->stage_host + k * c->stage_half; char* d = c->stage_dev + k * c->stage_half;
-        RT_CUDA(c, cudaEventSynchronize(c->stage_copied[k]));          // the copy out of this half two chunks ago is done
+        char* h = sg.host + k * sg.half; char* d = sg.dev + k * sg.half;
+        RT_CUDA(c, cudaEventSynchronize(sg.copied[k]));          // the copy out of this half two chunks ago is done
         memcpy(h, triangles + first, (size_t)m * sizeof(RtTriangle));
         RT_CUDA(c, cudaMemcpyAsync(d, h, (size_t)m * sizeof(RtTriangle), cudaMemcpyHostToDevice, c->stream));
-        RT_CUDA(c, cudaEventRecord(c->stage_copied[k], c->stream));
+        RT_CUDA(c, cudaEventRecord(sg.copied[k], c->stream));
         int rc = launch_refit_records(c, d, (uint32_t)first, m); if (rc) return rc;
     }
     return finish_update(c);
@@ -1977,47 +1927,32 @@ int rt_read_bvh(rt_ctx* c, RtLinearBVHNode* nodes, float* records, uint64_t* n_r
 // ---- BVH rebuild: rt_rebuild_bvh (include/rt_b200.h, kernels in rt_lbvh.cuh)
 
 // The first rebuild after an upload: the nodes, records and refit map of a tree of 2n - 1 nodes replace the upload's (which a
-// frame in flight may still read: blocking), and the build temporaries are allocated.  Everything is allocated before anything
-// is freed, so a failure leaves the uploaded tree in place.
+// frame in flight may still read: blocking), and the build temporaries are allocated.  The new tree group replaces the old one
+// only once all of it is allocated, so a failure leaves the uploaded tree in place.
 static int alloc_lbvh(rt_ctx* c)
 {
     const size_t n = c->n_tris, nn = 2 * n - 1, n_rec = n > 1 ? n - 1 : 1;
-    std::vector<void*> got;
+    DevAllocs g;
     cudaError_t e = cudaSuccess;
-    auto get = [&](size_t bytes) -> void* {
-        void* d = nullptr;
-        if (e == cudaSuccess && (e = cudaMalloc(&d, bytes)) == cudaSuccess) got.push_back(d);
-        return d;
-    };
+    auto get = [&](auto*& view, size_t count) { if (e == cudaSuccess) e = g.alloc(view, count); };
     rt_ctx::Lbvh L;
     L.live = true;
-    void* nodes = get(nn * sizeof(RtLinearBVHNode)); void* wnodes = get(n_rec * 64);
-    void* link = get(nn * 8); void* leaves = get(n * 4); void* arrivals = get(nn * 4);
-    L.bounds = (uint32_t*)get(6 * 4); L.top = (uint2*)get(RT_BVH_TOP_RECORDS * 8); L.inner = (uint4*)get(n_rec * 16);
-    for (int k = 0; k < 2; ++k) { L.codes[k] = (uint32_t*)get(n * 4); L.ids[k] = (uint32_t*)get(n * 4); }
+    float4 *nodes = nullptr, *wnodes = nullptr; uint2* link = nullptr; uint32_t *leaves = nullptr, *arrivals = nullptr;
+    get(nodes, nn * 3); get(wnodes, n_rec * 4);                     // 3 float4 per RtLinearBVHNode, 4 per record
+    get(link, nn); get(leaves, n); get(arrivals, nn);
+    get(L.bounds, 6); get(L.top, RT_BVH_TOP_RECORDS); get(L.inner, n_rec);
+    for (int k = 0; k < 2; ++k) { get(L.codes[k], n); get(L.ids[k], n); }
     if (e == cudaSuccess)
     {
         cub::DoubleBuffer<uint32_t> keys(L.codes[0], L.codes[1]), vals(L.ids[0], L.ids[1]);
         e = cub::DeviceRadixSort::SortPairs(nullptr, L.sort_bytes, keys, vals, (int)n, 0, 30, c->stream);
-        L.sort_tmp = get(L.sort_bytes ? L.sort_bytes : 16);
+        get(L.sort_tmp, L.sort_bytes ? L.sort_bytes : 16);
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess)
-    {
-        for (void* p : got) cudaFree(p);
-        RT_FAIL(c, RT_ERR_CUDA, "rt_rebuild_bvh: allocating the rebuilt tree: %s", cudaGetErrorString(e));
-    }
-    DevScene& ds = c->scene;
-    for (const void* old : { (const void*)ds.nodes_ref, (const void*)ds.wnodes })
-    {
-        auto it = std::find(c->scene_allocs.begin(), c->scene_allocs.end(), old);
-        if (it != c->scene_allocs.end()) { cudaFree(*it); c->scene_allocs.erase(it); }
-    }
-    free_refit_map(c);
-    ds.nodes_ref = (const float4*)nodes; ds.wnodes = (const float4*)wnodes;
-    c->refit_link = (uint2*)link; c->refit_leaves = (uint32_t*)leaves; c->refit_arrivals = (uint32_t*)arrivals;
-    for (void* p : got)
-        if (p != link && p != leaves && p != arrivals) c->scene_allocs.push_back(p);
+    if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "rt_rebuild_bvh: allocating the rebuilt tree: %s", cudaGetErrorString(e));
+    c->tree_mem = std::move(g);                        // frees the uploaded nodes, records and refit map
+    c->scene.nodes_ref = nodes; c->scene.wnodes = wnodes;
+    c->refit_link = link; c->refit_leaves = leaves; c->refit_arrivals = arrivals;
     c->lbvh = L;
     ++c->config_gen;                                   // new buffers and sizes: the frame graph is re-captured
     return RT_OK;
@@ -2231,7 +2166,7 @@ int rt_upload_sampler_tables(rt_ctx* c, const int32_t* sobol, const int32_t* scr
     int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_;
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
     const size_t n = (size_t)RT_BN_SOBOL_COUNT + 2 * (size_t)RT_BN_TILE_COUNT;
-    if (!c->d_bn) RT_CUDA(c, cudaMalloc(&c->d_bn, n * sizeof(int)));
+    if (!c->d_bn) RT_CUDA(c, c->ctx_mem.alloc(c->d_bn, n));
     RT_CUDA(c, cudaMemcpy(c->d_bn, sobol, RT_BN_SOBOL_COUNT * sizeof(int), cudaMemcpyHostToDevice));
     RT_CUDA(c, cudaMemcpy(c->d_bn + RT_BN_SOBOL_COUNT, scrambling, RT_BN_TILE_COUNT * sizeof(int), cudaMemcpyHostToDevice));
     RT_CUDA(c, cudaMemcpy(c->d_bn + RT_BN_SOBOL_COUNT + RT_BN_TILE_COUNT, ranking, RT_BN_TILE_COUNT * sizeof(int), cudaMemcpyHostToDevice));
@@ -2243,13 +2178,17 @@ int rt_reset(rt_ctx* c)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_reset(k));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
+    { int rc = frame_buffers_ready(c); if (rc) return rc; }
     RT_CUDA(c, cudaSetDevice(c->device));
     if (!c->denoiser) c->sample_count = 0;                                   // cl_pt_integrator.cpp:499-504
-    {   // the adaptive-sampling setting takes effect here; a changed setting changes the frame's launch arguments
-        if (c->ad_error != c->ad_req_error || c->ad_min != c->ad_req_min) ++c->config_gen;
-        c->ad_error = c->ad_req_error; c->ad_min = c->ad_req_min;
-        int rc = adaptive_on(c) ? reset_adaptive(c) : (free_adaptive(c), RT_OK);
-        if (rc) return rc;
+    // the adaptive-sampling setting takes effect here; a changed setting changes the frame's launch arguments
+    if (c->ad_error != c->ad_req_error || c->ad_min != c->ad_req_min) ++c->config_gen;
+    c->ad_error = c->ad_req_error; c->ad_min = c->ad_req_min;
+    if (adaptive_on(c)) { int rc = reset_adaptive(c); if (rc) return rc; }
+    else if (!c->ad_mem.empty())
+    {   // the per-pixel state exists only while the setting is on
+        cudaStreamSynchronize(c->stream);
+        c->ad_mem.clear(); c->ad = {}; ++c->config_gen;
     }
     TimedLaunch t(c, RT_K_MISC);
     k_reset<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->radiance, c->n_local);
@@ -2262,6 +2201,7 @@ int rt_advance_sample_count(rt_ctx* c)
     int rc = join_shadow(c); if (rc) return rc;     // end of the bounce loop: everything of this frame is ordered on the render stream
     if (adaptive_on(c))
     {
+        if ((rc = frame_buffers_ready(c))) return rc;
         RT_CUDA(c, cudaSetDevice(c->device));
         if ((rc = launch_adaptive_update(c))) return rc;
     }
@@ -2301,11 +2241,11 @@ int rt_set_spatial_denoiser(rt_ctx* c, uint32_t iterations, float sigma_color, f
     c->sd_iters = iterations;
     c->sd_sigma_c = sigma_color; c->sd_sigma_n = sigma_normal; c->sd_sigma_z = sigma_depth;
     if (iterations != 0) return ensure_aov_buffers(c);
-    if (c->sd_col[0] || c->sd_col[1] || c->sd_guide)
+    if (!c->sd_mem.empty())
     {   // the scratch planes exist only while the filter is on
         if (c->copy_stream) RT_CUDA(c, cudaStreamSynchronize(c->copy_stream));
         RT_CUDA(c, cudaStreamSynchronize(c->stream));
-        cudaFree(c->sd_col[0]); cudaFree(c->sd_col[1]); cudaFree(c->sd_guide);
+        c->sd_mem.clear();
         c->sd_col[0] = c->sd_col[1] = c->sd_guide = nullptr;
     }
     return RT_OK;
@@ -2458,7 +2398,7 @@ int rt_denoise(rt_ctx* c)
     if (!c->denoiser) return RT_OK;
     if (c->world != 1) RT_FAIL(c, RT_ERR_UNSUPPORTED, "temporal denoiser is single-GPU only");
     RT_CUDA(c, cudaSetDevice(c->device));
-    int rc = ensure_aov_buffers(c); if (rc) return rc;
+    int rc = frame_buffers_ready(c); if (rc || (rc = ensure_aov_buffers(c))) return rc;
     TimedLaunch t(c, RT_K_MISC);
     k_temporal<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->width, c->height, c->radiance, c->prev_radiance, c->aov_depth, c->prev_depth, c->aov_velocity);
     return post_launch(c, "k_temporal");
@@ -2470,7 +2410,7 @@ int rt_copy_history(rt_ctx* c)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     if (!c->denoiser) return RT_OK;
     RT_CUDA(c, cudaSetDevice(c->device));
-    int rc = ensure_aov_buffers(c); if (rc) return rc;
+    int rc = frame_buffers_ready(c); if (rc || (rc = ensure_aov_buffers(c))) return rc;
     RT_CUDA(c, cudaMemcpyAsync(c->prev_radiance, c->radiance, (size_t)c->n_local * 16, cudaMemcpyDeviceToDevice, c->stream));
     RT_CUDA(c, cudaMemcpyAsync(c->prev_depth, c->aov_depth, (size_t)c->n_local * 4, cudaMemcpyDeviceToDevice, c->stream));
     return RT_OK;
@@ -2514,9 +2454,8 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
 static int ensure_shadow_stream(rt_ctx* c)
 {
     if (c->shadow_stream) return RT_OK;
-    RT_CUDA(c, cudaStreamCreateWithFlags(&c->shadow_stream, cudaStreamNonBlocking));
-    RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shaded, cudaEventDisableTiming));
-    RT_CUDA(c, cudaEventCreateWithFlags(&c->ev_shadowed, cudaEventDisableTiming));
+    RT_CUDA(c, make_event(c->ev_shaded)); RT_CUDA(c, make_event(c->ev_shadowed));
+    RT_CUDA(c, make_stream(c->shadow_stream));          // last: the stream marks the set complete
     return RT_OK;
 }
 
@@ -2566,17 +2505,10 @@ static int integrate_body(rt_ctx* c, uint32_t max_bounces)
     return rt_advance_sample_count(c);      // joins the shadow stream: the frame is complete in render-stream order
 }
 
-static void drop_graph(rt_ctx* c)
-{
-    if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
-    if (c->graph) cudaGraphDestroy(c->graph);
-    c->graph_exec = nullptr; c->graph = nullptr; c->graph_set_frame_node = nullptr; c->graph_gen = 0;
-}
-
 // Captures one frame (both streams) into a graph.  Nothing executes during capture; host-side frame state is restored.
 static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
 {
-    drop_graph(c);
+    c->graph_exec.reset(); c->graph.reset(); c->graph_set_frame_node = nullptr; c->graph_gen = 0;
     int rc = join_shadow(c); if (rc) return rc;
     if (c->overlap == 1 && (rc = ensure_shadow_stream(c))) return rc;      // created outside the capture
     const uint32_t saved_samples = c->sample_count, saved_bounce = c->cur_bounce;
@@ -2584,13 +2516,14 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
     const bool saved_started = c->frame_started, saved_aov_ready = c->aov_ready, saved_ad_fresh = c->ad_fresh;
     RT_CUDA(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
     rc = integrate_body(c, max_bounces);
-    cudaGraph_t graph = nullptr;
-    cudaError_t e = cudaStreamEndCapture(c->stream, &graph);
+    cudaGraph_t captured = nullptr;
+    cudaError_t e = cudaStreamEndCapture(c->stream, &captured);
+    Owned<cudaGraph_t> graph(captured);
     c->graph_launches = c->launches - saved_launches;
     c->sample_count = saved_samples; c->cur_bounce = saved_bounce; c->launches = saved_launches; c->frame_started = saved_started;
     c->aov_ready = saved_aov_ready; c->ad_fresh = saved_ad_fresh;
     c->shadow_pending = false; c->shadow_deferred = false;
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+    if (rc) return rc;
     if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
     size_t n_nodes = 0;
     RT_CUDA(c, cudaGraphGetNodes(graph, nullptr, &n_nodes));
@@ -2608,10 +2541,11 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
             c->graph_set_frame_node = nd; c->graph_set_frame_func = kp.func;
         }
     }
-    if (!c->graph_set_frame_node) { cudaGraphDestroy(graph); RT_FAIL(c, RT_ERR_CUDA, "frame graph has no k_set_frame node"); }
-    e = cudaGraphInstantiate(&c->graph_exec, graph, 0);
-    if (e != cudaSuccess) { cudaGraphDestroy(graph); c->graph_exec = nullptr; RT_FAIL(c, RT_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e)); }
-    c->graph = graph;
+    if (!c->graph_set_frame_node) RT_FAIL(c, RT_ERR_CUDA, "frame graph has no k_set_frame node");
+    cudaGraphExec_t exec = nullptr;
+    e = cudaGraphInstantiate(&exec, graph, 0);
+    if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(e));
+    c->graph_exec.reset(exec); c->graph = std::move(graph);
     c->graph_gen = c->config_gen; c->graph_max_bounces = max_bounces;
     return RT_OK;
 }
@@ -2789,7 +2723,7 @@ int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
     int rc = require_ready(c); if (rc) return rc;
     if ((rc = join_shadow(c))) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
-    if (!c->counters_sum) RT_CUDA(c, cudaMalloc(&c->counters_sum, sizeof(DevCounters)));
+    if (!c->counters_sum) RT_CUDA(c, c->ctx_mem.alloc(c->counters_sum, 1));
     RT_CUDA(c, cudaMemsetAsync(c->counters_sum, 0, sizeof(DevCounters), c->stream));
     c->stats_summed = false;
     bool pushed = true;
@@ -2845,7 +2779,7 @@ static int launch_resolve(rt_ctx* c, float4* out)
             RT_FAIL(c, RT_ERR_NOT_READY, "the spatial denoiser needs the AOVs of a frame rendered with it on: render a frame first");
         const size_t n = std::max(c->n_local, 1u);
         for (float4** p : { &c->sd_col[0], &c->sd_col[1], &c->sd_guide })
-            if (!*p) RT_CUDA(c, cudaMalloc(p, n * 16));
+            if (!*p) RT_CUDA(c, c->sd_mem.alloc(*p, n));
     }
     {
         TimedLaunch t(c, RT_K_RESOLVE);
@@ -2878,12 +2812,8 @@ static int launch_resolve(rt_ctx* c, float4* out)
 static int ensure_copy_stream(rt_ctx* c)
 {
     if (c->copy_stream) return RT_OK;
-    RT_CUDA(c, cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i)
-    {
-        RT_CUDA(c, cudaEventCreateWithFlags(&c->resolve_done[i], cudaEventDisableTiming));
-        RT_CUDA(c, cudaEventCreateWithFlags(&c->copy_done[i], cudaEventDisableTiming));
-    }
+    for (int i = 0; i < 2; ++i) { RT_CUDA(c, make_event(c->resolve_done[i])); RT_CUDA(c, make_event(c->copy_done[i])); }
+    RT_CUDA(c, make_stream(c->copy_stream));            // last: the stream marks the set complete
     return RT_OK;
 }
 
@@ -2891,6 +2821,7 @@ static int ensure_copy_stream(rt_ctx* c)
 static int resolve_enqueue(rt_ctx* c, float* dst)
 {
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
+    { int rc = frame_buffers_ready(c); if (rc) return rc; }
     RT_CUDA(c, cudaSetDevice(c->device));
     if (c->copy_pending[0]) RT_CUDA(c, cudaStreamWaitEvent(c->stream, c->copy_done[0], 0));   // rt_resolve_async may still copy out of c->resolved
     { int rc = launch_resolve(c, c->resolved); if (rc) return rc; }
@@ -2948,9 +2879,10 @@ int rt_resolve_async(rt_ctx* c, float* dst)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_resolve_async(k, dst));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     if (!dst) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_resolve_async: null destination");
+    { int rc = frame_buffers_ready(c); if (rc) return rc; }
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = ensure_copy_stream(c); if (rc) return rc; }
-    if (!c->resolved2) RT_CUDA(c, cudaMalloc(&c->resolved2, (size_t)(c->n_local ? c->n_local : 1) * 16));
+    if (!c->resolved2) RT_CUDA(c, c->frame_mem.alloc(c->resolved2, c->n_local ? c->n_local : 1));
     const int k = (int)(c->async_index++ & 1u);
     float4* buf = k ? c->resolved2 : c->resolved;
     if (c->copy_pending[k]) RT_CUDA(c, cudaStreamWaitEvent(c->stream, c->copy_done[k], 0));   // buffer k is being re-used
@@ -2985,7 +2917,7 @@ static int resolve_gathered_impl(rt_ctx* c, const void* slabs, uint64_t stride_b
         k = (int)(c->async_index++ & 1u);
         if (c->copy_pending[k]) RT_CUDA(c, cudaStreamWaitEvent(c->stream, c->copy_done[k], 0));
     }
-    if (!c->resolved_full[k]) RT_CUDA(c, cudaMalloc(&c->resolved_full[k], n * 16));
+    if (!c->resolved_full[k]) RT_CUDA(c, c->ctx_mem.alloc(c->resolved_full[k], n));
     {
         TimedLaunch t(c, RT_K_RESOLVE);
         k_resolve_gathered<<<grid_for((uint32_t)n), 256, 0, c->stream>>>((const float4*)slabs, (size_t)(stride_bytes / 16), c->resolved_full[k],
@@ -3026,20 +2958,12 @@ int rt_sync(rt_ctx* c)
     return RT_OK;
 }
 
-static int ensure_scratch(rt_ctx* c, size_t bytes)
-{
-    if (c->scratch_bytes >= bytes) return RT_OK;
-    cudaFree(c->scratch); c->scratch = nullptr; c->scratch_bytes = 0;
-    RT_CUDA(c, cudaMalloc(&c->scratch, bytes));
-    c->scratch_bytes = bytes;
-    return RT_OK;
-}
-
 int rt_read_hits(rt_ctx* c, uint32_t bounce, RtHit* hits, uint32_t* pixels, uint32_t* n_out)
 {
     RT_CHECK_CTX(c); RT_NOT_ON_GROUP(c, "rt_read_hits");
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     if (bounce > RT_MAX_BOUNCES || !n_out) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_hits: bad arguments");
+    { int rc = frame_buffers_ready(c); if (rc) return rc; }
     RT_CUDA(c, cudaSetDevice(c->device));
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
     uint32_t n = 0;
@@ -3060,10 +2984,11 @@ int rt_read_rays(rt_ctx* c, uint32_t bounce, RtRay* rays, uint32_t* pixels, uint
     RT_CHECK_CTX(c); RT_NOT_ON_GROUP(c, "rt_read_rays");
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     if (bounce > RT_MAX_BOUNCES || !n_out || !rays || !pixels) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_rays: bad arguments");
+    int rc = frame_buffers_ready(c); if (rc) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
-    int rc = ensure_scratch(c, (size_t)c->n_local * (sizeof(RtRay) + 4) + 64); if (rc) return rc;
+    if ((rc = ensure_scratch(c, (size_t)c->n_local * (sizeof(RtRay) + 4) + 64))) return rc;
     RtRay* drays = (RtRay*)c->scratch;
-    uint32_t* dpix = (uint32_t*)((char*)c->scratch + (size_t)c->n_local * sizeof(RtRay));
+    uint32_t* dpix = (uint32_t*)(c->scratch + (size_t)c->n_local * sizeof(RtRay));
     k_unpack_rays<<<grid_for(c->n_local), 256, 0, c->stream>>>(c->q.A[bounce & 1], c->q.B[bounce & 1], in_count_ptr(c->counters, bounce), c->width, drays, dpix);
     ++c->launches;
     if ((rc = post_launch(c, "k_unpack_rays"))) return rc;
@@ -3084,6 +3009,7 @@ int rt_read_radiance(rt_ctx* c, float* dst)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_read_radiance(k, dst));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     if (!dst) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_radiance: null destination");
+    { int rc = frame_buffers_ready(c); if (rc) return rc; }
     RT_CUDA(c, cudaSetDevice(c->device));
     if (c->local_rows)
         RT_CUDA(c, cudaMemcpy2DAsync(dst + (size_t)c->rank * c->width * 4, (size_t)c->world * c->width * 16, c->radiance,
@@ -3172,7 +3098,7 @@ int rt_kernel_times(rt_ctx* c, float* ms, uint32_t* launches)
         float m = 0.0f;
         RT_CUDA(c, cudaEventElapsedTime(&m, t.a, t.b));
         c->ms[t.cls] += m; c->nlaunch[t.cls] += 1;
-        c->event_pool.push_back(t.a); c->event_pool.push_back(t.b);
+        c->event_pool.push_back(std::move(t.a)); c->event_pool.push_back(std::move(t.b));
     }
     c->timed.clear();
     for (int k = 0; k < RT_K_CLASS_COUNT; ++k)
@@ -3268,18 +3194,18 @@ int rt_gather_radiance(rt_ctx* c)
     RT_CUDA(c, cudaSetDevice(k0->device));
     if (!c->gather_buf)
     {
-        RT_CUDA(c, cudaMalloc(&c->gather_buf, stride * c->world * 16));
+        RT_CUDA(c, c->gather_mem.alloc(c->gather_buf, stride * c->world));
         RT_CUDA(c, cudaMemsetAsync(c->gather_buf, 0, stride * c->world * 16, k0->stream));
         RT_CUDA(c, cudaStreamSynchronize(k0->stream));
         c->gather_stride_f4 = stride;
-        c->gather_events.resize(c->world, nullptr);
+        c->gather_events.resize(c->world);
     }
     for (uint32_t i = 0; i < c->world; ++i)
     {
         rt_ctx* k = c->children[i];
         { int rc = join_shadow(k); if (rc) { c->error = k->error; return rc; } }
         RT_CUDA(c, cudaSetDevice(k->device));
-        if (!c->gather_events[i]) RT_CUDA(c, cudaEventCreateWithFlags(&c->gather_events[i], cudaEventDisableTiming));
+        if (!c->gather_events[i]) RT_CUDA(c, make_event(c->gather_events[i]));
         if (k->n_local)
             RT_CUDA(c, cudaMemcpyPeerAsync(c->gather_buf + (size_t)i * stride, k0->device, k->radiance, k->device, (size_t)k->n_local * 16, k->stream));
         RT_CUDA(c, cudaEventRecord(c->gather_events[i], k->stream));
@@ -3329,10 +3255,10 @@ int rt_gather_buffer(rt_ctx* c, void** dev_ptr, uint64_t* stride_bytes, uint64_t
     const size_t stride = rows_max * c->width * 16;
     const size_t total = stride * c->world + 256;
     RT_CUDA(c, cudaSetDevice(c->device));
-    if (c->own_gather && c->own_gather_stride != stride) { cudaFree(c->own_gather); c->own_gather = nullptr; }
+    if (c->own_gather && c->own_gather_stride != stride) { c->gather_mem.clear(); c->own_gather = nullptr; }
     if (!c->own_gather)
     {
-        RT_CUDA(c, cudaMalloc(&c->own_gather, total));
+        RT_CUDA(c, c->gather_mem.alloc(c->own_gather, total));
         RT_CUDA(c, cudaMemset(c->own_gather, 0, total));
         c->own_gather_stride = stride;
     }
@@ -3360,7 +3286,7 @@ int rt_ipc_open(rt_ctx* c, const void* handle64, void** dev_ptr)
     cudaIpcMemHandle_t h; memcpy(&h, handle64, 64);
     void* p = nullptr;
     RT_CUDA(c, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-    c->ipc_opened.push_back(p);
+    c->ipc_opened.emplace_back(p);
     *dev_ptr = p;
     return RT_OK;
 }
@@ -3400,10 +3326,11 @@ int rt_math_eval(int device, int fn, const float* a, const float* b, float* out,
     if (!a || !b || !out || fn < 0 || fn > 10) return RT_ERR_INVALID_ARGUMENT;
     if (n == 0) return RT_OK;
     if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); g_create_error = "rt_math_eval: no such CUDA device"; return RT_ERR_NO_DEVICE; }
+    DevAllocs g;
     float *da = nullptr, *db = nullptr, *dout = nullptr;
-    cudaError_t e = cudaMalloc(&da, n * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&db, n * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&dout, n * 4);
+    cudaError_t e = g.alloc(da, n);
+    if (e == cudaSuccess) e = g.alloc(db, n);
+    if (e == cudaSuccess) e = g.alloc(dout, n);
     if (e == cudaSuccess) e = cudaMemcpy(da, a, n * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(db, b, n * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
@@ -3412,7 +3339,6 @@ int rt_math_eval(int device, int fn, const float* a, const float* b, float* out,
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaMemcpy(out, dout, n * 4, cudaMemcpyDeviceToHost);
-    cudaFree(da); cudaFree(db); cudaFree(dout);
     if (e != cudaSuccess) { g_create_error = std::string("rt_math_eval: ") + cudaGetErrorString(e); return RT_ERR_CUDA; }
     return RT_OK;
 }
