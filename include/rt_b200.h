@@ -99,9 +99,14 @@ typedef enum RtOption {
     RT_OPT_EMITTER_SAMPLING = 30, /* 0 (default): emissive triangles add light only when a BSDF-sampled ray hits them; 1: next-event
                                    estimation on the emissive triangles too, combined with BSDF sampling by MIS (the rule is stated
                                    in the emitter-sampling block below; the image converges to the same expectation) */
-    RT_OPT_ENV_SAMPLING = 31    /* 0 (default): the environment map adds light only when a BSDF-sampled ray misses; 1: next-event
+    RT_OPT_ENV_SAMPLING = 31,   /* 0 (default): the environment map adds light only when a BSDF-sampled ray misses; 1: next-event
                                    estimation on the environment map too, combined with BSDF sampling by MIS (the environment-sampling
                                    block below; the image converges to the same expectation) */
+    RT_OPT_OCTANT_BVH = 32      /* 1 (default): a scene staged whole into shared memory (RT_OPT_SMEM_BVH) whose interior records fit
+                                   eight more times within the same 40 KB is traversed through per-direction-octant copies of
+                                   the records that every CTA builds after staging: the box test needs no pairwise min/max and
+                                   no near/far selection (the per-phase kernels; the one-kernel frame keeps the canonical records).
+                                   0: the canonical records only.  Results are bit-identical */
 } RtOption;
 
 #define RT_MAX_BOUNCES 255u     /* bounce index range supported per frame (reference GUI: 0..5) */
@@ -476,6 +481,11 @@ int rt_read_sample_count(rt_ctx* ctx, uint32_t* out);
 int rt_read_aovs(rt_ctx* ctx, float* albedo_rgba, float* depth, float* normal_rgba, float* velocity_xy);
 /* Accumulated milliseconds and launch counts per RtKernelClass since the last call (RT_OPT_KERNEL_TIMING). */
 int rt_kernel_times(rt_ctx* ctx, float* ms_per_class, uint32_t* launches_per_class);
+/* How the traversal kernels of the next frame stage the BVH into shared memory, for the current scene and options: *mode =
+ * 0 nothing, 1 the whole structure, 2 the first RT_OPT_TOP_SMEM records, 3 the whole structure plus the octant-ordered record
+ * tables (RT_OPT_OCTANT_BVH); *bytes = dynamic shared memory per CTA.  Either pointer may be NULL.  (The one-kernel frame
+ * of RT_OPT_FRAME_KERNEL runs mode 1 where this says 3; RT_OPT_COUNT_TRAVERSAL runs unstaged kernels whatever this says.) */
+int rt_bvh_staging(rt_ctx* ctx, uint32_t* mode, uint64_t* bytes);
 /* Number of kernels launched by this context since creation. */
 int rt_launch_count(rt_ctx* ctx, uint64_t* out);
 

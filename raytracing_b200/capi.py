@@ -21,6 +21,7 @@ OPT_COUNT_TRAVERSAL, OPT_KERNEL_TIMING, OPT_TRAVERSAL = 16, 17, 18
 OPT_AOV_ALWAYS, OPT_SMEM_BVH, OPT_OVERLAP, OPT_GRAPH, OPT_PDL, OPT_FRAME_KERNEL, OPT_PRESENT, OPT_FRAME_THREADS, OPT_TOP_SMEM = 21, 22, 23, 24, 25, 26, 27, 28, 29
 OPT_EMITTER_SAMPLING = 30       # 1: next-event estimation on the emissive triangles, MIS with BSDF sampling (include/rt_b200.h)
 OPT_ENV_SAMPLING = 31           # 1: next-event estimation on the environment map, MIS with BSDF sampling (include/rt_b200.h)
+OPT_OCTANT_BVH = 32             # 1 (default): octant-ordered record copies for scenes staged whole in shared memory (include/rt_b200.h)
 KERNEL_CLASSES = ["raygen", "intersect", "miss", "hit", "intersect_shadow", "accumulate", "extend_shade",
                   "shadow_accumulate", "resolve", "aov", "misc", "trace_closest", "shade_queues", "trace_both"]
 
@@ -37,7 +38,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
            "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh",
-           "rt_rebuild_bvh"]
+           "rt_rebuild_bvh", "rt_bvh_staging"]
 
 
 class RtSceneDesc(C.Structure):
@@ -102,6 +103,8 @@ def load_library():
     L.rt_read_aovs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.rt_kernel_times.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.rt_launch_count.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    if hasattr(L, "rt_bvh_staging"):        # absent from a variant library built from an earlier commit (RT_B200_LIB)
+        L.rt_bvh_staging.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     L.rt_local_pixel_count.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rt_radiance_device_ptr.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
     L.rt_stream_handle.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
@@ -413,6 +416,12 @@ class Context:
         nl = np.zeros(len(KERNEL_CLASSES), dtype="<u4")
         self._ck(self.lib.rt_kernel_times(self.h, ms.ctypes.data, nl.ctypes.data))
         return {k: (float(ms[i]), int(nl[i])) for i, k in enumerate(KERNEL_CLASSES)}
+
+    def bvh_staging(self):
+        """-> (mode, bytes): how the next frame's traversal kernels stage the BVH in shared memory (rt_bvh_staging)."""
+        m, b = C.c_uint32(), C.c_uint64()
+        self._ck(self.lib.rt_bvh_staging(self.h, C.byref(m), C.byref(b)))
+        return m.value, b.value
 
     def launch_count(self):
         n = C.c_uint64()

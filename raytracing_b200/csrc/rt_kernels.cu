@@ -1056,7 +1056,7 @@ struct rt_ctx
     std::string error;
 
     // options
-    int white_furnace = 0, sampler = 0, aov = 0, denoiser = 0, count_traversal = 0, kernel_timing = 0, traversal = 1, smem_bvh = 1;
+    int white_furnace = 0, sampler = 0, aov = 0, denoiser = 0, count_traversal = 0, kernel_timing = 0, traversal = 1, smem_bvh = 1, octant_bvh = 1;
     uint32_t top_smem_records = 0;                 // RT_OPT_TOP_SMEM
 
     // per-pixel buffers
@@ -1435,16 +1435,23 @@ cudaError_t launch_chain(rt_ctx* c, void (*kernel)(KArgs...), int grid, size_t s
 
 // How a traversal kernel stages the BVH (TMA bulk copies into dynamic shared memory), decided per launch:
 //   mode 1  the whole structure (interior records + triangle records) when it fits 40 KB (5 resident CTAs x 40 KB stay under
-//           the 227 KB of an SM): CornellBox;
+//           the 227 KB of an SM);
+//   mode 3  mode 1 plus the eight octant-ordered copies of the interior records that every CTA builds from the staged ones
+//           (rt_octant.h) and a flag word, when all of it fits the same 40 KB (RT_OPT_OCTANT_BVH, default on): CornellBox,
+//           2.6 KB + 8.7 KB;
 //   mode 2  only the top of the tree — the first top_k interior records in breadth-first order (RT_OPT_TOP_SMEM records,
 //           default 0 = off, DESIGN.md section 4 says why) — when the structure does not fit;
 //   mode 0  nothing staged: literal traversal (RT_OPT_TRAVERSAL 0), RT_OPT_SMEM_BVH off.
 struct Stage { int mode; size_t bytes; uint32_t top_k; };
-Stage bvh_stage(const rt_ctx* c)
+// octant = false: the one-kernel frame (k_frame, k_frame_regen) stays on mode 1 — at its 64 registers the second traversal loop
+// that mode 3 needs for the guarded rays spills inside the frame loop (measured: CornellBox on rank 0 of 4, 0.761 -> 0.811 ms).
+Stage bvh_stage(const rt_ctx* c, bool octant = true)
 {
     Stage st = { 0, 0, 0 };
     if (!c->smem_bvh || c->traversal != 1) return st;
     size_t bytes = ((size_t)c->scene.wnodes_f4 + c->scene.wtris_f4) * 16;
+    const size_t oct_bytes = bytes + 8 * (size_t)c->scene.wnodes_f4 * 16 + 16;
+    if (octant && c->octant_bvh && oct_bytes <= 40 * 1024) { st.mode = 3; st.bytes = oct_bytes; return st; }
     if (bytes <= 40 * 1024) { st.mode = 1; st.bytes = bytes; return st; }
     uint32_t k = c->top_smem_records < c->scene.top_n ? c->top_smem_records : c->scene.top_n;
     if (k >= 8) { st.mode = 2; st.bytes = (size_t)k * 64; st.top_k = k; }
@@ -1455,13 +1462,17 @@ Stage bvh_stage(const rt_ctx* c)
 // dynamic shared-memory bytes) once, for the launch's staging mode, and returns its result.  At most 40 KB are staged, under the
 // 48 KB that every kernel may take without raising its shared-memory limit.
 template <class F>
-auto launch_staged(const rt_ctx* c, F&& launch)
+auto launch_staged(const rt_ctx* c, F&& launch, bool octant = true)
 {
-    const Stage sg = bvh_stage(c);
+    const Stage sg = bvh_stage(c, octant);
     DevScene sc = c->scene;
     sc.top_k = sg.top_k;
     if (sg.mode == 1) return launch(std::integral_constant<int, 1>(), sc, sg.bytes);
     if (sg.mode == 2) return launch(std::integral_constant<int, 2>(), sc, sg.bytes);
+    if constexpr (std::is_void_v<decltype(launch(std::integral_constant<int, 1>(), sc, sg.bytes))>)
+    {   // the per-phase kernels (their launchers return nothing); the frame kernels never ask for mode 3
+        if (sg.mode == 3) return launch(std::integral_constant<int, 3>(), sc, sg.bytes);
+    }
     return launch(std::integral_constant<int, 0>(), sc, sg.bytes);
 }
 
@@ -2138,6 +2149,7 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
         if (value > 2) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "frame-kernel mode must be 0 (per-phase kernels), 1 (one kernel per frame) or 2 (by partition size)");
         c->frame_kernel = (int)value; return RT_OK;
     case RT_OPT_SMEM_BVH: c->smem_bvh = value != 0; return RT_OK;
+    case RT_OPT_OCTANT_BVH: c->octant_bvh = value != 0; return RT_OK;
     case RT_OPT_TOP_SMEM:
         if (value > 640u) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "at most 640 top-of-tree records (40 KB per CTA) can be staged");
         c->top_smem_records = value; return RT_OK;
@@ -2569,7 +2581,8 @@ static bool frame_kernel_selected(const rt_ctx* c)
 static int frame_kernel_threads(const rt_ctx* c)
 {
     if (c->frame_threads) return c->frame_threads;
-    if (bvh_stage(c).mode == 1) return 1024;
+    const int mode = bvh_stage(c).mode;
+    if (mode == 1 || mode == 3) return 1024;      // the whole BVH in shared memory
     return (size_t)c->n_local > (size_t)c->num_sms * 4096u ? 1024 : 256;
 }
 
@@ -2626,7 +2639,7 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
         TimedLaunch t(c, RT_K_MISC);
         k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
         return RT_OK;
-    });
+    }, false);
     if (rc || (rc = post_launch(c, "k_frame"))) return rc;
     note_frame_aovs(c);
     if (adaptive_on(c) && (rc = launch_adaptive_update(c))) return rc;
@@ -2651,7 +2664,7 @@ static int integrate_regen_kernel(rt_ctx* c, uint32_t max_bounces, uint32_t n_sa
         k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters_sum, c->radiance, aov_params(c), max_bounces, n_samples,
                                             slots_per_cta, dyn);
         return RT_OK;
-    });
+    }, false);
     if (rc || (rc = post_launch(c, "k_frame_regen"))) return rc;
     note_frame_aovs(c);
     c->frame_started = true; c->cur_bounce = max_bounces;
@@ -3107,6 +3120,15 @@ int rt_kernel_times(rt_ctx* c, float* ms, uint32_t* launches)
         if (launches) launches[k] = c->nlaunch[k];
         c->ms[k] = 0.0f; c->nlaunch[k] = 0;
     }
+    return RT_OK;
+}
+
+int rt_bvh_staging(rt_ctx* c, uint32_t* mode, uint64_t* bytes)
+{
+    RT_CHECK_CTX(c); if (!mode && !bytes) return RT_ERR_INVALID_ARGUMENT;
+    const Stage sg = bvh_stage(c->children.empty() ? c : c->children[0]);
+    if (mode) *mode = (uint32_t)sg.mode;
+    if (bytes) *bytes = sg.bytes;
     return RT_OK;
 }
 

@@ -5,6 +5,8 @@
  */
 #pragma once
 
+#include "rt_octant.h"
+
 // ------------------------------------------------------------------------------------ TMA staging of a small BVH
 // When the whole traversal structure (interior records + triangle records) is small enough, every CTA of a
 // traversal kernel copies it ONCE into shared memory with two TMA bulk copies (cp.async.bulk, completion signalled
@@ -17,13 +19,16 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 
 // SMEM 1 stages the whole structure (records, then triangles: two bulk copies), SMEM 2 the first sc.top_k interior records —
 // breadth-first, the top of the tree (rt_bvh_layout.h) — with one bulk copy, deeper records and all triangles staying behind
-// L1/L2 (RT_OPT_TOP_SMEM); SMEM 0 stages nothing.
+// L1/L2 (RT_OPT_TOP_SMEM); SMEM 0 stages nothing.  SMEM 3 stages what SMEM 1 does and then builds, behind the triangles, the
+// eight octant-ordered copies of the interior records (rt_octant.h; table s at dst + wnodes_f4 + wtris_f4 + s * wnodes_f4) and
+// one flag word behind them: 1 when every record passed rt_oct_record_ok and the tables exist, 0 when the CTA must not use them.
 template <int SMEM>
 __device__ __forceinline__ void stage_bvh(float4* dst, const DevScene& sc, uint64_t* mbar)
 {
     if (SMEM == 0) return;
     const uint32_t bar = smem_u32(mbar);
-    const uint32_t nodes_bytes = (SMEM == 1 ? sc.wnodes_f4 : sc.top_k * 4u) * 16u, tris_bytes = SMEM == 1 ? sc.wtris_f4 * 16u : 0u;
+    constexpr bool WHOLE = SMEM == 1 || SMEM == 3;
+    const uint32_t nodes_bytes = (WHOLE ? sc.wnodes_f4 : sc.top_k * 4u) * 16u, tris_bytes = WHOLE ? sc.wtris_f4 * 16u : 0u;
     if (threadIdx.x == 0)
     {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1));
@@ -36,7 +41,7 @@ __device__ __forceinline__ void stage_bvh(float4* dst, const DevScene& sc, uint6
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(nodes_bytes + tris_bytes) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(smem_u32(dst)), "l"(sc.wnodes), "r"(nodes_bytes), "r"(bar) : "memory");
-        if (SMEM == 1)
+        if (WHOLE)
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                          ::"r"(smem_u32(dst + sc.wnodes_f4)), "l"(sc.wtris), "r"(tris_bytes), "r"(bar) : "memory");
     }
@@ -44,6 +49,19 @@ __device__ __forceinline__ void stage_bvh(float4* dst, const DevScene& sc, uint6
     while (!done)
         asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
                      : "=r"(done) : "r"(bar), "r"(0) : "memory");
+    if (SMEM == 3)
+    {   // every thread has seen the copies complete; each reorders a few of the records it can now read
+        const uint32_t n = sc.root_ref < 0 ? 0u : sc.wnodes_f4 / 4u;      // a root-leaf tree has no interior record to visit
+        float4* oct = dst + sc.wnodes_f4 + sc.wtris_f4;
+        bool ok = true;
+        for (uint32_t r = threadIdx.x; r < n; r += blockDim.x) ok = ok && rt_oct_record_ok((const float*)(dst + r * 4u));
+        ok = __syncthreads_and(ok) != 0;
+        if (ok)
+            for (uint32_t i = threadIdx.x; i < 8u * n; i += blockDim.x)
+                rt_oct_order((const float*)(dst + (i % n) * 4u), i / n, (float*)(oct + i * 4u));
+        if (threadIdx.x == 0) *(uint32_t*)(oct + 8u * sc.wnodes_f4) = ok ? 1u : 0u;
+        __syncthreads();
+    }
 }
 
 // Programmatic dependent launch (RT_OPT_PDL): a kernel launched with the programmatic-stream-serialization attribute may
@@ -136,15 +154,25 @@ __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d
 // still match) take the literal path.
 // PIN: the whole-frame kernel shares its register budget with the shading code and ptxas then re-derives the sign bits on
 // every step and recomputes the determinant after its branch; an empty asm makes both values opaque (kept in registers).
+// SMEM 3: `wnodes` and `wtris` are those of SMEM 1 and the octant tables follow the triangles (stage_bvh).  The interior step
+// reads the record of the ray's octant and runs the ordered slab test, which takes the same decisions as the pairwise one for a
+// ray that passes rt_oct_ray_ok on records that passed rt_oct_record_ok (rt_octant.h has the argument).  Any other ray, and
+// every ray of a CTA whose records failed, is traced by the SMEM 1 traversal on the canonical staged records (a loop of its
+// own: a branch inside the ordered loop was measured and cost half the gain):
+// exactly what RT_OPT_OCTANT_BVH 0 computes, also where that differs from the literal traversal (a NaN t_max from a triangle
+// with an infinite vertex ends the staged traversal and not the literal one).
 template <bool ANY, bool COUNT, int SMEM, bool PIN = false>
 __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4* wnodes, const float4* wtris, f3 o, f3 d, float t_min, float t_max,
                                                float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
 {
+    constexpr bool OCT = SMEM == 3, PACKED = SMEM == 1 || OCT;
     float fin = ((o.x + o.y) + o.z) + ((d.x + d.y) + d.z);
     if (!(fabsf(fin) <= 3.0e38f) || COUNT)
         return trace_literal<ANY, COUNT>(sc, o, d, t_min, t_max, bu, bv, bt, nv, nt);
 
     f3 inv = splat(1.0f) / d;
+    if (OCT && !(rt_oct_ray_ok(inv.x, inv.y, inv.z) && *(const uint32_t*)(wtris + sc.wtris_f4 + 8u * sc.wnodes_f4) != 0u))
+        return trace_fast<ANY, COUNT, OCT ? 1 : SMEM, PIN>(sc, wnodes, wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt);
     const bool sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
     uint32_t sign_bits = (sx ? 1u : 0u) | (sy ? 2u : 0u) | (sz ? 4u : 0u);
     if (PIN) asm volatile("" : "+r"(sign_bits));
@@ -155,9 +183,13 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
     // (measured, same results): with the records in shared memory the kernel is purely issue-bound and the packed
     // 64-bit stack entry + the sign-bit axis test win (CornellBox frame -2.7 %); with the records behind L1/L2 the two
     // 32-bit arrays (a discarded pop costs one load) and predicate selects are faster (ShaderBalls +1 %, Dragon +3.5 %).
-    int2 stack[SMEM == 1 ? 64 : 1];
-    int stack_ref[SMEM == 1 ? 1 : 64];
-    float stack_t[SMEM == 1 ? 1 : 64];
+    int2 stack[PACKED ? 64 : 1];
+    int stack_ref[PACKED ? 1 : 64];
+    float stack_t[PACKED ? 1 : 64];
+    // the records of this ray's octant, as an offset from the canonical ones; opaque, so that it stays in a register instead of
+    // being re-derived from the sign bits and the two sizes on every step
+    uint32_t oct_at = OCT ? sc.wnodes_f4 + sc.wtris_f4 + sign_bits * sc.wnodes_f4 : 0u;
+    if (OCT) asm volatile("" : "+r"(oct_at));
     if (cur < 0)
     {   // single-leaf tree: the root box is tested like any visited node
         float4 r0 = __ldg(sc.nodes_ref), r1 = __ldg(sc.nodes_ref + 1);
@@ -179,36 +211,51 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
         while (cur >= 0)
         {
             // SMEM == 2: `wnodes` is the staged top of the tree (records [0, sc.top_k)), deeper records come from sc.wnodes
-            const float4* np = (SMEM == 2 && (uint32_t)cur >= sc.top_k) ? sc.wnodes + (size_t)cur * 4 : wnodes + (size_t)cur * 4;
+            const float4* np = OCT ? wnodes + (oct_at + (uint32_t)cur * 4u)
+                             : (SMEM == 2 && (uint32_t)cur >= sc.top_k) ? sc.wnodes + (size_t)cur * 4 : wnodes + (size_t)cur * 4;
             float4 a = ld_bvh<SMEM>(np), b = ld_bvh<SMEM>(np + 1), c = ld_bvh<SMEM>(np + 2), m = ld_bvh<SMEM>(np + 3);
-            // child 0 box: min (a.x,a.y,a.z) max (a.w,b.x,b.y); child 1 box: min (b.z,b.w,c.x) max (c.y,c.z,c.w)
+            int near_ref, far_ref;
+            bool near_hit, far_hit;
+            float far_lo;
+            if (OCT)
+            {   // near child: entry (a.x,a.y,a.z) exit (a.w,b.x,b.y); far child: entry (b.z,b.w,c.x) exit (c.y,c.z,c.w)
+                float lo_n, hi_n, hi_f;
+                rt_slab_ordered(a.x, a.y, a.z, a.w, b.x, b.y, o.x, o.y, o.z, inv.x, inv.y, inv.z, t_min, lo_n, hi_n);
+                rt_slab_ordered(b.z, b.w, c.x, c.y, c.z, c.w, o.x, o.y, o.z, inv.x, inv.y, inv.z, t_min, far_lo, hi_f);
+                near_hit = fminf(hi_n, t_max) >= lo_n; far_hit = fminf(hi_f, t_max) >= far_lo;
+                near_ref = __float_as_int(m.x); far_ref = __float_as_int(m.y);
+            }
+            else
+            {
+                // child 0 box: min (a.x,a.y,a.z) max (a.w,b.x,b.y); child 1 box: min (b.z,b.w,c.x) max (c.y,c.z,c.w)
 #ifdef RT_FMA_TRAVERSAL
-            // experiment (NOT bit-exact): contracted slab test, plane * inv - origin * inv in one FFMA per plane
-            const f3 noi = mk3(-(o.x * inv.x), -(o.y * inv.y), -(o.z * inv.z));
-            f3 t00 = mk3(__fmaf_rn(a.x, inv.x, noi.x), __fmaf_rn(a.y, inv.y, noi.y), __fmaf_rn(a.z, inv.z, noi.z));
-            f3 t01 = mk3(__fmaf_rn(a.w, inv.x, noi.x), __fmaf_rn(b.x, inv.y, noi.y), __fmaf_rn(b.y, inv.z, noi.z));
-            f3 t10 = mk3(__fmaf_rn(b.z, inv.x, noi.x), __fmaf_rn(b.w, inv.y, noi.y), __fmaf_rn(c.x, inv.z, noi.z));
-            f3 t11 = mk3(__fmaf_rn(c.y, inv.x, noi.x), __fmaf_rn(c.z, inv.y, noi.y), __fmaf_rn(c.w, inv.z, noi.z));
+                // experiment (NOT bit-exact): contracted slab test, plane * inv - origin * inv in one FFMA per plane
+                const f3 noi = mk3(-(o.x * inv.x), -(o.y * inv.y), -(o.z * inv.z));
+                f3 t00 = mk3(__fmaf_rn(a.x, inv.x, noi.x), __fmaf_rn(a.y, inv.y, noi.y), __fmaf_rn(a.z, inv.z, noi.z));
+                f3 t01 = mk3(__fmaf_rn(a.w, inv.x, noi.x), __fmaf_rn(b.x, inv.y, noi.y), __fmaf_rn(b.y, inv.z, noi.z));
+                f3 t10 = mk3(__fmaf_rn(b.z, inv.x, noi.x), __fmaf_rn(b.w, inv.y, noi.y), __fmaf_rn(c.x, inv.z, noi.z));
+                f3 t11 = mk3(__fmaf_rn(c.y, inv.x, noi.x), __fmaf_rn(c.z, inv.y, noi.y), __fmaf_rn(c.w, inv.z, noi.z));
 #else
-            f3 t00 = (mk3(a.x, a.y, a.z) - o) * inv, t01 = (mk3(a.w, b.x, b.y) - o) * inv;
-            f3 t10 = (mk3(b.z, b.w, c.x) - o) * inv, t11 = (mk3(c.y, c.z, c.w) - o) * inv;
+                f3 t00 = (mk3(a.x, a.y, a.z) - o) * inv, t01 = (mk3(a.w, b.x, b.y) - o) * inv;
+                f3 t10 = (mk3(b.z, b.w, c.x) - o) * inv, t11 = (mk3(c.y, c.z, c.w) - o) * inv;
 #endif
-            float lo0 = fmaxf(fmaxf(fmaxf(fminf(t00.x, t01.x), fminf(t00.y, t01.y)), fminf(t00.z, t01.z)), t_min);
-            float hi0 = fminf(fminf(fmaxf(t00.x, t01.x), fmaxf(t00.y, t01.y)), fmaxf(t00.z, t01.z));
-            float lo1 = fmaxf(fmaxf(fmaxf(fminf(t10.x, t11.x), fminf(t10.y, t11.y)), fminf(t10.z, t11.z)), t_min);
-            float hi1 = fminf(fminf(fmaxf(t10.x, t11.x), fmaxf(t10.y, t11.y)), fmaxf(t10.z, t11.z));
-            bool h0 = fminf(hi0, t_max) >= lo0, h1 = fminf(hi1, t_max) >= lo1;
-            int r0 = __float_as_int(m.x), r1 = __float_as_int(m.y);
-            uint32_t axis = __float_as_uint(m.z);
-            bool swap = SMEM == 1 ? ((sign_bits >> axis) & 1u) != 0u : (axis == 0 ? sx : (axis == 1 ? sy : sz));   // near child = second iff inv_dir[axis] < 0
-            int near_ref = swap ? r1 : r0, far_ref = swap ? r0 : r1;
-            bool near_hit = swap ? h1 : h0, far_hit = swap ? h0 : h1;
-            float far_lo = swap ? lo0 : lo1;
+                float lo0 = fmaxf(fmaxf(fmaxf(fminf(t00.x, t01.x), fminf(t00.y, t01.y)), fminf(t00.z, t01.z)), t_min);
+                float hi0 = fminf(fminf(fmaxf(t00.x, t01.x), fmaxf(t00.y, t01.y)), fmaxf(t00.z, t01.z));
+                float lo1 = fmaxf(fmaxf(fmaxf(fminf(t10.x, t11.x), fminf(t10.y, t11.y)), fminf(t10.z, t11.z)), t_min);
+                float hi1 = fminf(fminf(fmaxf(t10.x, t11.x), fmaxf(t10.y, t11.y)), fmaxf(t10.z, t11.z));
+                bool h0 = fminf(hi0, t_max) >= lo0, h1 = fminf(hi1, t_max) >= lo1;
+                int r0 = __float_as_int(m.x), r1 = __float_as_int(m.y);
+                uint32_t axis = __float_as_uint(m.z);
+                bool swap = PACKED ? ((sign_bits >> axis) & 1u) != 0u : (axis == 0 ? sx : (axis == 1 ? sy : sz));   // near child = second iff inv_dir[axis] < 0
+                near_ref = swap ? r1 : r0; far_ref = swap ? r0 : r1;
+                near_hit = swap ? h1 : h0; far_hit = swap ? h0 : h1;
+                far_lo = swap ? lo0 : lo1;
+            }
             if (near_hit)
             {
                 if (far_hit)
                 {
-                    if (SMEM == 1) stack[sp] = make_int2(far_ref, __float_as_int(far_lo));
+                    if (PACKED) stack[sp] = make_int2(far_ref, __float_as_int(far_lo));
                     else { stack_ref[sp] = far_ref; stack_t[sp] = far_lo; }
                     ++sp;
                 }
@@ -222,7 +269,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
                 while (sp > 0)
                 {
                     --sp;
-                    if (SMEM == 1) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
+                    if (PACKED) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
                     else if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; }
                 }
                 if (!found) return prim;
@@ -233,7 +280,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
         for (;;)
         {
             const float4* tp = wtris + (size_t)ti * 3;
-            float4 q0 = ld_bvh<(SMEM == 1)>(tp), q1 = ld_bvh<(SMEM == 1)>(tp + 1), q2 = ld_bvh<(SMEM == 1)>(tp + 2);
+            float4 q0 = ld_bvh<PACKED>(tp), q1 = ld_bvh<PACKED>(tp + 1), q2 = ld_bvh<PACKED>(tp + 2);
             f3 p1 = mk3(q0.x, q0.y, q0.z), e1 = mk3(q0.w, q1.x, q1.y), e2 = mk3(q1.z, q1.w, q2.x);
             bool last = __float_as_uint(q2.y) != 0u;
 #ifdef RT_FMA_TRAVERSAL
@@ -273,7 +320,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
         while (sp > 0)
                 {
                     --sp;
-                    if (SMEM == 1) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
+                    if (PACKED) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
                     else if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; }
                 }
         if (!found) return prim;
@@ -294,7 +341,7 @@ template <bool ANY, bool COUNT, int SMEM, bool PIN>
 __device__ __forceinline__ uint32_t trace_staged(const DevScene& sc, int mode, const float4* s_bvh, float4 a, float4 b,
                                                  float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
 {
-    if (SMEM == 1) return trace_fast<ANY, COUNT, 1, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    if (SMEM == 1 || SMEM == 3) return trace_fast<ANY, COUNT, SMEM, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
     if (SMEM == 2) return trace_fast<ANY, COUNT, 2, PIN>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
     return trace<ANY, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
 }
