@@ -466,6 +466,47 @@ int rt_read_bvh(rt_ctx* ctx, RtLinearBVHNode* nodes, float* records, uint64_t* n
  * (the radix sort counts as one). */
 int rt_rebuild_bvh(rt_ctx* ctx, uint64_t* n_nodes);
 
+/* ---- BVH rebuild at SAH quality (new capability): parallel locally-ordered clustering (PLOC), built on the device ---------------
+ * Replaces the BVH, like rt_rebuild_bvh, by a tree over the device copy of the positions with one triangle per leaf, built by
+ * PLOC (Meister & Bittner 2018): a slower build than rt_rebuild_bvh's, for a tree that traces about as fast as the SAH tree of
+ * the upload (DESIGN.md section 4, "PLOC rebuild").  Which one pays off depends on how many frames the tree serves, which only
+ * the caller knows.  The rule, with n triangles and every operation in float without contraction, in the order written; min and
+ * max are the refit rule's, Union(A, B) is min(A.lo, B.lo), max(A.hi, B.hi) per component (order-sensitive for NaN and zeros):
+ *  1. Initial clusters: the triangles in the ascending key order of rt_rebuild_bvh steps 1-3, each with the refit rule's leaf
+ *     box of its triangle, at positions 0 .. c - 1 (c = n).
+ *  2. Distance: A(lo, hi) = (ex*ey + ey*ez) + ez*ex with e = hi - lo, and A = +inf unless A >= 0 and finite (NaN, inf, inverted
+ *     boxes).  For positions i < j, d(i, j) = d(j, i) = A(Union(box_i, box_j)), the lower position first.
+ *  3. Nearest neighbour: nn(i) = the j != i in [i - R, i + R] with 0 <= j < c and the smallest d(i, j).  Ties go to the smaller
+ *     gap |j - i|, then to the pair whose lower position is even, then to the smaller j.  (Ties to the smallest j alone would chain
+ *     a run of equal boxes, such as coincident triangles, one merge per iteration and one level per triangle; this order pairs
+ *     the run off in neighbours, halving it.)  R = RT_PLOC_RADIUS.
+ *  4. Merge: i and j = nn(i) merge iff nn(j) = i.  The new cluster, an interior node, takes position min(i, j) with box
+ *     Union(box_lower, box_higher); the other position is removed and the list compacted in order.  Steps 2-4 repeat until one
+ *     cluster is left.  Distance and the tie order together order the pairs totally, so the first pair in that order is mutual:
+ *     each iteration merges at least one pair.
+ *  5. Each interior node (lower-position cluster L, higher H): cL = L.lo + L.hi, cH = H.lo + H.hi, delta_a = |cH_a - cL_a|; the
+ *     axis starts at 0, becomes 1 if delta_1 > delta_axis, then 2 if delta_2 > delta_axis (NaN compares false); the first child
+ *     is H iff cH_axis < cL_axis, else L.  The split axis is that axis.
+ *  6. Nodes, records, end-of-leaf flags and boxes follow rt_rebuild_bvh steps 5-6 (depth-first preorder, a leaf's offset is its
+ *     triangle id, boxes by the refit rule); the cluster boxes only steer the build.  Triangles are not reordered, so primitive
+ *     ids, emissive_indices, the leaf order rt_update_triangles expects, the AOVs and the light tables keep their meaning.
+ * The depth is not bounded by the rule (a chain of triangles whose extent grows geometrically merges one triangle per
+ * iteration): a tree deeper than 64 levels (root = 1; the 64-entry traversal stack) gives RT_ERR_UNSUPPORTED and writes
+ * nothing: the tree, records, refit map, shared-memory staging and a captured frame graph stay as they were.  rt_rebuild_bvh
+ * always succeeds on the same triangles.
+ * Memory: the tree group of rt_rebuild_bvh (either call allocates it, the other reuses it, so a context can alternate between
+ * the two builds) plus the clustering temporaries, allocated all-or-nothing at the first call of this function after an upload:
+ * about 97 bytes per triangle (the cluster list and its compaction target 64, the interior nodes 20, the parent links 8, the
+ * neighbours and flags 5) and the compaction's scratch.  If no rebuild of either kind has run since the upload, the call also
+ * allocates the tree group as rt_rebuild_bvh does and re-captures the frame graph (once the tree is known to fit); after that,
+ * calls of either build move no buffer, so a captured graph stays valid.
+ * Blocking: the host reads the cluster count after each iteration (about 50-70 for 50 000 triangles) and the depth flag before
+ * anything of the tree is written.  Ordering, fan-out over multi-device contexts, n_nodes and what frames see afterwards are as
+ * for rt_rebuild_bvh.  Errors: RT_ERR_NOT_READY before an upload, RT_ERR_UNSUPPORTED for the depth.  The launches count under
+ * RT_K_MISC and in rt_launch_count: 9 + 3 per iteration for n > 1 (the sort and each compaction count as one), 2 for n = 1. */
+#define RT_PLOC_RADIUS 16
+int rt_rebuild_bvh_ploc(rt_ctx* ctx, uint64_t* n_nodes);
+
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);
 /* Hits of the rays currently in the incoming queue of `bounce` after rt_intersect(bounce): n = live rays;

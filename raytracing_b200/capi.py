@@ -38,7 +38,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
            "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh",
-           "rt_rebuild_bvh", "rt_bvh_staging"]
+           "rt_rebuild_bvh", "rt_bvh_staging", "rt_rebuild_bvh_ploc"]
 
 
 class RtSceneDesc(C.Structure):
@@ -128,6 +128,7 @@ def load_library():
     L.rt_update_triangles_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     L.rt_read_bvh.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     L.rt_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    L.rt_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -311,11 +312,15 @@ class Context:
         read.record(render)
         self._update_srcs = [(x, e) for x, e in self._update_srcs if not e.query()] + [(tris, read)]
 
-    def rebuild_bvh(self):
-        """Replace the BVH by a linear BVH over the current triangles, built on the device (rt_rebuild_bvh); -> the new node count
+    def rebuild_bvh(self, method="linear"):
+        """Replace the BVH by a tree over the current triangles, built on the device: method "linear" a linear BVH
+        (rt_rebuild_bvh, the faster build), "ploc" a clustered one (rt_rebuild_bvh_ploc, the faster trace); -> the new node count
         (2n - 1).  The triangles keep their ids; the accumulation is kept: call reset() if the geometry moved."""
+        fn = {"linear": self.lib.rt_rebuild_bvh, "ploc": self.lib.rt_rebuild_bvh_ploc}.get(method)
+        if fn is None:
+            raise ValueError("rebuild_bvh: method must be 'linear' or 'ploc', not %r" % (method,))
         n = C.c_uint64()
-        self._ck(self.lib.rt_rebuild_bvh(self.h, C.byref(n)))
+        self._ck(fn(self.h, C.byref(n)))
         self._n_nodes = n.value
         return n.value
 

@@ -44,6 +44,7 @@
 #include "rt_envmap.h"
 #include "rt_refit.cuh"
 #include "rt_lbvh.cuh"
+#include "rt_ploc.cuh"
 #include "rt_owned.h"
 
 using namespace rt;
@@ -1130,6 +1131,17 @@ struct rt_ctx
         uint4* inner = nullptr;                    // per internal node: first leaf, last leaf, split, axis
         uint2* top = nullptr;                      // the breadth-first top records by preorder (k_lbvh_top)
         char* sort_tmp = nullptr; size_t sort_bytes = 0;
+        // rt_rebuild_bvh_ploc's clustering temporaries (allocated at its first call, in tree_mem; clusters = null before)
+        struct Ploc
+        {
+            PlocCluster* clusters = nullptr;       // 2 x n: the list and the compaction's output
+            uint32_t* nn = nullptr; uint8_t* keep = nullptr;                  // per position
+            uint4* inner = nullptr; uint32_t* size = nullptr;                 // per interior node (k_ploc_merge)
+            uint32_t* parent = nullptr;            // per node reference
+            uint32_t* made = nullptr;              // device word: interior nodes allocated so far
+            uint32_t* host = nullptr;              // pinned: [0] the compaction's count, [1] the depth flag of k_ploc_number
+            char* select_tmp = nullptr; size_t select_bytes = 0;
+        } ploc;
     } lbvh;
     RtCamera camera = {};
     RayGenConsts raygen = {};
@@ -1184,7 +1196,7 @@ struct rt_ctx
     DevAllocs sd_mem;              // sd_col, sd_guide: while the spatial denoiser is on
     DevAllocs ad_mem;              // ad: while adaptive sampling is on
     DevAllocs scene_mem;           // the upload's arrays but the tree
-    DevAllocs tree_mem;            // scene.nodes_ref, scene.wnodes, the refit map, lbvh's temporaries
+    DevAllocs tree_mem;            // scene.nodes_ref, scene.wnodes, the refit map, lbvh's temporaries (the clustering's included)
     Staging stage;                 // rt_update_triangles' staging
     DevAllocs light_mem;           // the emitter and environment tables
     std::vector<std::unique_ptr<void, IpcClose>> ipc_opened;
@@ -1935,22 +1947,26 @@ int rt_read_bvh(rt_ctx* c, RtLinearBVHNode* nodes, float* records, uint64_t* n_r
     return RT_OK;
 }
 
-// ---- BVH rebuild: rt_rebuild_bvh (include/rt_b200.h, kernels in rt_lbvh.cuh)
+// ---- BVH rebuild: rt_rebuild_bvh and rt_rebuild_bvh_ploc (include/rt_b200.h, kernels in rt_lbvh.cuh and rt_ploc.cuh)
 
-// The first rebuild after an upload: the nodes, records and refit map of a tree of 2n - 1 nodes replace the upload's (which a
-// frame in flight may still read: blocking), and the build temporaries are allocated.  The new tree group replaces the old one
-// only once all of it is allocated, so a failure leaves the uploaded tree in place.
-static int alloc_lbvh(rt_ctx* c)
+// A rebuilt tree's group, allocated but not yet in place: the nodes, records and refit map of a tree of 2n - 1 nodes and the
+// linear BVH's temporaries.
+struct TreeGroup
+{
+    DevAllocs mem;
+    rt_ctx::Lbvh L;
+    float4 *nodes = nullptr, *wnodes = nullptr; uint2* link = nullptr; uint32_t *leaves = nullptr, *arrivals = nullptr;
+};
+
+static cudaError_t alloc_tree(rt_ctx* c, TreeGroup& t)
 {
     const size_t n = c->n_tris, nn = 2 * n - 1, n_rec = n > 1 ? n - 1 : 1;
-    DevAllocs g;
     cudaError_t e = cudaSuccess;
-    auto get = [&](auto*& view, size_t count) { if (e == cudaSuccess) e = g.alloc(view, count); };
-    rt_ctx::Lbvh L;
+    auto get = [&](auto*& view, size_t count) { if (e == cudaSuccess) e = t.mem.alloc(view, count); };
+    rt_ctx::Lbvh& L = t.L;
     L.live = true;
-    float4 *nodes = nullptr, *wnodes = nullptr; uint2* link = nullptr; uint32_t *leaves = nullptr, *arrivals = nullptr;
-    get(nodes, nn * 3); get(wnodes, n_rec * 4);                     // 3 float4 per RtLinearBVHNode, 4 per record
-    get(link, nn); get(leaves, n); get(arrivals, nn);
+    get(t.nodes, nn * 3); get(t.wnodes, n_rec * 4);                 // 3 float4 per RtLinearBVHNode, 4 per record
+    get(t.link, nn); get(t.leaves, n); get(t.arrivals, nn);
     get(L.bounds, 6); get(L.top, RT_BVH_TOP_RECORDS); get(L.inner, n_rec);
     for (int k = 0; k < 2; ++k) { get(L.codes[k], n); get(L.ids[k], n); }
     if (e == cudaSuccess)
@@ -1959,71 +1975,96 @@ static int alloc_lbvh(rt_ctx* c)
         e = cub::DeviceRadixSort::SortPairs(nullptr, L.sort_bytes, keys, vals, (int)n, 0, 30, c->stream);
         get(L.sort_tmp, L.sort_bytes ? L.sort_bytes : 16);
     }
+    return e;
+}
+
+// The new tree group replaces the current one (the caller has synchronised the render stream: a frame in flight may read it).
+static void install_tree(rt_ctx* c, TreeGroup& t)
+{
+    c->tree_mem = std::move(t.mem);                    // frees the uploaded nodes, records and refit map
+    c->scene.nodes_ref = t.nodes; c->scene.wnodes = t.wnodes;
+    c->refit_link = t.link; c->refit_leaves = t.leaves; c->refit_arrivals = t.arrivals;
+    c->lbvh = t.L;
+    ++c->config_gen;                                   // new buffers and sizes: the frame graph is re-captured
+}
+
+// The first rebuild after an upload: the new tree group replaces the old one only once all of it is allocated, so a failure
+// leaves the uploaded tree in place.
+static int alloc_lbvh(rt_ctx* c)
+{
+    TreeGroup t;
+    cudaError_t e = alloc_tree(c, t);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "rt_rebuild_bvh: allocating the rebuilt tree: %s", cudaGetErrorString(e));
-    c->tree_mem = std::move(g);                        // frees the uploaded nodes, records and refit map
-    c->scene.nodes_ref = nodes; c->scene.wnodes = wnodes;
-    c->refit_link = link; c->refit_leaves = leaves; c->refit_arrivals = arrivals;
-    c->lbvh = L;
-    ++c->config_gen;                                   // new buffers and sizes: the frame graph is re-captured
+    install_tree(c, t);
     return RT_OK;
 }
 
-int rt_rebuild_bvh(rt_ctx* c, uint64_t* n_nodes)
+// The clustering temporaries of rt_rebuild_bvh_ploc, about 97 bytes per triangle plus the compaction's scratch; P is set only
+// if all of them are allocated.
+static cudaError_t alloc_ploc(rt_ctx* c, DevAllocs& g, rt_ctx::Lbvh::Ploc& out)
 {
-    RT_CHECK_CTX(c); RT_FANOUT(c, rt_rebuild_bvh(k, n_nodes));
-    if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_rebuild_bvh: rt_upload_scene has not been called");
-    RT_CUDA(c, cudaSetDevice(c->device));
-    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the tree this call rewrites
-    if (!c->lbvh.live) { int rc = alloc_lbvh(c); if (rc) return rc; }
+    const size_t n = c->n_tris;
+    rt_ctx::Lbvh::Ploc P;
+    cudaError_t e = cudaSuccess;
+    auto get = [&](auto*& view, size_t count, bool host = false) { if (e == cudaSuccess) e = g.alloc(view, count, host); };
+    get(P.clusters, 2 * n); get(P.nn, n); get(P.keep, n); get(P.inner, n); get(P.size, n); get(P.parent, 2 * n);
+    get(P.made, 1); get(P.host, 2, true);
+    if (e == cudaSuccess)
+    {
+        e = cub::DeviceSelect::Flagged(nullptr, P.select_bytes, P.clusters, P.keep, P.clusters + n, P.host, (int)n, c->stream);
+        get(P.select_tmp, P.select_bytes ? P.select_bytes : 16);
+    }
+    if (e == cudaSuccess) out = P;
+    return e;
+}
+
+// Steps 1-3 of the build rule: the key-point bounds, the keys and their sort into keys.Current() (codes) / vals.Current() (ids).
+// k_lbvh_keys writes the end-of-leaf flags of the wtris records to `flags`.
+static int sort_keys(rt_ctx* c, rt_ctx::Lbvh& L, float4* flags, cub::DoubleBuffer<uint32_t>& keys, cub::DoubleBuffer<uint32_t>& vals)
+{
+    const uint32_t n = (uint32_t)c->n_tris;
+    RT_CUDA(c, cudaMemsetAsync(L.bounds, 0, 6 * 4, c->stream));
+    int rc;
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        const uint32_t g = std::min<uint32_t>(grid_for(n).x, (uint32_t)c->num_sms * 8u);
+        k_lbvh_bounds<<<g, 256, 0, c->stream>>>(c->scene.tris_ref, n, L.bounds);
+        if ((rc = post_launch(c, "k_lbvh_bounds"))) return rc;
+    }
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        k_lbvh_keys<<<grid_for(n), 256, 0, c->stream>>>(c->scene.tris_ref, n, L.bounds, L.codes[0], L.ids[0], flags);
+        if ((rc = post_launch(c, "k_lbvh_keys"))) return rc;
+    }
+    // a stable sort of the 30-bit codes with the ids (ascending) as values orders the keys (code << 32) | id
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        size_t bytes = L.sort_bytes;
+        RT_CUDA(c, cub::DeviceRadixSort::SortPairs(L.sort_tmp, bytes, keys, vals, (int)n, 0, 30, c->stream));
+        if ((rc = post_launch(c, "DeviceRadixSort"))) return rc;
+    }
+    return RT_OK;
+}
+
+// Steps 5-6 from the tree in radix-tree form (lbvh.inner, ipre, ids: the triangle of each leaf in preorder; unused for n = 1):
+// the top records, the nodes, records and refit map, then the boxes.
+static int write_tree(rt_ctx* c, const uint32_t* ipre, const uint32_t* ids)
+{
     rt_ctx::Lbvh& L = c->lbvh;
     DevScene& ds = c->scene;
     const uint32_t n = (uint32_t)c->n_tris, n_inner = n - 1;
     const uint32_t top_n = n_inner < RT_BVH_TOP_RECORDS ? n_inner : RT_BVH_TOP_RECORDS;
     float4* nodes = (float4*)ds.nodes_ref; float4* wnodes = (float4*)ds.wnodes; float4* wtris = (float4*)ds.wtris;
-    // Every launch below is a plain launch (none triggers dependent launches early), like the refit's: the next frame's
-    // traversal kernel, even one launched with programmatic dependent launch, sees the finished tree.
+    int rc;
     if (n == 1)
     {
         TimedLaunch t(c, RT_K_MISC);
         k_lbvh_single<<<1, 1, 0, c->stream>>>(nodes, wnodes, wtris, c->refit_link, c->refit_leaves);
-        int rc = post_launch(c, "k_lbvh_single"); if (rc) return rc;
+        if ((rc = post_launch(c, "k_lbvh_single"))) return rc;
     }
     else
     {
-        RT_CUDA(c, cudaMemsetAsync(L.bounds, 0, 6 * 4, c->stream));
-        int rc;
-        {
-            TimedLaunch t(c, RT_K_MISC);
-            const uint32_t g = std::min<uint32_t>(grid_for(n).x, (uint32_t)c->num_sms * 8u);
-            k_lbvh_bounds<<<g, 256, 0, c->stream>>>(ds.tris_ref, n, L.bounds);
-            if ((rc = post_launch(c, "k_lbvh_bounds"))) return rc;
-        }
-        {
-            TimedLaunch t(c, RT_K_MISC);
-            k_lbvh_keys<<<grid_for(n), 256, 0, c->stream>>>(ds.tris_ref, n, L.bounds, L.codes[0], L.ids[0], wtris);
-            if ((rc = post_launch(c, "k_lbvh_keys"))) return rc;
-        }
-        // a stable sort of the 30-bit codes with the ids (ascending) as values orders the keys (code << 32) | id
-        cub::DoubleBuffer<uint32_t> keys(L.codes[0], L.codes[1]), vals(L.ids[0], L.ids[1]);
-        {
-            TimedLaunch t(c, RT_K_MISC);
-            size_t bytes = L.sort_bytes;
-            RT_CUDA(c, cub::DeviceRadixSort::SortPairs(L.sort_tmp, bytes, keys, vals, (int)n, 0, 30, c->stream));
-            if ((rc = post_launch(c, "DeviceRadixSort"))) return rc;
-        }
-        const uint32_t* codes = keys.Current(); const uint32_t* ids = vals.Current();
-        uint32_t* parent = keys.Alternate(); uint32_t* ipre = vals.Alternate();       // the sort's inputs are dead
-        {
-            TimedLaunch t(c, RT_K_MISC);
-            k_lbvh_karras<<<grid_for(n_inner), 256, 0, c->stream>>>(codes, ids, n, L.inner, parent);
-            if ((rc = post_launch(c, "k_lbvh_karras"))) return rc;
-        }
-        {
-            TimedLaunch t(c, RT_K_MISC);
-            k_lbvh_number<<<grid_for(n_inner), 256, 0, c->stream>>>(L.inner, parent, n_inner, ipre);
-            if ((rc = post_launch(c, "k_lbvh_number"))) return rc;
-        }
         {
             TimedLaunch t(c, RT_K_MISC);
             k_lbvh_top<<<1, 1024, 0, c->stream>>>(L.inner, ipre, top_n, L.top);
@@ -2044,8 +2085,133 @@ int rt_rebuild_bvh(rt_ctx* c, uint64_t* n_nodes)
         TimedLaunch t(c, RT_K_MISC);
         k_refit<<<grid_for(n), 256, 0, c->stream>>>(c->refit_leaves, n, c->refit_link, c->refit_arrivals, (float*)nodes, ds.tris_ref,
                                                     (float*)wnodes);
-        int rc = post_launch(c, "k_refit"); if (rc) return rc;
+        if ((rc = post_launch(c, "k_refit"))) return rc;
     }
+    return RT_OK;
+}
+
+int rt_rebuild_bvh(rt_ctx* c, uint64_t* n_nodes)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_rebuild_bvh(k, n_nodes));
+    if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_rebuild_bvh: rt_upload_scene has not been called");
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the tree this call rewrites
+    if (!c->lbvh.live) { int rc = alloc_lbvh(c); if (rc) return rc; }
+    rt_ctx::Lbvh& L = c->lbvh;
+    const uint32_t n = (uint32_t)c->n_tris, n_inner = n - 1;
+    // Every launch below is a plain launch (none triggers dependent launches early), like the refit's: the next frame's
+    // traversal kernel, even one launched with programmatic dependent launch, sees the finished tree.
+    const uint32_t* ipre = nullptr; const uint32_t* ids = nullptr;
+    int rc;
+    if (n > 1)
+    {
+        cub::DoubleBuffer<uint32_t> keys(L.codes[0], L.codes[1]), vals(L.ids[0], L.ids[1]);
+        if ((rc = sort_keys(c, L, (float4*)c->scene.wtris, keys, vals))) return rc;
+        const uint32_t* codes = keys.Current(); ids = vals.Current();
+        uint32_t* parent = keys.Alternate(); uint32_t* pre = vals.Alternate();       // the sort's inputs are dead
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_karras<<<grid_for(n_inner), 256, 0, c->stream>>>(codes, ids, n, L.inner, parent);
+            if ((rc = post_launch(c, "k_lbvh_karras"))) return rc;
+        }
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_lbvh_number<<<grid_for(n_inner), 256, 0, c->stream>>>(L.inner, parent, n_inner, pre);
+            if ((rc = post_launch(c, "k_lbvh_number"))) return rc;
+        }
+        ipre = pre;
+    }
+    if ((rc = write_tree(c, ipre, ids))) return rc;
+    if (n_nodes) *n_nodes = c->n_nodes;
+    return RT_OK;
+}
+
+int rt_rebuild_bvh_ploc(rt_ctx* c, uint64_t* n_nodes)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_rebuild_bvh_ploc(k, n_nodes));
+    if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_rebuild_bvh_ploc: rt_upload_scene has not been called");
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the tree this call rewrites
+    // The first call after an upload builds in a new tree group, which replaces the uploaded tree only once the clustered tree is
+    // known to fit the traversal stack.  The first call after rt_rebuild_bvh adds the clustering temporaries to its group.
+    TreeGroup fresh;
+    const bool install = !c->lbvh.live;
+    rt_ctx::Lbvh& L = install ? fresh.L : c->lbvh;
+    if (!L.ploc.clusters)
+    {
+        DevAllocs g;
+        cudaError_t e = install ? alloc_tree(c, fresh) : cudaSuccess;
+        if (e == cudaSuccess) e = alloc_ploc(c, g, L.ploc);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "rt_rebuild_bvh_ploc: allocating the rebuilt tree: %s", cudaGetErrorString(e));
+        (install ? fresh.mem : c->tree_mem).adopt(std::move(g));
+    }
+    rt_ctx::Lbvh::Ploc& P = L.ploc;
+    const uint32_t n = (uint32_t)c->n_tris;
+    // Plain launches only, as in rt_rebuild_bvh.
+    const uint32_t* ipre = nullptr; const uint32_t* ids = nullptr;
+    int rc;
+    if (n > 1)
+    {
+        cub::DoubleBuffer<uint32_t> keys(L.codes[0], L.codes[1]), vals(L.ids[0], L.ids[1]);
+        // k_lbvh_keys' end-of-leaf flags land in the cluster list (48 of its 64 bytes per triangle), which k_ploc_init then
+        // overwrites: nothing of the current tree changes before the depth check (k_ploc_flags writes the flags after it)
+        if ((rc = sort_keys(c, L, (float4*)P.clusters, keys, vals))) return rc;
+        RT_CUDA(c, cudaMemsetAsync(P.parent, 0xFF, (2ull * n - 1) * 4, c->stream));
+        RT_CUDA(c, cudaMemsetAsync(P.made, 0, 4, c->stream));
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_ploc_init<<<grid_for(n), 256, 0, c->stream>>>(vals.Current(), n, c->scene.tris_ref, P.clusters);
+            if ((rc = post_launch(c, "k_ploc_init"))) return rc;
+        }
+        PlocCluster *cur = P.clusters, *next = P.clusters + n;
+        for (uint32_t count = n; count > 1; std::swap(cur, next))
+        {
+            {
+                TimedLaunch t(c, RT_K_MISC);
+                k_ploc_nearest<<<grid_for(count, RT_PLOC_TILE), RT_PLOC_TILE, 0, c->stream>>>(cur, count, P.nn);
+                if ((rc = post_launch(c, "k_ploc_nearest"))) return rc;
+            }
+            {
+                TimedLaunch t(c, RT_K_MISC);
+                k_ploc_merge<<<grid_for(count), 256, 0, c->stream>>>(cur, count, P.nn, P.keep, n, P.made, P.inner, P.size, P.parent);
+                if ((rc = post_launch(c, "k_ploc_merge"))) return rc;
+            }
+            {
+                TimedLaunch t(c, RT_K_MISC);
+                size_t bytes = P.select_bytes;
+                RT_CUDA(c, cub::DeviceSelect::Flagged(P.select_tmp, bytes, cur, P.keep, next, P.host, (int)count, c->stream));
+                if ((rc = post_launch(c, "DeviceSelect"))) return rc;
+            }
+            RT_CUDA(c, cudaStreamSynchronize(c->stream));
+            if (P.host[0] >= count) RT_FAIL(c, RT_ERR_CUDA, "rt_rebuild_bvh_ploc: an iteration merged no pair");
+            count = P.host[0];
+        }
+        uint32_t* leaf_ids = keys.Current(); uint32_t* pre = vals.Alternate();      // the codes and the sort's inputs are dead
+        P.host[1] = 0;
+        {
+            TimedLaunch t(c, RT_K_MISC);
+            k_ploc_number<<<grid_for(2 * n - 1), 256, 0, c->stream>>>(n, P.inner, P.size, P.parent, leaf_ids, L.inner, pre, P.host + 1);
+            if ((rc = post_launch(c, "k_ploc_number"))) return rc;
+        }
+        RT_CUDA(c, cudaStreamSynchronize(c->stream));
+        if (P.host[1])
+            RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_rebuild_bvh_ploc: the clustered tree is deeper than the 64 levels of the traversal "
+                    "stack; the tree is unchanged (rt_rebuild_bvh builds a tree of at most 62 levels over any triangles)");
+        ipre = pre; ids = leaf_ids;
+    }
+    if (install)
+    {
+        RT_CUDA(c, cudaStreamSynchronize(c->stream));
+        install_tree(c, fresh);
+    }
+    if (n > 1)
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        k_ploc_flags<<<grid_for(n), 256, 0, c->stream>>>(n, (float4*)c->scene.wtris);
+        if ((rc = post_launch(c, "k_ploc_flags"))) return rc;
+    }
+    if ((rc = write_tree(c, ipre, ids))) return rc;
     if (n_nodes) *n_nodes = c->n_nodes;
     return RT_OK;
 }

@@ -67,21 +67,11 @@ __device__ __forceinline__ void refit_store(float* nodes_ref, float* wnodes, uin
     w[0] = lo[0]; w[1] = lo[1]; w[2] = lo[2]; w[3] = hi[0]; w[4] = hi[1]; w[5] = hi[2];
 }
 
-// Bottom-up refit, one thread per leaf.  Leaf box: start at (FLT_MAX, -FLT_MAX) and fold Union(Bounds3(p1, p2), p3) of every
-// triangle in leaf order (Triangle::GetBounds).  The thread then publishes the box (__threadfence, then one atomicAdd on the
-// parent's arrival counter); the second thread to arrive reads both children back from L2 and writes Union(first, second), and
-// climbs.  Every box is a fixed function of its children, so the result does not depend on the arrival order.  The depth is at
-// most 64 (build_layout checks it), which bounds the climb.  tris_ref holds the new positions (k_refit_records ran before).
-__global__ void __launch_bounds__(256) k_refit(const uint32_t* __restrict__ leaves, uint32_t n_leaves, const uint2* __restrict__ link,
-                                               uint32_t* arrivals, float* nodes_ref, const float4* __restrict__ tris_ref, float* wnodes)
+// Leaf box of triangles off .. off + count - 1: start at (FLT_MAX, -FLT_MAX) and fold Union(Bounds3(p1, p2), p3) of every
+// triangle in leaf order (Triangle::GetBounds).
+__device__ __forceinline__ void refit_leaf_box(const float4* __restrict__ tris_ref, uint32_t off, uint32_t count, float* lo, float* hi)
 {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_leaves) return;
-    uint32_t node = leaves[i];
-    const float4* nodes4 = reinterpret_cast<const float4*>(nodes_ref);
-    const float4 meta = __ldcg(nodes4 + (size_t)node * 3 + 2);
-    const uint32_t off = __float_as_uint(meta.x), count = __float_as_uint(meta.y) >> 16;
-    float lo[3] = { FLT_MAX, FLT_MAX, FLT_MAX }, hi[3] = { -FLT_MAX, -FLT_MAX, -FLT_MAX };
+    lo[0] = FLT_MAX; lo[1] = FLT_MAX; lo[2] = FLT_MAX; hi[0] = -FLT_MAX; hi[1] = -FLT_MAX; hi[2] = -FLT_MAX;
     for (uint32_t k = 0; k < count; ++k)
     {
         const float4* t = tris_ref + (size_t)(off + k) * 3;
@@ -93,6 +83,23 @@ __global__ void __launch_bounds__(256) k_refit(const uint32_t* __restrict__ leav
         hi[1] = refit_max(hi[1], refit_max(refit_max(p1.y, p2.y), p3.y));
         hi[2] = refit_max(hi[2], refit_max(refit_max(p1.z, p2.z), p3.z));
     }
+}
+
+// Bottom-up refit, one thread per leaf, from its refit_leaf_box.  The thread then publishes the box (__threadfence, then one
+// atomicAdd on the parent's arrival counter); the second thread to arrive reads both children back from L2 and writes
+// Union(first, second), and climbs.  Every box is a fixed function of its children, so the result does not depend on the arrival order.  The depth is at
+// most 64 (build_layout checks it), which bounds the climb.  tris_ref holds the new positions (k_refit_records ran before).
+__global__ void __launch_bounds__(256) k_refit(const uint32_t* __restrict__ leaves, uint32_t n_leaves, const uint2* __restrict__ link,
+                                               uint32_t* arrivals, float* nodes_ref, const float4* __restrict__ tris_ref, float* wnodes)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_leaves) return;
+    uint32_t node = leaves[i];
+    const float4* nodes4 = reinterpret_cast<const float4*>(nodes_ref);
+    const float4 meta = __ldcg(nodes4 + (size_t)node * 3 + 2);
+    const uint32_t off = __float_as_uint(meta.x), count = __float_as_uint(meta.y) >> 16;
+    float lo[3], hi[3];
+    refit_leaf_box(tris_ref, off, count, lo, hi);
     for (;;)
     {
         const uint2 l = link[node];

@@ -150,10 +150,10 @@ void CUDAPathTraceIntegrator::UpdateTriangles(const Triangle* triangles, size_t 
     Check(rt_update_triangles(ctx_, triangles, count), "UpdateTriangles");
 }
 
-std::uint64_t CUDAPathTraceIntegrator::RebuildBvh()
+std::uint64_t CUDAPathTraceIntegrator::RebuildBvh(BvhBuild build)
 {
     std::uint64_t n_nodes = 0;
-    Check(rt_rebuild_bvh(ctx_, &n_nodes), "RebuildBvh");
+    Check(build == BvhBuild::kPloc ? rt_rebuild_bvh_ploc(ctx_, &n_nodes) : rt_rebuild_bvh(ctx_, &n_nodes), "RebuildBvh");
     return n_nodes;
 }
 

@@ -52,6 +52,8 @@ class CUDAPathTraceIntegrator : public Integrator
 {
 public:
     enum class Schedule { kFrame, kFused, kStepwise };
+    // RebuildBvh: kLinear a linear BVH (rt_rebuild_bvh, the faster build), kPloc clustering (rt_rebuild_bvh_ploc, the faster trace)
+    enum class BvhBuild { kLinear, kPloc };
 
     CUDAPathTraceIntegrator(std::uint32_t width, std::uint32_t height, AccelerationStructure& acc_structure,
                             int device = 0, Schedule schedule = Schedule::kFrame);
@@ -97,9 +99,10 @@ public:
     // materials are kept); the BVH is refit on the device.  No reset: like a camera move, whether the old samples are kept is the
     // caller's choice (RequestReset() starts over; an animation that keeps them gets motion blur).
     void UpdateTriangles(const Triangle* triangles, size_t count);
-    // BVH rebuild (rt_rebuild_bvh): replaces the tree by a linear BVH over the current triangles, built on the device, when a refit
-    // no longer traces well; returns the new node count (2n - 1).  Triangle ids do not change.  No reset, as above.
-    std::uint64_t RebuildBvh();
+    // BVH rebuild (rt_rebuild_bvh, or rt_rebuild_bvh_ploc for BvhBuild::kPloc): replaces the tree by one over the current
+    // triangles, built on the device, when a refit no longer traces well; returns the new node count (2n - 1).  Triangle ids do
+    // not change.  No reset, as above.
+    std::uint64_t RebuildBvh(BvhBuild build = BvhBuild::kLinear);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

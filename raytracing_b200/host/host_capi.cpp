@@ -214,6 +214,11 @@ int rth_render_rebuild_bvh(void* h, std::uint64_t* n_nodes)
     try { *n_nodes = ((RenderHandle*)h)->render->RebuildBvh(); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_rebuild_bvh_ploc(void* h, std::uint64_t* n_nodes)
+{
+    try { *n_nodes = ((RenderHandle*)h)->render->RebuildBvh(Render::BvhBuild::kPloc); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_active_pixels(void* h, std::uint32_t* n)
 {
     try { *n = ((RenderHandle*)h)->render->ActivePixels(); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

@@ -58,7 +58,8 @@ public:
     void UpdateTriangles(const Triangle* triangles, size_t count) { Cuda().UpdateTriangles(triangles, count); }
     // BVH rebuild (CUDAPathTraceIntegrator::RebuildBvh): a device-built tree over the current triangles; returns its node count.
     // Keeps the accumulation, as above
-    std::uint64_t RebuildBvh() { return Cuda().RebuildBvh(); }
+    using BvhBuild = CUDAPathTraceIntegrator::BvhBuild;
+    std::uint64_t RebuildBvh(BvhBuild build = BvhBuild::kLinear) { return Cuda().RebuildBvh(build); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

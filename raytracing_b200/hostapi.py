@@ -50,6 +50,7 @@ def load_library():
     L.rth_render_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
     L.rth_render_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.rth_render_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    L.rth_render_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_sampler.argtypes = [C.c_void_p, C.c_int]
@@ -249,11 +250,14 @@ class HostRender:
         if self.L.rth_render_update_triangles(self.h, t.ctypes.data, t.shape[0]) != 0:
             raise _err(self.L)
 
-    def rebuild_bvh(self):
-        """Render::RebuildBvh: a linear BVH over the current triangles, built on the device; -> the new node count (2n - 1).
-        Keeps the accumulation (request_reset() starts over)."""
+    def rebuild_bvh(self, method="linear"):
+        """Render::RebuildBvh: a tree over the current triangles, built on the device, by method "linear" (BvhBuild::kLinear) or
+        "ploc" (BvhBuild::kPloc); -> the new node count (2n - 1).  Keeps the accumulation (request_reset() starts over)."""
+        fn = {"linear": self.L.rth_render_rebuild_bvh, "ploc": self.L.rth_render_rebuild_bvh_ploc}.get(method)
+        if fn is None:
+            raise ValueError("rebuild_bvh: method must be 'linear' or 'ploc', not %r" % (method,))
         n = C.c_uint64()
-        if self.L.rth_render_rebuild_bvh(self.h, C.byref(n)) != 0:
+        if fn(self.h, C.byref(n)) != 0:
             raise _err(self.L)
         return n.value
 

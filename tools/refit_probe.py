@@ -14,10 +14,11 @@ the GPU's name and power limit read in the same run.
 
   python tools/refit_probe.py --rebuild [--scenes ...] [--rigid 0.05,0.2] [--amplitudes 0.01,0.02,0.05,0.2,1.0]
 
-The device rebuild instead (rt_rebuild_bvh): the first call (allocates and re-captures) and the median of 5 later calls as wall
-time to the end of rt_sync, their device time (RT_K_MISC events) and, from torch.profiler, the device time of each kernel; the
-frame time of the undeformed scene with the uploaded SAH tree and with the rebuilt tree; and, for rigid moves and per-vertex
-noise of growing amplitude, the frame time after a refit of the uploaded tree against the frame time after a device rebuild.
+The device rebuilds instead (rt_rebuild_bvh "linear" and rt_rebuild_bvh_ploc "ploc", --methods), each in a context of its own:
+the first call (allocates and re-captures) and the median of 5 later calls as wall time to the end of rt_sync, their device time
+(RT_K_MISC events) and, from torch.profiler, the device time of each kernel and the PLOC iteration count; the frame time of the
+undeformed scene with the uploaded SAH tree and with the rebuilt tree; and, for rigid moves and per-vertex noise of growing
+amplitude, the frame time after a refit of the uploaded tree against the frame time after each device rebuild.
 """
 import argparse
 import json
@@ -79,51 +80,61 @@ def update_ms(c, src, runs=5):
     return float(np.median(wall)), float(np.median(dev))
 
 
-def rebuild_ms(c, runs=5):
-    """(median wall ms of rt_rebuild_bvh to the end of rt_sync, median device ms of its launches)."""
+def rebuild_ms(c, method, runs=5):
+    """(median wall ms of the rebuild to the end of rt_sync, median device ms of its launches)."""
     wall, dev = [], []
     c.set_option(capi.OPT_KERNEL_TIMING, 1)
     for _ in range(runs):
         c.kernel_times()
-        wall.append(timed(c.rebuild_bvh, c.sync))
+        wall.append(timed(lambda: c.rebuild_bvh(method), c.sync))
         dev.append(c.kernel_times()["misc"][0])
     c.set_option(capi.OPT_KERNEL_TIMING, 0)
     return float(np.median(wall)), float(np.median(dev))
 
 
-def kernel_ms(c, runs=3):
-    """Device ms per kernel name of one rebuild (torch.profiler, mean over `runs` rebuilds)."""
+def kernel_ms(c, method, runs=3):
+    """(device ms per kernel name of one rebuild, launches per kernel name of one rebuild) from torch.profiler, mean over `runs`
+    rebuilds; the PLOC iterations are the launches of k_ploc_nearest."""
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(runs):
-            c.rebuild_bvh()
+            c.rebuild_bvh(method)
         c.sync()
-    out = {}
+    out, count = {}, {}
     for e in prof.key_averages():
         if e.device_type.name == "CUDA" and e.device_time_total > 0:
             out[e.key[:60]] = round(e.device_time_total / 1e3 / runs, 4)
-    return out
+            count[e.key[:60]] = e.count // runs
+    return out, count
 
 
 def rebuild_arm(a, name, sc, cam, emit):
     n = len(sc["triangles"])
-    c = capi.Context(a.width, a.height)
-    c.upload_scene(sc); c.set_camera(cam)
-    sah_ms = frame_ms(c, a.bounces)
-    first = timed(c.rebuild_bvh, c.sync)
-    wall, dev = rebuild_ms(c)
-    emit({"scene": name, "triangles": n, "nodes_sah": len(sc["nodes"]), "first_rebuild_ms": first, "rebuild_ms": wall,
-          "rebuild_device_ms": dev, "kernels_ms": kernel_ms(c), "frame_ms_sah": sah_ms, "frame_ms_lbvh": frame_ms(c, a.bounces)})
+    ctx = {}
+    for method in a.methods.split(","):
+        c = ctx[method] = capi.Context(a.width, a.height)
+        c.upload_scene(sc); c.set_camera(cam)
+        sah_ms = frame_ms(c, a.bounces)
+        first = timed(lambda: c.rebuild_bvh(method), c.sync)
+        wall, dev = rebuild_ms(c, method)
+        kernels, launches = kernel_ms(c, method)
+        emit({"scene": name, "method": method, "triangles": n, "nodes_sah": len(sc["nodes"]), "first_rebuild_ms": first,
+              "rebuild_ms": wall, "rebuild_device_ms": dev, "iterations": next((v for k, v in launches.items() if k.startswith("k_ploc_nearest")), None),
+              "kernels_ms": kernels, "frame_ms_sah": sah_ms, "frame_ms_rebuilt": frame_ms(c, a.bounces)})
     refit = capi.Context(a.width, a.height)
     refit.upload_scene(sc); refit.set_camera(cam)
     moves = [("rigid", float(x)) for x in a.rigid.split(",") if x] + [("noise", float(x)) for x in a.amplitudes.split(",") if x]
     for kind, amp in moves:
         tt = deform(sc["triangles"], kind, seed=3, amount=amp)
         refit.update_triangles(tt)
-        c.update_triangles(tt); c.rebuild_bvh()
-        emit({"scene": name, "deformation": kind, "amplitude": amp, "frame_ms_refit": frame_ms(refit, a.bounces),
-              "frame_ms_rebuilt": frame_ms(c, a.bounces)})
-    refit.destroy(); c.destroy()
+        row = {"scene": name, "deformation": kind, "amplitude": amp, "frame_ms_refit": frame_ms(refit, a.bounces)}
+        for method, c in ctx.items():
+            c.update_triangles(tt); c.rebuild_bvh(method)
+            row["frame_ms_" + method] = frame_ms(c, a.bounces)
+        emit(row)
+    refit.destroy()
+    for c in ctx.values():
+        c.destroy()
 
 
 def main():
@@ -136,6 +147,7 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--rebuild", action="store_true", help="measure rt_rebuild_bvh instead of rt_update_triangles")
     ap.add_argument("--rigid", default="0.05,0.2", help="--rebuild: amplitudes of the rigid moves (empty: none)")
+    ap.add_argument("--methods", default="linear,ploc", help="--rebuild: the device builds to measure (rt_rebuild_bvh, rt_rebuild_bvh_ploc)")
     a = ap.parse_args()
     import torch
 
