@@ -102,11 +102,13 @@ typedef enum RtOption {
     RT_OPT_ENV_SAMPLING = 31,   /* 0 (default): the environment map adds light only when a BSDF-sampled ray misses; 1: next-event
                                    estimation on the environment map too, combined with BSDF sampling by MIS (the environment-sampling
                                    block below; the image converges to the same expectation) */
-    RT_OPT_OCTANT_BVH = 32      /* 1 (default): a scene staged whole into shared memory (RT_OPT_SMEM_BVH) whose interior records fit
+    RT_OPT_OCTANT_BVH = 32,     /* 1 (default): a scene staged whole into shared memory (RT_OPT_SMEM_BVH) whose interior records fit
                                    eight more times within the same 40 KB is traversed through per-direction-octant copies of
                                    the records that every CTA builds after staging: the box test needs no pairwise min/max and
                                    no near/far selection (the per-phase kernels; the one-kernel frame keeps the canonical records).
                                    0: the canonical records only.  Results are bit-identical */
+    RT_OPT_OBJECT_MOTION = 33   /* 0 (default): the motion-vector AOV follows the camera only (as the reference's); 1: it also follows
+                                   rt_update_triangles* (the object-motion block below) */
 } RtOption;
 
 #define RT_MAX_BOUNCES 255u     /* bounce index range supported per frame (reference GUI: 0..5) */
@@ -402,8 +404,8 @@ int rt_set_light_selection(rt_ctx* ctx, float analytic, float emitters, float en
  * Ordering: the update is enqueued on the render stream after everything submitted before it (a shadow pass deferred by
  * RT_OPT_OVERLAP 2 is launched first, the second stream of RT_OPT_OVERLAP 1 is joined) and is asynchronous; the next frame sees the
  * new geometry.  The buffers keep their sizes and addresses, so a captured frame graph stays valid.  The accumulation is kept, as
- * for a camera move: call rt_reset.  Motion vectors stay camera-only (as in the reference), so the temporal denoiser gets no help
- * from an update.  The sort-key origin of the sorted shading pass stays the upload's root-box centre (ray order, not results).
+ * for a camera move: call rt_reset.  Motion vectors stay camera-only (as in the reference) unless RT_OPT_OBJECT_MOTION is on (the
+ * object-motion block below), which lets the velocity AOV and the temporal denoiser follow the update.  The sort-key origin of the sorted shading pass stays the upload's root-box centre (ray order, not results).
  * rt_update_triangles reads the caller's array before it returns, through a pinned staging buffer of at most 2 x 32 MB (allocated
  * at the first call) whose copies overlap the record kernel.  rt_update_triangles_device reads `device_triangles` (RtTriangle
  * layout, 16-byte aligned device memory of the context's device, else RT_ERR_INVALID_ARGUMENT) on the render stream: the caller
@@ -417,6 +419,30 @@ int rt_set_light_selection(rt_ctx* ctx, float analytic, float emitters, float en
  * under RT_K_MISC (RT_OPT_KERNEL_TIMING) and in rt_launch_count. */
 int rt_update_triangles(rt_ctx* ctx, const RtTriangle* triangles, uint64_t n_triangles);
 int rt_update_triangles_device(rt_ctx* ctx, const void* device_triangles, uint64_t n_triangles);
+
+/* ---- object motion vectors (new capability): rt_set_option(ctx, RT_OPT_OBJECT_MOTION, 1) ------------------------------------------
+ * The velocity AOV of a bounce-0 hit follows the triangle's own motion as well as the camera's.  While the option is on, the context
+ * keeps the previous positions Q[t] = (q1, q2, q3) of every triangle t, in upload (leaf) order:
+ *     rt_upload_scene: Q = the uploaded positions;
+ *     switching the option from 0 to 1 after an upload: Q = the current positions (those of the last update, if any);
+ *     rt_update_triangles, rt_update_triangles_device: Q = every triangle's positions before the call, then the new ones are written
+ *     (in render-stream order, like the update itself);
+ *     unchanged by rt_rebuild_bvh, rt_rebuild_bvh_ploc, frames, rt_reset and camera changes (none of them moves a triangle).
+ * This mirrors the camera rule, where the previous camera is that of the previous rt_set_camera call: an animation that updates
+ * once per frame gets the motion of that frame; one that stops updating keeps the last update's motion until its next update.
+ * A bounce-0 hit on triangle t at barycentrics (u, v), w0 = 1 - u - v, all float without contraction, in the order written:
+ *     position = (p1 * w0 + p2 * u) + p3 * v;  prev = (q1 * w0 + q2 * u) + q3 * v;
+ *     velocity = project_screen(position, camera) - project_screen(prev, previous camera)   (aov.cl's projection, as with it off)
+ * With Q equal to the current positions, prev is position bit for bit and so is the velocity of the option off: turning the option on
+ * changes no output until the next update.  Misses, the albedo, depth and normal AOVs, radiance, statistics and every other view
+ * are unchanged; the temporal denoiser keeps its rule and reads these motion vectors; a pixel stopped by adaptive sampling keeps the
+ * AOVs of its last traced sample.  Values other than 0 and 1 are RT_ERR_INVALID_ARGUMENT.
+ * Device memory while the option is on and a scene is uploaded: 48 B per triangle (tris_ref's layout; 2.5 MB on CornellBox_Dragon,
+ * 481 MB on Synthetic10M), allocated when the option is turned on after an upload or at an upload with it on, freed when it is
+ * turned off.  If the allocation fails the call returns RT_ERR_CUDA and the option is off (an upload then leaves no scene).  Turning
+ * the option on or off re-captures the frame graph; updates with it on move no buffer, so a captured graph stays valid.  An update
+ * launches the same kernels with the option on (its record kernel also copies the old positions: about 96 B more per triangle).
+ * Multi-device contexts fan out: each device keeps its own Q. */
 /* Parity tap: the device's reference-layout nodes (n_nodes entries of the current tree: the upload's, or 2n - 1 after
  * rt_rebuild_bvh) and, if records != NULL, the traversal records
  * (16 floats per interior record, rt_bvh_layout.h; one zero record for a single-leaf tree); *n_records is set whenever n_records

@@ -22,6 +22,7 @@ OPT_AOV_ALWAYS, OPT_SMEM_BVH, OPT_OVERLAP, OPT_GRAPH, OPT_PDL, OPT_FRAME_KERNEL,
 OPT_EMITTER_SAMPLING = 30       # 1: next-event estimation on the emissive triangles, MIS with BSDF sampling (include/rt_b200.h)
 OPT_ENV_SAMPLING = 31           # 1: next-event estimation on the environment map, MIS with BSDF sampling (include/rt_b200.h)
 OPT_OCTANT_BVH = 32             # 1 (default): octant-ordered record copies for scenes staged whole in shared memory (include/rt_b200.h)
+OPT_OBJECT_MOTION = 33          # 1: the velocity AOV follows update_triangles as well as the camera (include/rt_b200.h)
 KERNEL_CLASSES = ["raygen", "intersect", "miss", "hit", "intersect_shadow", "accumulate", "extend_shade",
                   "shadow_accumulate", "resolve", "aov", "misc", "trace_closest", "shade_queues", "trace_both"]
 

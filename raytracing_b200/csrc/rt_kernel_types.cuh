@@ -74,6 +74,7 @@ struct AovParams
 {
     int enabled;
     float4* albedo; float* depth; float4* normal; float2* velocity;
+    const float4* prev_pos;        // RT_OPT_OBJECT_MOTION: the previous positions, 3 float4 per triangle (tris_ref layout); else nullptr
 };
 
 struct FrameDyn

@@ -134,7 +134,13 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         aov.albedo[li] = make_float4(material.diffuse_albedo.x, material.diffuse_albedo.y, material.diffuse_albedo.z, 0.0f);
         aov.depth[li] = length(ray_origin - position);
         aov.normal[li] = make_float4(normal.x, normal.y, normal.z, 0.0f);
-        f2 s0 = project_screen(position, p.dyn->cam), s1 = project_screen(position, p.dyn->prev);
+        f3 prev = position;
+        if (aov.prev_pos)
+        {   // object motion: the same barycentrics on the triangle's previous positions
+            const float4* qp = aov.prev_pos + (size_t)prim * 3;
+            prev = mk3(__ldg(qp)) * w0 + mk3(__ldg(qp + 1)) * u + mk3(__ldg(qp + 2)) * v;
+        }
+        f2 s0 = project_screen(position, p.dyn->cam), s1 = project_screen(prev, p.dyn->prev);
         aov.velocity[li] = make_float2(s0.x - s1.x, s0.y - s1.y);
     }
 
@@ -1121,6 +1127,10 @@ struct rt_ctx
     uint2* refit_link = nullptr; uint32_t* refit_leaves = nullptr; uint32_t* refit_arrivals = nullptr; uint32_t refit_n_leaves = 0;
     struct Staging { DevAllocs mem; char* host = nullptr; char* dev = nullptr; size_t half = 0; Owned<cudaEvent_t> copied[2]; };
     bool emit_moved = false;                       // emit_tris' positions predate an update: refresh_lights reads them from tris_ref
+    // object motion (RT_OPT_OBJECT_MOTION): the previous positions, tris_ref's layout, in motion_mem while the option is on and a
+    // scene is uploaded
+    int object_motion = 0;
+    float4* prev_pos = nullptr;
     // rt_rebuild_bvh: the build temporaries of the linear BVH (allocated with its nodes and records at the first rebuild after an
     // upload, in tree_mem; live = scene.nodes_ref / wnodes and the refit map hold a rebuilt tree's 2n - 1 nodes)
     struct Lbvh
@@ -1199,6 +1209,7 @@ struct rt_ctx
     DevAllocs tree_mem;            // scene.nodes_ref, scene.wnodes, the refit map, lbvh's temporaries (the clustering's included)
     Staging stage;                 // rt_update_triangles' staging
     DevAllocs light_mem;           // the emitter and environment tables
+    DevAllocs motion_mem;          // prev_pos: while object motion is on and a scene is uploaded
     std::vector<std::unique_ptr<void, IpcClose>> ipc_opened;
 };
 
@@ -1529,6 +1540,7 @@ AovParams aov_params(const rt_ctx* c)
     memset(&a, 0, sizeof(a));
     a.enabled = (aov_wanted(c) && c->aov_albedo) ? 1 : 0;
     a.albedo = c->aov_albedo; a.depth = c->aov_depth; a.normal = c->aov_normal; a.velocity = c->aov_velocity;
+    a.prev_pos = c->prev_pos;
     return a;
 }
 
@@ -1725,6 +1737,29 @@ static int refresh_lights(rt_ctx* c)
 // Either table exists: the sampled-light instances of the shading kernels run
 static bool lights_sampled(const rt_ctx* c) { return c->scene.emit_pdfA || c->scene.env_pdf; }
 
+// Object motion (RT_OPT_OBJECT_MOTION): the previous positions become the current ones, a device-to-device copy of tris_ref on the
+// render stream (after every update submitted before).  The buffer is allocated all-or-nothing at the first call after an upload;
+// if that fails the option is turned off.
+static int set_prev_positions(rt_ctx* c)
+{
+    const size_t n = (size_t)c->n_tris * 3;
+    if (!c->prev_pos)
+    {
+        DevAllocs g;
+        float4* q = nullptr;
+        const cudaError_t e = g.alloc(q, n);
+        if (e != cudaSuccess)
+        {
+            c->object_motion = 0;
+            RT_FAIL(c, RT_ERR_CUDA, "object motion: allocating the previous positions (%llu bytes) failed: %s", (unsigned long long)n * 16,
+                    cudaGetErrorString(e));
+        }
+        c->motion_mem = std::move(g); c->prev_pos = q;
+    }
+    RT_CUDA(c, cudaMemcpyAsync(c->prev_pos, c->scene.tris_ref, n * 16, cudaMemcpyDeviceToDevice, c->stream));
+    return RT_OK;
+}
+
 int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_upload_scene(k, s));
@@ -1768,6 +1803,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     { int rc = join_shadow(c); if (rc) return rc; }     // a shadow pass of an unfinished frame may still read the old scene
     RT_CUDA(c, cudaStreamSynchronize(c->stream));
     c->scene_mem.clear(); c->tree_mem.clear(); c->stage = {};
+    c->motion_mem.clear(); c->prev_pos = nullptr;
     c->refit_link = nullptr; c->refit_leaves = nullptr; c->refit_arrivals = nullptr; c->refit_n_leaves = 0;
     c->lbvh = rt_ctx::Lbvh();
     c->scene_ready = false;
@@ -1827,6 +1863,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     c->emit_moved = false;
     c->n_tris = s->n_triangles; c->n_nodes = s->n_nodes;
     c->analytic_lit = rtenv::analytic_lit(s->lights, s->scene_info.analytic_light_count);
+    if (c->object_motion && (rc = set_prev_positions(c))) return rc;
     c->scene_ready = true;
     ++c->config_gen;
     return refresh_lights(c);
@@ -1865,7 +1902,12 @@ static int launch_refit_records(rt_ctx* c, const void* src, uint32_t first, uint
 {
     DevScene& ds = c->scene;
     TimedLaunch t(c, RT_K_MISC);
-    k_refit_records<<<grid_for(n), 256, 0, c->stream>>>((const float4*)src, first, n, (float4*)ds.tris_ref, (float4*)ds.wtris, (float4*)ds.tri_shade);
+    if (c->prev_pos)       // object motion: the positions this launch overwrites become the previous ones
+        k_refit_records<true><<<grid_for(n), 256, 0, c->stream>>>((const float4*)src, first, n, (float4*)ds.tris_ref, (float4*)ds.wtris,
+                                                                  (float4*)ds.tri_shade, c->prev_pos);
+    else
+        k_refit_records<false><<<grid_for(n), 256, 0, c->stream>>>((const float4*)src, first, n, (float4*)ds.tris_ref, (float4*)ds.wtris,
+                                                                   (float4*)ds.tri_shade, nullptr);
     return post_launch(c, "k_refit_records");
 }
 
@@ -2282,6 +2324,18 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
         if ((int)value == c->env_sampling) return RT_OK;
         c->env_sampling = (int)value;
         return refresh_lights(c);
+    case RT_OPT_OBJECT_MOTION:
+        if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "object motion must be 0 (camera-only motion vectors) or 1 (triangle updates too)");
+        if ((int)value == c->object_motion) return RT_OK;
+        RT_CUDA(c, cudaSetDevice(c->device));
+        if (value == 0)
+        {   // a frame in flight may still read the previous positions
+            RT_CUDA(c, cudaStreamSynchronize(c->stream));
+            c->motion_mem.clear(); c->prev_pos = nullptr; c->object_motion = 0;
+            return RT_OK;
+        }
+        c->object_motion = 1;
+        return c->scene_ready ? set_prev_positions(c) : RT_OK;
     case RT_OPT_SAMPLER:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "sampler type must be 0 (kRandom) or 1 (kBlueNoise)");
         if (value == 1 && !c->d_bn)

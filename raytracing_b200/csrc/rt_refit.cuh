@@ -19,14 +19,22 @@ __device__ __forceinline__ float refit_max(float a, float b) { return (a < b) ? 
 // Triangle first + i from src[i] (RtTriangle: 10 float4 = v1 {position, texcoord, normal}, v2, v3, mtlIndex + padding) into the
 // tris_ref, wtris and tri_shade records (build_layout / build_tri_shade).  Kept: the end-of-leaf flag word of wtris and the
 // material word of tri_shade (materials stay those of the upload; mtlIndex is never read).
+// MOTION (RT_OPT_OBJECT_MOTION): the triangle's tris_ref entry is copied to prev_pos before it is overwritten, so prev_pos holds
+// the positions of the call before; the instance without it is the code of the option off (prev_pos is not read).
+template <bool MOTION = false>
 __global__ void __launch_bounds__(256) k_refit_records(const float4* __restrict__ src, uint32_t first, uint32_t n, float4* tris_ref,
-                                                       float4* wtris, float4* tri_shade)
+                                                       float4* wtris, float4* tri_shade, float4* prev_pos)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float4* t = src + (size_t)i * 10;
     const float4 p1 = t[0], uv1 = t[1], n1 = t[2], p2 = t[3], uv2 = t[4], n2 = t[5], p3 = t[6], uv3 = t[7], n3 = t[8];
     const size_t g = (size_t)first + i;
+    if (MOTION)
+    {
+        const float4 q1 = tris_ref[g * 3 + 0], q2 = tris_ref[g * 3 + 1], q3 = tris_ref[g * 3 + 2];
+        prev_pos[g * 3 + 0] = q1; prev_pos[g * 3 + 1] = q2; prev_pos[g * 3 + 2] = q3;
+    }
     tris_ref[g * 3 + 0] = p1; tris_ref[g * 3 + 1] = p2; tris_ref[g * 3 + 2] = p3;   // RtRTTriangle, the .w words included
     const float e1x = p2.x - p1.x, e1y = p2.y - p1.y, e1z = p2.z - p1.z;
     const float e2x = p3.x - p1.x, e2y = p3.y - p1.y, e2z = p3.z - p1.z;

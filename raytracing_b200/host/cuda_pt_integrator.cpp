@@ -140,6 +140,11 @@ void CUDAPathTraceIntegrator::SetEmitterSampling(bool on)
     Check(rt_set_option(ctx_, RT_OPT_EMITTER_SAMPLING, on ? 1u : 0u), "SetEmitterSampling");
 }
 
+void CUDAPathTraceIntegrator::SetObjectMotion(bool on)
+{
+    Check(rt_set_option(ctx_, RT_OPT_OBJECT_MOTION, on ? 1u : 0u), "SetObjectMotion");
+}
+
 void CUDAPathTraceIntegrator::SetEnvironmentSampling(bool on)
 {
     Check(rt_set_option(ctx_, RT_OPT_ENV_SAMPLING, on ? 1u : 0u), "SetEnvironmentSampling");

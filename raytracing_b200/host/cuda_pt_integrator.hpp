@@ -28,6 +28,7 @@
  * SetSpatialDenoiser(iterations, sigmas): ResolveRadiance() filters the shaded colour (include/rt_b200.h states the rule).
  * SetEmitterSampling(on): next-event estimation on the emissive triangles as well, combined with BSDF sampling by MIS
  * (RT_OPT_EMITTER_SAMPLING; the image converges to the same expectation, so the accumulation is kept).
+ * SetObjectMotion(on): motion vectors that follow UpdateTriangles as well as the camera (RT_OPT_OBJECT_MOTION).
  * SetEnvironmentSampling(on): the same for the environment map (RT_OPT_ENV_SAMPLING); SetLightSelection(a, e, v): relative weights of
  * the light kind drawn at each vertex (rt_set_light_selection).  Neither resets the accumulation.
  * AOVs (ComputeAOVs) are produced inside the bounce-0 shading pass, and only when SetAOV selected a view other than
@@ -91,6 +92,9 @@ public:
     // emitter sampling (RT_OPT_EMITTER_SAMPLING): sample the emissive triangles at every hit too, with MIS.  No reset: the estimator has
     // the same expectation, so it applies from the next frame and keeps the accumulation.
     void SetEmitterSampling(bool on);
+    // object motion (RT_OPT_OBJECT_MOTION): the motion-vector AOV (view 4, the temporal denoiser's reprojection) follows
+    // UpdateTriangles as well as the camera.  Changes no image until the next UpdateTriangles.
+    void SetObjectMotion(bool on);
     // environment sampling (RT_OPT_ENV_SAMPLING): sample the environment map at every hit too, with MIS.  No reset, as above.
     void SetEnvironmentSampling(bool on);
     // light-kind weights (rt_set_light_selection): analytic, emitters, environment, each finite and > 0.  No reset, as above.

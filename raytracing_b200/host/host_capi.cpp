@@ -195,6 +195,10 @@ int rth_render_set_emitter_sampling(void* h, int on)
 {
     try { ((RenderHandle*)h)->render->SetEmitterSampling(on != 0); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_object_motion(void* h, int on)
+{
+    try { ((RenderHandle*)h)->render->SetObjectMotion(on != 0); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_set_environment_sampling(void* h, int on)
 {
     try { ((RenderHandle*)h)->render->SetEnvironmentSampling(on != 0); return 0; } catch (std::exception& e) { g_error = e.what(); return -1; }

@@ -50,6 +50,8 @@ public:
     }
     // emitter sampling (CUDAPathTraceIntegrator::SetEmitterSampling): applies from the next RenderFrame(), keeps the accumulation
     void SetEmitterSampling(bool on) { Cuda().SetEmitterSampling(on); }
+    // object motion vectors (CUDAPathTraceIntegrator::SetObjectMotion): AOV view 4 and the temporal denoiser follow UpdateTriangles
+    void SetObjectMotion(bool on) { Cuda().SetObjectMotion(on); }
     // environment sampling and light-kind weights (CUDAPathTraceIntegrator): apply from the next RenderFrame(), keep the accumulation
     void SetEnvironmentSampling(bool on) { Cuda().SetEnvironmentSampling(on); }
     void SetLightSelection(float analytic, float emitters, float environment) { Cuda().SetLightSelection(analytic, emitters, environment); }

@@ -47,6 +47,7 @@ def load_library():
     L.rth_render_set_spatial_denoiser.argtypes = [C.c_void_p, C.c_uint32, C.c_float, C.c_float, C.c_float]
     L.rth_render_set_emitter_sampling.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_environment_sampling.argtypes = [C.c_void_p, C.c_int]
+    L.rth_render_set_object_motion.argtypes = [C.c_void_p, C.c_int]
     L.rth_render_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
     L.rth_render_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.rth_render_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
@@ -231,6 +232,11 @@ class HostRender:
     def set_emitter_sampling(self, on):
         """Render::SetEmitterSampling: next-event estimation on the emissive triangles too (MIS); applies from the next render_frame()."""
         if self.L.rth_render_set_emitter_sampling(self.h, int(bool(on))) != 0:
+            raise _err(self.L)
+
+    def set_object_motion(self, on):
+        """Render::SetObjectMotion: motion vectors (AOV view 4, the temporal denoiser) follow update_triangles as well as the camera."""
+        if self.L.rth_render_set_object_motion(self.h, int(bool(on))) != 0:
             raise _err(self.L)
 
     def set_environment_sampling(self, on):

@@ -12,6 +12,11 @@ same geometry; and, for per-vertex noise of growing amplitude, the median device
 events on the render stream, 3 runs) after a refit against a context that rebuilt and uploaded the deformed scene.  Prints one JSON line per measurement, headed by
 the GPU's name and power limit read in the same run.
 
+  python tools/refit_probe.py --motion [--scenes ...]
+
+Object motion vectors (RT_OPT_OBJECT_MOTION) off against on, alternated twice on one context: the median host and device update
+as above, and the median device time of a frame with AOV view 4 (the velocity AOV computed every frame) after an update.
+
   python tools/refit_probe.py --rebuild [--scenes ...] [--rigid 0.05,0.2] [--amplitudes 0.01,0.02,0.05,0.2,1.0]
 
 The device rebuilds instead (rt_rebuild_bvh "linear" and rt_rebuild_bvh_ploc "ploc", --methods), each in a context of its own:
@@ -137,6 +142,29 @@ def rebuild_arm(a, name, sc, cam, emit):
         c.destroy()
 
 
+def motion_arm(a, name, sc, cam, emit):
+    """RT_OPT_OBJECT_MOTION off against on, alternated twice on one context: the host and device update (update_ms) and the frame
+    time with AOV view 4 (the velocity AOV produced every frame) after an update."""
+    import torch
+    n = len(sc["triangles"])
+    t = deform(sc["triangles"], "rigid", seed=1, amount=0.02)
+    d = torch.from_numpy(t.view(np.uint8).reshape(n, 160).copy()).cuda()
+    torch.cuda.synchronize()
+    c = capi.Context(a.width, a.height)
+    c.upload_scene(sc); c.set_camera(cam); c.set_camera(cam)
+    c.set_option(capi.OPT_AOV, 4)
+    c.update_triangles(t); c.sync()                          # builds the refit map
+    for rep in range(2):
+        for motion in (0, 1):
+            c.set_option(capi.OPT_OBJECT_MOTION, motion)
+            host, host_k = update_ms(c, t)
+            dev, dev_k = update_ms(c, d)
+            emit({"scene": name, "triangles": n, "object_motion": motion, "rep": rep, "update_host_ms": host,
+                  "update_host_kernels_ms": host_k, "update_device_ms": dev, "update_device_kernels_ms": dev_k,
+                  "frame_ms_aov4": frame_ms(c, a.bounces), "prev_positions_bytes": n * 48 if motion else 0})
+    c.destroy()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scenes", default="CornellBox_Dragon,Synthetic10M")
@@ -146,6 +174,7 @@ def main():
     ap.add_argument("--amplitudes", default="0.01,0.05,0.2,1.0")
     ap.add_argument("--out", default=None)
     ap.add_argument("--rebuild", action="store_true", help="measure rt_rebuild_bvh instead of rt_update_triangles")
+    ap.add_argument("--motion", action="store_true", help="measure updates and AOV frames with RT_OPT_OBJECT_MOTION off and on")
     ap.add_argument("--rigid", default="0.05,0.2", help="--rebuild: amplitudes of the rigid moves (empty: none)")
     ap.add_argument("--methods", default="linear,ploc", help="--rebuild: the device builds to measure (rt_rebuild_bvh, rt_rebuild_bvh_ploc)")
     a = ap.parse_args()
@@ -163,6 +192,9 @@ def main():
         sc, cam = load(name, a.width, a.height)
         if a.rebuild:
             rebuild_arm(a, name, sc, cam, emit)
+            continue
+        if a.motion:
+            motion_arm(a, name, sc, cam, emit)
             continue
         n = len(sc["triangles"])
         t = deform(sc["triangles"], "noise", seed=1, amount=0.01)
