@@ -29,9 +29,17 @@ __host__ __device__ __forceinline__ const uint32_t* in_count_ptr(const DevCounte
     return bounce == 0 ? &c->n_primary : &c->emit[bounce - 1].next;
 }
 
+// The two buffers of one plane of the extension-ray queue, by bounce parity.  Read through a select, not an array index: a kernel
+// parameter indexed by a run-time value is first copied to the thread's stack, which every thread of every launch then writes.
+struct PlanePair
+{
+    float4* p[2];
+    __host__ __device__ __forceinline__ float4* operator[](int i) const { return i ? p[1] : p[0]; }
+};
+
 struct Queues
 {
-    float4* A[2]; float4* B[2]; float4* C[2];
+    PlanePair A, B, C;
     float4* sA; float4* sB; float4* sC;
     float4* hits;
     uint32_t* shadow_flags;

@@ -64,6 +64,12 @@ using namespace rt;
 #define RT_SHADE_BATCH 1024
 #endif
 #define RT_SORT_BINS 64
+// Probe-only builds (tools/shade_probe.py, through tools/build_variant.py); their results are not the renderer's.
+// RT_SHADE_PROBE 1: memory floor, shade_hit makes its table reads and spawns both rays but does no shading arithmetic (every
+// schedule); 2: math floor, each warp of k_shade_queues<false> shades its first hit group's entries again for every hit group it takes.
+#ifndef RT_SHADE_PROBE
+#define RT_SHADE_PROBE 0
+#endif
 // The whole-frame kernel (k_frame) is compiled for up to 1024 threads per CTA (64 registers): the CTA size is chosen at launch
 // (RT_OPT_FRAME_THREADS) — 1024 threads = one CTA per SM, all 32 warps of an SM in the same phase; 256 threads = 4 CTAs per SM
 // in different phases
@@ -110,6 +116,28 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
                                           f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
                                           uint32_t sample_offset, ShadeOut& out)
 {
+#if RT_SHADE_PROBE == 1
+    {   // memory floor: the shading record, material and blue-noise reads of the hit, each value used by a few adds, and a shadow
+        // ray and a continuation ray (back along the incoming ray) for every hit
+        const float4* tq = sc.tri_shade + (size_t)prim * 7;
+        const float4 q0 = __ldg(tq), q1 = __ldg(tq + 1), q2 = __ldg(tq + 2), q3 = __ldg(tq + 3), q4 = __ldg(tq + 4), q5 = __ldg(tq + 5);
+        const float4* mr = sc.mat_rec + (size_t)__float_as_uint(q0.w) * 4;
+        const float4 m0 = __ldg(mr), m2 = __ldg(mr + 2);
+        float s = 0.0f;
+        if (p.bn)
+            for (uint32_t d = 0; d < 5; ++d)
+                s += sample_blue_noise(p.bn, pxy & 0xFFFFu, pxy >> 16, p.dyn->sample_idx + sample_offset, bounce * 5u + d);
+        const float w0 = 1.0f - u - v;
+        const f3 position = mk3(q0) * w0 + mk3(q1) * u + mk3(q2) * v;
+        out.emissive = false;
+        out.spawn_shadow = out.spawn_next = true;
+        out.s_origin = position; out.s_dir = mk3(q3) + mk3(q4) + mk3(q5) + mk3(q1.w, q2.w, q3.w); out.s_tmax = s + m2.x;
+        out.s_sample = hit_throughput * mk3(m0);
+        out.n_origin = position; out.n_dir = -ray_dir; out.n_throughput = hit_throughput * mk3(m0); out.n_pdf = prev_pdf + q4.w + q5.w;
+        (void)ray_origin; (void)aov;
+        return;
+    }
+#endif
     f3 incoming = -ray_dir;
     uint32_t px = pxy & 0xFFFFu, py = pxy >> 16;
     const float4* tp = sc.tri_shade + (size_t)prim * 7;
@@ -672,10 +700,12 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
     if (!SORT)
     {
         const int lane = threadIdx.x & 31;
+        uint32_t first = ~0u;                                   // RT_SHADE_PROBE 2 only
         for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < total;)
         {
             if (at < hit_span)
             {
+                if (RT_SHADE_PROBE == 2) { if (first == ~0u) first = at; at = first; }
                 const uint32_t k = at + lane;
                 const bool hit = k < n_hit;
                 float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -1397,7 +1427,7 @@ int alloc_frame_buffers(rt_ctx* c)
     float4 *radiance = nullptr, *resolved = nullptr;
     cudaError_t e = cudaSuccess;
     auto get = [&](auto*& view) { if (e == cudaSuccess) e = g.alloc(view, n); };
-    for (int i = 0; i < 2; ++i) { get(q.A[i]); get(q.B[i]); get(q.C[i]); }
+    for (int i = 0; i < 2; ++i) { get(q.A.p[i]); get(q.B.p[i]); get(q.C.p[i]); }
     get(q.sA); get(q.sB); get(q.sC); get(q.hits); get(q.shadow_flags); get(q.hitq); get(q.missq); get(radiance); get(resolved);
     if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "allocating the frame buffers failed: %s", cudaGetErrorString(e));
     c->frame_mem = std::move(g); c->q = q; c->radiance = radiance; c->resolved = resolved;
