@@ -50,7 +50,8 @@ typedef struct RtSceneDesc {
     const RtLinearBVHNode* nodes;       uint64_t n_nodes;          /* >= 1 */
     const RtPackedMaterial* materials;  uint64_t n_materials;      /* >= 1 */
     const RtLight* lights;              uint64_t n_lights;         /* >= 1 (light.h:46 divides by the count) */
-    const RtTexture* textures;          uint64_t n_textures;
+    const RtTexture* textures;          uint64_t n_textures;       /* each RtTexture: data_start + width * height <= 2^31 (texels
+                                                                      are indexed in int); rt_upload_scene refuses any other */
     const uint32_t* texture_data;       uint64_t n_texture_data;
     const uint32_t* emissive_indices;   uint64_t n_emissive;       /* triangle ids; sampled only with RT_OPT_EMITTER_SAMPLING 1 */
     const float* env_image;             uint32_t env_width, env_height;   /* RGBA32F rows, first row = v 0 */

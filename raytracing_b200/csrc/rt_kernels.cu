@@ -1819,6 +1819,9 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
         const RtTexture& t = s->textures[i];
         if (t.width <= 0 || t.height <= 0 || t.data_start < 0 || (uint64_t)t.data_start + (uint64_t)t.width * t.height > s->n_texture_data)
             RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: texture %llu lies outside the texel array", (unsigned long long)i);
+        // sample_texture (rt_device.cuh) and material.h:259 index texels in int: the last texel must lie below 2^31
+        if ((uint64_t)t.data_start + (uint64_t)t.width * t.height > 0x80000000ull)
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: texture %llu ends beyond texel 2^31 - 1", (unsigned long long)i);
     }
     if (c->emitter_sampling)
     {
