@@ -14,6 +14,7 @@ from raytracing_b200.camera import default_camera
 from tests.helpers import bits, scene
 from tests.scenes_extra import closed_cornell, many_lights_scene, single_leaf_scene, textured_cornell
 from tests.test_gpu_parity import run_frame, schedule_ctx
+from tests.trace_cases import axis_camera
 
 pytestmark = pytest.mark.gpu
 
@@ -88,14 +89,6 @@ def test_both_sides_of_the_size_limit():
     cam = scene("ShaderBalls").get("camera_pose", default_camera(W, H))
     for n, mode in ((under, 3), (over, 1)):
         assert_on_equals_off(subset_scene(n), cam, W, H, 3, ("subset", n), runs=("frame", "phase_graph"), mode_on=mode)
-
-
-def axis_camera(w, h, position, front, up):
-    """A camera whose every primary ray is exactly `front`: fov 0 and no aperture, axes filled in by hand (default_camera goes
-    through float32 sin/cos of pi/2 and never gives an exact axis)."""
-    cam = default_camera(w, h)
-    cam["position"][:3] = position; cam["front"][:3] = front; cam["up"][:3] = up; cam["fov"] = 0.0
-    return cam
 
 
 @pytest.mark.parametrize("view", ["+y", "+x", "-z"])
