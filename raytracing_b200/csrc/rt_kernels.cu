@@ -1489,9 +1489,9 @@ cudaError_t launch_chain(rt_ctx* c, void (*kernel)(KArgs...), int grid, size_t s
 // How a traversal kernel stages the BVH (TMA bulk copies into dynamic shared memory), decided per launch:
 //   mode 1  the whole structure (interior records + triangle records) when it fits 40 KB (5 resident CTAs x 40 KB stay under
 //           the 227 KB of an SM);
-//   mode 3  mode 1 plus the eight octant-ordered copies of the interior records that every CTA builds from the staged ones
-//           (rt_octant.h) and a flag word, when all of it fits the same 40 KB (RT_OPT_OCTANT_BVH, default on): CornellBox,
-//           2.6 KB + 8.7 KB;
+//   mode 3  mode 1 plus the eight 4-wide octant tables that every CTA builds from the staged records (rt_octant.h; each at
+//           most the 64 bytes per record reserved here) and a flag word, when all of it fits the same 40 KB
+//           (RT_OPT_OCTANT_BVH, default on): CornellBox, 2.6 KB + 8.7 KB;
 //   mode 2  only the top of the tree — the first top_k interior records in breadth-first order (RT_OPT_TOP_SMEM records,
 //           default 0 = off, DESIGN.md section 4 says why) — when the structure does not fit;
 //   mode 0  nothing staged: literal traversal (RT_OPT_TRAVERSAL 0), RT_OPT_SMEM_BVH off.

@@ -92,6 +92,77 @@ RT_OCT_FN void rt_oct_order(const float* rec, uint32_t s, float* out)
     out[12] = rec[12 + swap]; out[13] = rec[13 - swap]; out[14] = rec[14]; out[15] = rec[15];
 }
 
+/*
+ * 4-WIDE OCTANT TABLES.  The binary tree is collapsed as tools/wide_bvh_model.cpp does: the wide nodes are the interior records
+ * at even depth (the root is depth 0), and each takes its children, except that an interior child is replaced by that child's
+ * two children — 2..4 children per wide node.  In the table of octant s a wide node is a run of consecutive 32-byte slots in
+ * the order the binary traversal visits them for a ray of that octant: near child (or, when it is interior, its near and far
+ * child), then far child (likewise).  A slot is
+ *   [0..2] entry planes   [3..5] exit planes   [6] child ref   [7] the node's child count (2..4), in every slot of the node
+ * with the planes ordered as rt_oct_order orders them, child ref < 0 a leaf (first triangle ~ref) and >= 0 the first slot of
+ * a wide node.  The slot numbering is the same in every octant: wide nodes in record order, each taking rt_wide_count slots,
+ * so every octant's table holds at most twice as many slots as there are records (every binary node but the root takes at
+ * most one slot) — the 64 bytes per record of a binary ordered table.  The builder keeps, in word 15 of each record (which no
+ * traversal reads), the record's first slot, or 0xFFFFFFFF for a record that is not a wide node.
+ *
+ * Testing the children of a collapsed child without testing that child's box takes the same decisions as the binary
+ * traversal only when the child's box contains both boxes of its own children (then, under monotone rounding, its slab
+ * interval contains theirs): rt_wide_nests is that guard.
+ */
+RT_OCT_FN uint32_t rt_oct_u(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+RT_OCT_FN float rt_oct_f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
+
+// Slots of the wide node at a record: 1 per leaf child, 2 per interior child.
+RT_OCT_FN uint32_t rt_wide_count(const float* rec) { return ((int)rt_oct_u(rec[12]) < 0 ? 1u : 2u) + ((int)rt_oct_u(rec[13]) < 0 ? 1u : 2u); }
+
+// The nesting guard of the wide node at record `rec` of the n records `recs`: every interior child's box contains both
+// boxes of that child's own record on every axis (false for a reference out of range and for a NaN plane).
+RT_OCT_FN bool rt_wide_nests(const float* rec, const float* recs, uint32_t n)
+{
+    bool ok = true;
+    for (int c = 0; c < 2; ++c)
+    {
+        const int ref = (int)rt_oct_u(rec[12 + c]);
+        if (ref < 0) continue;
+        if ((uint32_t)ref >= n) return false;
+        const float* box = rec + 6 * c;
+        const float* kid = recs + 16 * (uint32_t)ref;
+        for (int g = 0; g < 2; ++g)
+            for (int k = 0; k < 3; ++k)
+                ok = ok && kid[6 * g + k] >= box[k] && kid[6 * g + 3 + k] <= box[3 + k];
+    }
+    return ok;
+}
+
+// The slots of the wide node at record r for octant s, written to out (8 floats per slot).  Every record passed
+// rt_oct_record_ok, every child reference is in range and word 15 of every record holds its first slot.
+RT_OCT_FN void rt_wide_node(const float* recs, uint32_t r, uint32_t s, float* out)
+{
+    const float cnt = rt_oct_f(rt_wide_count(recs + 16 * r));
+    float ord[16];
+    rt_oct_order(recs + 16 * r, s, ord);
+    uint32_t k = 0;
+    for (int c = 0; c < 2; ++c)
+    {
+        const int ref = (int)rt_oct_u(ord[12 + c]);
+        if (ref < 0)
+        {
+            for (int j = 0; j < 6; ++j) out[8 * k + j] = ord[6 * c + j];
+            out[8 * k + 6] = ord[12 + c]; out[8 * k + 7] = cnt; ++k;
+            continue;
+        }
+        float kid[16];
+        rt_oct_order(recs + 16 * (uint32_t)ref, s, kid);
+        for (int g = 0; g < 2; ++g)
+        {
+            const int gref = (int)rt_oct_u(kid[12 + g]);
+            for (int j = 0; j < 6; ++j) out[8 * k + j] = kid[6 * g + j];
+            out[8 * k + 6] = gref < 0 ? kid[12 + g] : recs[16 * (uint32_t)gref + 15];
+            out[8 * k + 7] = cnt; ++k;
+        }
+    }
+}
+
 // One child's slab interval, pairwise (trace_fast on canonical records): box = min xyz, max xyz.
 RT_OCT_FN void rt_slab_pairwise(const float* box, float ox, float oy, float oz, float ix, float iy, float iz, float t_min, float& lo, float& hi)
 {

@@ -50,16 +50,66 @@ __device__ __forceinline__ void stage_bvh(float4* dst, const DevScene& sc, uint6
         asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
                      : "=r"(done) : "r"(bar), "r"(0) : "memory");
     if (SMEM == 3)
-    {   // every thread has seen the copies complete; each reorders a few of the records it can now read
+    {   // every thread has seen the copies complete: build the 4-wide octant tables (rt_octant.h) from the staged records
         const uint32_t n = sc.root_ref < 0 ? 0u : sc.wnodes_f4 / 4u;      // a root-leaf tree has no interior record to visit
+        float* recs = (float*)dst;
         float4* oct = dst + sc.wnodes_f4 + sc.wtris_f4;
+        uint32_t* flag = (uint32_t*)(oct + 8u * sc.wnodes_f4);
+        // Which records are wide nodes (even depth): parent links, then pointer jumping over the depth parity.  Scratch in the
+        // table area, which is written only after the numbering: word = (ancestor + 1) << 1 | parity of the distance to it.
+        uint32_t *link = (uint32_t*)oct, *next = link + n;
+        for (uint32_t r = threadIdx.x; r < n; r += blockDim.x) link[r] = 0u;
+        __syncthreads();
         bool ok = true;
-        for (uint32_t r = threadIdx.x; r < n; r += blockDim.x) ok = ok && rt_oct_record_ok((const float*)(dst + r * 4u));
+        for (uint32_t r = threadIdx.x; r < n; r += blockDim.x)
+            for (int c = 0; c < 2; ++c)
+            {
+                const int ref = __float_as_int(recs[16u * r + 12u + c]);
+                if (ref >= 0) { if ((uint32_t)ref < n) link[ref] = ((r + 1u) << 1) | 1u; else ok = false; }
+            }
+        __syncthreads();
+        for (int round = 0; round < 6; ++round)                          // 2^6 levels: trees are at most 64 deep (build_layout)
+        {
+            bool more = false;
+            for (uint32_t r = threadIdx.x; r < n; r += blockDim.x)
+            {
+                const uint32_t w = link[r];
+                const uint32_t up = (w >> 1) ? link[(w >> 1) - 1u] : 0u;
+                next[r] = (w >> 1) ? ((up & ~1u) | ((w ^ up) & 1u)) : w;
+                more = more || (up >> 1) != 0u;
+            }
+            uint32_t* t = link; link = next; next = t;
+            if (!__syncthreads_or(more)) break;                           // every record has reached the root
+        }
+        // first slots: a prefix sum over the wide records in record order, by the first warp; kept in word 15 of each record
+        if (threadIdx.x < 32u)
+        {
+            uint32_t base = 0;
+            for (uint32_t r0 = 0; r0 < n; r0 += 32u)
+            {
+                const uint32_t r = r0 + threadIdx.x;
+                const uint32_t w = r < n ? link[r] : 1u;
+                const uint32_t cnt = (w & 1u) ? 0u : rt_wide_count(recs + 16u * r);
+                uint32_t incl = cnt;
+                for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)threadIdx.x >= d) incl += v; }
+                if (r < n) recs[16u * r + 15u] = __uint_as_float(cnt ? base + incl - cnt : 0xFFFFFFFFu);
+                ok = ok && !(w >> 1);                                    // every record reached the root (no cycle, not too deep)
+                base += __shfl_sync(0xFFFFFFFFu, incl, 31);
+            }
+            ok = ok && base <= 2u * n;                                   // the tables' room (a tree takes at most 2n slots)
+        }
         ok = __syncthreads_and(ok) != 0;
         if (ok)
             for (uint32_t i = threadIdx.x; i < 8u * n; i += blockDim.x)
-                rt_oct_order((const float*)(dst + (i % n) * 4u), i / n, (float*)(oct + i * 4u));
-        if (threadIdx.x == 0) *(uint32_t*)(oct + 8u * sc.wnodes_f4) = ok ? 1u : 0u;
+            {
+                const uint32_t r = i % n, s = i / n, slot = __float_as_uint(recs[16u * r + 15u]);
+                if (s == 0u) ok = ok && rt_oct_record_ok(recs + 16u * r);
+                if (slot == 0xFFFFFFFFu) continue;
+                if (s == 0u) ok = ok && rt_wide_nests(recs + 16u * r, recs, n);
+                rt_wide_node(recs, r, s, (float*)(oct + s * sc.wnodes_f4) + 8u * slot);
+            }
+        ok = __syncthreads_and(ok) != 0;
+        if (threadIdx.x == 0) *flag = ok ? 1u : 0u;
         __syncthreads();
     }
 }
@@ -154,11 +204,14 @@ __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d
 // still match) take the literal path.
 // PIN: the whole-frame kernel shares its register budget with the shading code and ptxas then re-derives the sign bits on
 // every step and recomputes the determinant after its branch; an empty asm makes both values opaque (kept in registers).
-// SMEM 3: `wnodes` and `wtris` are those of SMEM 1 and the octant tables follow the triangles (stage_bvh).  The interior step
-// reads the record of the ray's octant and runs the ordered slab test, which takes the same decisions as the pairwise one for a
-// ray that passes rt_oct_ray_ok on records that passed rt_oct_record_ok (rt_octant.h has the argument).  Any other ray, and
-// every ray of a CTA whose records failed, is traced by the SMEM 1 traversal on the canonical staged records (a loop of its
-// own: a branch inside the ordered loop was measured and cost half the gain):
+// SMEM 3: `wnodes` and `wtris` are those of SMEM 1 and the 4-wide octant tables follow the triangles (stage_bvh).  The interior
+// step reads the wide node from the table of the ray's octant, slab-tests its 2..4 children in the order the binary traversal
+// visits them, continues into the first that hits and defers the others with their entry distances: the visits, hits and
+// results of the binary traversal in about half the steps (tools/wide_bvh_model.cpp).  The ordered slab test takes the same
+// decisions as the pairwise one for a ray that passes rt_oct_ray_ok on records that passed rt_oct_record_ok (rt_octant.h has
+// the argument), and skipping a collapsed child's own box test is exact where rt_wide_nests holds.  Any other ray, and every
+// ray of a CTA whose records failed, is traced by the SMEM 1 traversal on the canonical staged records (a loop of its own: a
+// branch inside the ordered loop was measured and cost half the gain):
 // exactly what RT_OPT_OCTANT_BVH 0 computes, also where that differs from the literal traversal (a NaN t_max from a triangle
 // with an infinite vertex ends the staged traversal and not the literal one).
 template <bool ANY, bool COUNT, int SMEM, bool PIN = false>
@@ -171,7 +224,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
         return trace_literal<ANY, COUNT>(sc, o, d, t_min, t_max, bu, bv, bt, nv, nt);
 
     f3 inv = splat(1.0f) / d;
-    if (OCT && !(rt_oct_ray_ok(inv.x, inv.y, inv.z) && *(const uint32_t*)(wtris + sc.wtris_f4 + 8u * sc.wnodes_f4) != 0u))
+    if (OCT && !(rt_oct_ray_ok(inv.x, inv.y, inv.z) && (!ANY || t_max == t_max) && *(const uint32_t*)(wtris + sc.wtris_f4 + 8u * sc.wnodes_f4) != 0u))
         return trace_fast<ANY, COUNT, OCT ? 1 : SMEM, PIN>(sc, wnodes, wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt);
     const bool sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
     uint32_t sign_bits = (sx ? 1u : 0u) | (sy ? 2u : 0u) | (sz ? 4u : 0u);
@@ -183,7 +236,12 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
     // (measured, same results): with the records in shared memory the kernel is purely issue-bound and the packed
     // 64-bit stack entry + the sign-bit axis test win (CornellBox frame -2.7 %); with the records behind L1/L2 the two
     // 32-bit arrays (a discarded pop costs one load) and predicate selects are faster (ShaderBalls +1 %, Dragon +3.5 %).
-    int2 stack[PACKED ? 64 : 1];
+    // A wide step can defer up to three children where the binary one defers one, so SMEM 3 has twice the 64 binary entries.
+    int2 stack[OCT && !ANY ? 128 : PACKED && !OCT ? 64 : 1];
+    // An any-hit ray returns at its first hit, so its t_max never shrinks and every deferred child passes the pop test (its entry
+    // distance was at most t_max when it was pushed): SMEM 3 keeps only the references.  A NaN t_max, which the pop test would
+    // reject, takes the SMEM 1 loop (the guard above).
+    int any_stack[OCT && ANY ? 128 : 1];
     int stack_ref[PACKED ? 1 : 64];
     float stack_t[PACKED ? 1 : 64];
     // the records of this ray's octant, as an offset from the canonical ones; opaque, so that it stays in a register instead of
@@ -210,22 +268,48 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
     {
         while (cur >= 0)
         {
+            if (OCT)
+            {   // the wide node at slot `cur` of this ray's table: 2..4 slots of (entry xyz, exit | exit yz, ref, count), in visiting order
+                // The children are tested last to first: each hit defers the one found before it, so the first child that hits
+                // is continued into and the other hit children are deferred in reverse order, with no per-child state kept.
+                const float4* np = wnodes + (oct_at + (uint32_t)cur * 2u);
+                const uint32_t cnt = __float_as_uint(np[1].w);
+                bool found = false;
+                int next_ref = 0;
+                float next_lo = 0.0f;
+#pragma unroll
+                for (int j = 3; j >= 0; --j)
+                {
+                    if (j >= 2 && (uint32_t)j >= cnt) continue;
+                    const float4 p = np[2 * j], q = np[2 * j + 1];
+                    float lo, hi;
+                    rt_slab_ordered(p.x, p.y, p.z, p.w, q.x, q.y, o.x, o.y, o.z, inv.x, inv.y, inv.z, t_min, lo, hi);
+                    if (fminf(hi, t_max) >= lo)
+                    {
+                        if (found)
+                        {
+                            if (ANY) any_stack[sp] = next_ref; else stack[sp] = make_int2(next_ref, __float_as_int(next_lo));
+                            ++sp;
+                        }
+                        next_ref = __float_as_int(q.z); next_lo = lo; found = true;
+                    }
+                }
+                if (found) { cur = next_ref; continue; }
+                if (ANY) { if (sp == 0) return prim; cur = any_stack[--sp]; continue; }
+                while (sp > 0)
+                {
+                    --sp;
+                    int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; }
+                }
+                if (!found) return prim;
+                continue;
+            }
             // SMEM == 2: `wnodes` is the staged top of the tree (records [0, sc.top_k)), deeper records come from sc.wnodes
-            const float4* np = OCT ? wnodes + (oct_at + (uint32_t)cur * 4u)
-                             : (SMEM == 2 && (uint32_t)cur >= sc.top_k) ? sc.wnodes + (size_t)cur * 4 : wnodes + (size_t)cur * 4;
+            const float4* np = (SMEM == 2 && (uint32_t)cur >= sc.top_k) ? sc.wnodes + (size_t)cur * 4 : wnodes + (size_t)cur * 4;
             float4 a = ld_bvh<SMEM>(np), b = ld_bvh<SMEM>(np + 1), c = ld_bvh<SMEM>(np + 2), m = ld_bvh<SMEM>(np + 3);
             int near_ref, far_ref;
             bool near_hit, far_hit;
             float far_lo;
-            if (OCT)
-            {   // near child: entry (a.x,a.y,a.z) exit (a.w,b.x,b.y); far child: entry (b.z,b.w,c.x) exit (c.y,c.z,c.w)
-                float lo_n, hi_n, hi_f;
-                rt_slab_ordered(a.x, a.y, a.z, a.w, b.x, b.y, o.x, o.y, o.z, inv.x, inv.y, inv.z, t_min, lo_n, hi_n);
-                rt_slab_ordered(b.z, b.w, c.x, c.y, c.z, c.w, o.x, o.y, o.z, inv.x, inv.y, inv.z, t_min, far_lo, hi_f);
-                near_hit = fminf(hi_n, t_max) >= lo_n; far_hit = fminf(hi_f, t_max) >= far_lo;
-                near_ref = __float_as_int(m.x); far_ref = __float_as_int(m.y);
-            }
-            else
             {
                 // child 0 box: min (a.x,a.y,a.z) max (a.w,b.x,b.y); child 1 box: min (b.z,b.w,c.x) max (c.y,c.z,c.w)
 #ifdef RT_FMA_TRAVERSAL
@@ -316,6 +400,7 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
             if (last) break;
             ++ti;
         }
+        if (OCT && ANY) { if (sp == 0) return prim; cur = any_stack[--sp]; continue; }
         bool found = false;
         while (sp > 0)
                 {

@@ -1,4 +1,4 @@
-"""Same-card A/B of the octant-ordered BVH records (RT_OPT_OCTANT_BVH): 1920x1080 x 8 bounces, CornellBox (staged whole in shared
+"""Same-card A/B of the 4-wide octant tables (RT_OPT_OCTANT_BVH): 1920x1080 x 8 bounces, CornellBox (staged whole in shared
 memory: the scene the tables exist for) and ShaderBalls (traversed through L1/L2: the control that must not move).
 Arms: "parent" = a library built from the parent commit (a path, or a variant name of tools/build_variant.py; skipped when the
 file does not exist), "off" = the in-tree library with the option 0, "on" = the in-tree library with the option 1.  Schedules:
