@@ -534,6 +534,50 @@ int rt_rebuild_bvh(rt_ctx* ctx, uint64_t* n_nodes);
 #define RT_PLOC_RADIUS 16
 int rt_rebuild_bvh_ploc(rt_ctx* ctx, uint64_t* n_nodes);
 
+/* ---- instanced scenes (new capability): placed copies of shared meshes, traced through a two-level BVH ---------------------------
+ * The scene kind is decided by the upload call: rt_upload_scene makes a flat scene, rt_upload_instanced_scene an instanced one; each
+ * replaces whatever scene came before.  Nothing changes for flat scenes.
+ * Meshes: scene->triangles and scene->nodes are the concatenation of the meshes; mesh k owns triangles [first_triangle,
+ * first_triangle + n_triangles) in its own leaf order and nodes [first_node, first_node + n_nodes), a Bvh::BuildCPU array whose
+ * offsets are relative to the mesh's own arrays.  Every mesh gets the records rt_upload_scene would derive from it alone
+ * (rt_bvh_layout.h), concatenated.  Materials, textures, lights and the environment are shared.  emissive_indices is ignored.
+ * Every mesh range must lie inside the arrays and each mesh's root box must be finite (else RT_ERR_INVALID_ARGUMENT).
+ * Instances: rt_set_instances replaces the whole list (0 instances is legal: every ray misses).  RtInstance.object_to_world is M,
+ * row-major 3x4.  The context computes W = M^-1 in double and rounds it to float, and rejects the whole call with
+ * RT_ERR_INVALID_ARGUMENT (the previous list stays) if an instance's matrix is not finite or singular (det == 0 in double), its
+ * mesh index is out of range, or the virtual triangle ids reach RT_INVALID_ID.  A negative determinant (a mirror) is allowed.
+ * The top-level tree and the world boxes follow the rule of raytracing_b200/csrc/rt_instances.h.
+ * Virtual triangle ids: instance i covers [base_i, base_i + n_triangles(mesh_i)), base = the prefix sum in instance order, so
+ * RtHit.primitive_id, rt_read_hits and the statistics read as for the flattened scene.
+ * Traversal: the top-level tree with the slab test, near/far order and deferred-child stack of the flat traversal; at an instance
+ * the ray goes to object space, all float without contraction: o' = ((W0*o.x + W1*o.y) + W2*o.z) + W3 per row, d' = (W0*d.x + W1*d.y)
+ * + W2*d.z; d' is not renormalised, so t is the same parameter in both spaces, and the mesh's tree is traced with the shared
+ * t_max as a flat scene's (a later equal-t hit replaces the earlier, across instances too), except that the back-face test reads
+ * det * sign(det M): a mirrored instance culls the faces its flattened triangles would.  Any-hit rays stop at the first hit.
+ * Shading: the object-space position p as for flat scenes, then position = M * p (same row order as o'); the shading normal is
+ * normalize(W^T * n) with n the interpolated vertex normal, the geometric normal normalize(W^T * n_g) * sign(det M); texture
+ * coordinates, materials and emission are those of the mesh triangle.  With W = M = identity a frame equals that of the meshes
+ * uploaded flat, except where a signed zero or a NaN coordinate meets the matrix arithmetic (0 * x, -0 + 0).
+ * Object motion (RT_OPT_OBJECT_MOTION): the previous transform M_prev of instance index i is its transform in the last earlier
+ * rt_set_instances (since the upload) whose list had index i, or its current one if none had; the velocity AOV of a bounce-0 hit is
+ * project(M * p) - project(M_prev * p), both points from the same object-space p, all float as the shading position.
+ * Schedules: always the per-phase kernels (RT_OPT_FRAME_KERNEL has no effect), nothing staged (rt_bvh_staging reports mode 0;
+ * RT_OPT_SMEM_BVH, RT_OPT_TOP_SMEM, RT_OPT_OCTANT_BVH and RT_OPT_TRAVERSAL have no effect).  Overlap modes, graphs, PDL, kernel
+ * timing, traversal counting, the stepwise calls and rt_integrate_samples work.  Traversal counting counts each top-level box
+ * tested once (the root, and both children of every top-level interior node visited) plus the mesh nodes the flat count would.
+ * The sort-key origin of the shading pass (ray order only) is the top-level root box centre as of the last rt_set_instances that
+ * grew the instance buffer.
+ * Ordering: rt_set_instances is enqueued on the render stream like rt_update_triangles (a deferred shadow pass is launched first);
+ * a captured frame graph stays valid while the instance count does not exceed the buffer's capacity (it grows to at least twice
+ * its size when a list exceeds it).
+ * RT_ERR_UNSUPPORTED on an instanced scene: rt_update_triangles*, rt_rebuild_bvh, rt_rebuild_bvh_ploc, rt_read_bvh and
+ * RT_OPT_EMITTER_SAMPLING 1 (whichever call comes second).  RT_ERR_NOT_READY: rt_set_instances without an instanced scene.
+ * Multi-device contexts fan out both calls. */
+typedef struct RtMeshDesc { uint64_t first_triangle, n_triangles, first_node, n_nodes; } RtMeshDesc;
+typedef struct RtInstance { float object_to_world[12]; uint32_t mesh; uint32_t padding[3]; } RtInstance;
+int rt_upload_instanced_scene(rt_ctx* ctx, const RtSceneDesc* scene, const RtMeshDesc* meshes, uint32_t n_meshes);
+int rt_set_instances(rt_ctx* ctx, const RtInstance* instances, uint32_t n_instances);
+
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);
 /* Hits of the rays currently in the incoming queue of `bounce` after rt_intersect(bounce): n = live rays;

@@ -39,7 +39,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
            "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh",
-           "rt_rebuild_bvh", "rt_bvh_staging", "rt_rebuild_bvh_ploc"]
+           "rt_rebuild_bvh", "rt_bvh_staging", "rt_rebuild_bvh_ploc", "rt_upload_instanced_scene", "rt_set_instances"]
 
 
 class RtSceneDesc(C.Structure):
@@ -130,8 +130,41 @@ def load_library():
     L.rt_read_bvh.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     L.rt_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rt_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    L.rt_upload_instanced_scene.argtypes = [C.c_void_p, C.POINTER(RtSceneDesc), C.c_void_p, C.c_uint32]
+    L.rt_set_instances.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     _lib = L
     return L
+
+
+# RtInstance (include/rt_b200.h): row-major 3x4 object-to-world matrix, mesh index, padding
+INSTANCE_DT = np.dtype([("object_to_world", "<f4", (12,)), ("mesh", "<u4"), ("padding", "<u4", (3,))])
+
+
+def _scene_desc(scene: dict):
+    """-> (RtSceneDesc, the arrays it points into; keep them alive until the call returns)."""
+    a = {
+        "triangles": np.ascontiguousarray(scene["triangles"], dtype=TRIANGLE_DT),
+        "nodes": np.ascontiguousarray(scene["nodes"], dtype=NODE_DT),
+        "materials": np.ascontiguousarray(scene["materials"], dtype=MATERIAL_DT),
+        "lights": np.ascontiguousarray(scene["lights"], dtype=LIGHT_DT),
+        "textures": np.ascontiguousarray(scene["textures"], dtype=TEXTURE_DT),
+        "texels": np.ascontiguousarray(scene["texels"], dtype="<u4"),
+        "emissive": np.ascontiguousarray(scene["emissive"], dtype="<u4"),
+        "env": np.ascontiguousarray(scene["env"], dtype="<f4"),
+    }
+    d = RtSceneDesc()
+    d.triangles, d.n_triangles = a["triangles"].ctypes.data, a["triangles"].shape[0]
+    d.nodes, d.n_nodes = a["nodes"].ctypes.data, a["nodes"].shape[0]
+    d.materials, d.n_materials = a["materials"].ctypes.data, a["materials"].shape[0]
+    d.lights, d.n_lights = a["lights"].ctypes.data, a["lights"].shape[0]
+    d.textures, d.n_textures = (a["textures"].ctypes.data if a["textures"].size else None), a["textures"].shape[0]
+    d.texture_data, d.n_texture_data = (a["texels"].ctypes.data if a["texels"].size else None), a["texels"].shape[0]
+    d.emissive_indices, d.n_emissive = (a["emissive"].ctypes.data if a["emissive"].size else None), a["emissive"].shape[0]
+    d.env_image, d.env_width, d.env_height = a["env"].ctypes.data, int(scene["env_width"]), int(scene["env_height"])
+    info = np.ascontiguousarray(scene["scene_info"], dtype=SCENE_INFO_DT).view("<u4").ravel()
+    for i in range(4):
+        d.scene_info[i] = int(info[i])
+    return d, a
 
 
 class Context:
@@ -199,30 +232,36 @@ class Context:
 
     # ---- Integrator public interface
     def upload_scene(self, scene: dict):
-        a = {
-            "triangles": np.ascontiguousarray(scene["triangles"], dtype=TRIANGLE_DT),
-            "nodes": np.ascontiguousarray(scene["nodes"], dtype=NODE_DT),
-            "materials": np.ascontiguousarray(scene["materials"], dtype=MATERIAL_DT),
-            "lights": np.ascontiguousarray(scene["lights"], dtype=LIGHT_DT),
-            "textures": np.ascontiguousarray(scene["textures"], dtype=TEXTURE_DT),
-            "texels": np.ascontiguousarray(scene["texels"], dtype="<u4"),
-            "emissive": np.ascontiguousarray(scene["emissive"], dtype="<u4"),
-            "env": np.ascontiguousarray(scene["env"], dtype="<f4"),
-        }
-        d = RtSceneDesc()
-        d.triangles, d.n_triangles = a["triangles"].ctypes.data, a["triangles"].shape[0]
-        d.nodes, d.n_nodes = a["nodes"].ctypes.data, a["nodes"].shape[0]
-        d.materials, d.n_materials = a["materials"].ctypes.data, a["materials"].shape[0]
-        d.lights, d.n_lights = a["lights"].ctypes.data, a["lights"].shape[0]
-        d.textures, d.n_textures = (a["textures"].ctypes.data if a["textures"].size else None), a["textures"].shape[0]
-        d.texture_data, d.n_texture_data = (a["texels"].ctypes.data if a["texels"].size else None), a["texels"].shape[0]
-        d.emissive_indices, d.n_emissive = (a["emissive"].ctypes.data if a["emissive"].size else None), a["emissive"].shape[0]
-        d.env_image, d.env_width, d.env_height = a["env"].ctypes.data, int(scene["env_width"]), int(scene["env_height"])
-        info = np.ascontiguousarray(scene["scene_info"], dtype=SCENE_INFO_DT).view("<u4").ravel()
-        for i in range(4):
-            d.scene_info[i] = int(info[i])
+        d, a = _scene_desc(scene)
         self._ck(self.lib.rt_upload_scene(self.h, C.byref(d)))
         self._n_nodes = a["nodes"].shape[0]
+
+    def upload_instanced_scene(self, meshes, shared: dict):
+        """An instanced scene (rt_upload_instanced_scene): meshes = a list of dicts with "triangles" (leaf order) and "nodes" (the
+        mesh's own Bvh::BuildCPU array, offsets relative to it), shared = a scene dict whose materials, lights, textures and
+        environment every mesh uses (its triangles and nodes are ignored).  Place the meshes with set_instances."""
+        tris = np.concatenate([np.ascontiguousarray(m["triangles"], dtype=TRIANGLE_DT) for m in meshes])
+        nodes = np.concatenate([np.ascontiguousarray(m["nodes"], dtype=NODE_DT) for m in meshes])
+        desc = np.zeros((len(meshes), 4), dtype="<u8")
+        t0 = n0 = 0
+        for k, m in enumerate(meshes):
+            nt, nn = len(m["triangles"]), len(m["nodes"])
+            desc[k] = (t0, nt, n0, nn)
+            t0 += nt; n0 += nn
+        d, a = _scene_desc(dict(shared, triangles=tris, nodes=nodes, emissive=np.zeros(0, "<u4")))
+        self._ck(self.lib.rt_upload_instanced_scene(self.h, C.byref(d), desc.ctypes.data, len(meshes)))
+
+    def set_instances(self, mesh_ids, transforms):
+        """Replace the instance list (rt_set_instances): instance i places mesh mesh_ids[i] by the row-major 3x4 object-to-world
+        matrix transforms[i] (shape (n, 3, 4))."""
+        ids = np.ascontiguousarray(mesh_ids, dtype="<u4").reshape(-1)
+        m = np.ascontiguousarray(transforms, dtype="<f4").reshape(-1, 12)
+        if len(ids) != len(m):
+            raise ValueError("set_instances: one mesh id per transform")
+        rec = np.zeros(len(ids), dtype=INSTANCE_DT)
+        rec["object_to_world"] = m
+        rec["mesh"] = ids
+        self._ck(self.lib.rt_set_instances(self.h, rec.ctypes.data if len(rec) else None, len(rec)))
 
     def set_camera(self, cam):
         c = np.ascontiguousarray(cam, dtype=CAMERA_DT)

@@ -42,6 +42,7 @@
 #include "rt_device.cuh"
 #include "rt_emitters.h"
 #include "rt_envmap.h"
+#include "rt_instances.h"
 #include "rt_refit.cuh"
 #include "rt_lbvh.cuh"
 #include "rt_ploc.cuh"
@@ -82,6 +83,18 @@ namespace
 #include "rt_traverse.cuh"
 
 // ------------------------------------------------------------------------------------ shading
+// Instanced scenes: a point through the 3x4 rows r (((r.x*p.x + r.y*p.y) + r.z*p.z) + r.w per row) and a normal through the
+// transpose of W's 3x3 part (rows w), all float in the order written
+__device__ __forceinline__ f3 xform_point(float4 r0, float4 r1, float4 r2, f3 p)
+{
+    return mk3(((r0.x * p.x + r0.y * p.y) + r0.z * p.z) + r0.w, ((r1.x * p.x + r1.y * p.y) + r1.z * p.z) + r1.w,
+               ((r2.x * p.x + r2.y * p.y) + r2.z * p.z) + r2.w);
+}
+__device__ __forceinline__ f3 xform_normal(float4 w0, float4 w1, float4 w2, f3 n)
+{
+    return mk3((w0.x * n.x + w1.x * n.y) + w2.x * n.z, (w0.y * n.x + w1.y * n.y) + w2.y * n.z, (w0.z * n.x + w1.z * n.y) + w2.z * n.z);
+}
+
 struct ShadeOut
 {
     bool spawn_shadow, spawn_next, emissive;
@@ -111,8 +124,11 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
 // prev_pdf: C.w of the ray (sampled lights: p_b of its direction at the previous vertex, 0 for primary rays and after a delta lobe).
 // EMIT: the scene has an active emitter table (sc.emit_*, RT_OPT_EMITTER_SAMPLING) or environment table (sc.env_*,
 // RT_OPT_ENV_SAMPLING), each read only while it exists; a template flag, so that the kernels without it are the code of both options off.
-template <bool EMIT = false>
-__device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
+// INST: an instanced scene (rt_b200.h): prim is a virtual id; the hit is shaded on its mesh triangle and moved to world space by the
+// instance's M (position) and W^T (normals); the AOV's previous position uses the instance's previous M (aov.prev_pos, 3 float4 per
+// instance) when object motion is on.
+template <bool EMIT = false, bool INST = false>
+__device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
                                           f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
                                           uint32_t sample_offset, ShadeOut& out)
 {
@@ -140,14 +156,38 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
 #endif
     f3 incoming = -ray_dir;
     uint32_t px = pxy & 0xFFFFu, py = pxy >> 16;
-    const float4* tp = sc.tri_shade + (size_t)prim * 7;
+    uint32_t tri = prim, inst = 0;
+    if constexpr (INST)
+    {   // the instance of the virtual id: the last base <= prim
+        uint32_t lo = 0, hi = __float_as_uint(__ldg(sc.inst_hdr + 1).w) - 1u;
+        while (lo < hi)
+        {
+            const uint32_t mid = (lo + hi + 1u) >> 1;
+            if (__ldg(sc.ibase + mid) <= prim) lo = mid; else hi = mid - 1u;
+        }
+        inst = lo;
+        const float4 mi = __ldg(sc.irec + (size_t)inst * 8 + 6);
+        tri = __float_as_uint(mi.z) + (prim - __float_as_uint(mi.w));
+    }
+    const float4* tp = sc.tri_shade + (size_t)tri * 7;
     float4 r0 = __ldg(tp), r1 = __ldg(tp + 1), r2 = __ldg(tp + 2), r3 = __ldg(tp + 3), r4 = __ldg(tp + 4), r5 = __ldg(tp + 5);
     f3 p1 = mk3(r0), p2 = mk3(r1), p3 = mk3(r2), n1 = mk3(r3), n2 = mk3(r4), n3 = mk3(r5);
     uint32_t mtl = __float_as_uint(r0.w);
     f3 geometry_normal = mk3(r1.w, r2.w, r3.w);       // normalize(cross(p2-p1, p3-p1)), precomputed at upload
     float w0 = 1.0f - u - v;
     f3 position = p1 * w0 + p2 * u + p3 * v;
-    f3 normal = normalize(n1 * w0 + n2 * u + n3 * v);
+    f3 normal;
+    f3 obj_position = position;
+    if constexpr (INST)
+    {   // world space: position = M * p; normals = normalize(W^T * n), the geometric one from the unnormalised cross product (the
+        // upload's normalize of it, when W is the identity) times sign(det M)
+        const float4* ir = sc.irec + (size_t)inst * 8;
+        const float4 wr0 = __ldg(ir), wr1 = __ldg(ir + 1), wr2 = __ldg(ir + 2);
+        position = xform_point(__ldg(ir + 3), __ldg(ir + 4), __ldg(ir + 5), obj_position);
+        normal = normalize(xform_normal(wr0, wr1, wr2, n1 * w0 + n2 * u + n3 * v));
+        geometry_normal = normalize(xform_normal(wr0, wr1, wr2, cross(p2 - p1, p3 - p1))) * __ldg(ir + 7).x;
+    }
+    else normal = normalize(n1 * w0 + n2 * u + n3 * v);
     f2 texcoord; texcoord.x = 0.0f; texcoord.y = 0.0f;
     if (__float_as_uint(__ldg(sc.mat_rec + (size_t)mtl * 4 + 3).y) != 0u)
     {   // texture coordinates are only needed by textured materials (hit_surface.cl:96-97)
@@ -164,9 +204,11 @@ __device__ __forceinline__ void shade_hit(const DevScene& sc, const FrameParams&
         aov.normal[li] = make_float4(normal.x, normal.y, normal.z, 0.0f);
         f3 prev = position;
         if (aov.prev_pos)
-        {   // object motion: the same barycentrics on the triangle's previous positions
-            const float4* qp = aov.prev_pos + (size_t)prim * 3;
-            prev = mk3(__ldg(qp)) * w0 + mk3(__ldg(qp + 1)) * u + mk3(__ldg(qp + 2)) * v;
+        {   // object motion: the same barycentrics on the triangle's previous positions (INST: the same object-space point under
+            // the instance's previous transform)
+            const float4* qp = aov.prev_pos + (size_t)(INST ? inst : prim) * 3;
+            if (INST) prev = xform_point(__ldg(qp), __ldg(qp + 1), __ldg(qp + 2), obj_position);
+            else prev = mk3(__ldg(qp)) * w0 + mk3(__ldg(qp + 1)) * u + mk3(__ldg(qp + 2)) * v;
         }
         f2 s0 = project_screen(position, p.dyn->cam), s1 = project_screen(prev, p.dyn->prev);
         aov.velocity[li] = make_float2(s0.x - s1.x, s0.y - s1.y);
@@ -344,8 +386,8 @@ __device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& 
 
 // Closest hit of the ray (a, b) of entry i (live lanes) and hit/miss stream compaction: __ballot + __popc give every lane its
 // slot, ONE 64-bit atomic per warp on `hm` reserves the slots of both queues (hits in the low word, misses in the high).
-template <bool COUNT, int SMEM, bool PIN>
-__device__ __forceinline__ void closest_group(const DevScene& sc, int mode, const float4* s_bvh, const Queues& q, uint32_t base, uint32_t i, bool live,
+template <bool COUNT, int SMEM, bool PIN, class Scene>
+__device__ __forceinline__ void closest_group(const Scene& sc, int mode, const float4* s_bvh, const Queues& q, uint32_t base, uint32_t i, bool live,
                                               float4 a, float4 b, unsigned long long* hm, uint32_t& nv, uint32_t& nt)
 {
     const int lane = threadIdx.x & 31;
@@ -369,8 +411,8 @@ __device__ __forceinline__ void closest_group(const DevScene& sc, int mode, cons
 
 // IntersectShadowRays + AccumulateDirectSamples (accumulate_direct_samples.cl:27-53) of shadow-queue entry i < n: any-hit trace,
 // the light sample of an unoccluded ray added to its pixel, the unoccluded rays counted on `n_unoccluded`
-template <bool COUNT, int SMEM, bool PIN>
-__device__ __forceinline__ void shadow_group(const FrameParams& p, const DevScene& sc, int mode, const float4* s_bvh, const Queues& q, uint32_t base,
+template <bool COUNT, int SMEM, bool PIN, class Scene>
+__device__ __forceinline__ void shadow_group(const FrameParams& p, const Scene& sc, int mode, const float4* s_bvh, const Queues& q, uint32_t base,
                                              uint32_t i, uint32_t n, float4* radiance, uint32_t* n_unoccluded, uint32_t& nv, uint32_t& nt)
 {
     bool un = false;
@@ -409,8 +451,8 @@ __device__ __forceinline__ uint32_t ray_key(f3 o, f3 d, float4 mid)
 // of both queues (shadow rays in the low word, continuation rays in the high).  With STAGE the continuation rays go to the CTA's
 // staging area `st` instead (flush_continuations writes them out and counts them) and the atomic reserves shadow-ray slots only.
 // Returns whether the lane's path ends at this hit (no continuation ray); `pixel` is the packed pixel of the ray.
-template <bool STAGE = false, bool EMIT = false>
-__device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevScene& sc, const AovParams& aov, const Queues& q, uint32_t base, uint32_t bounce,
+template <bool STAGE = false, bool EMIT = false, bool INST = false>
+__device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const SceneOf<INST>& sc, const AovParams& aov, const Queues& q, uint32_t base, uint32_t bounce,
                                                 bool hit, float4 h, uint32_t i, float4* radiance, unsigned long long* emit, uint32_t* n_emissive, uint32_t& pixel,
                                                 ContStage* st = nullptr)
 {
@@ -422,7 +464,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const DevS
     {
         const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
         pixel = __float_as_uint(a.w);
-        shade_hit<EMIT>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, 0u, so);
+        shade_hit<EMIT, INST>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, 0u, so);
         if (so.emissive) add_radiance(radiance, local_index(p, pixel), so.emission_add);
     }
     const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
@@ -496,8 +538,9 @@ __global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCoun
 }
 
 // IntersectRays (stepwise): closest hit of every live ray of bounce b -> hits[]
-template <bool COUNT>
-__global__ void __launch_bounds__(256) k_intersect(FrameParams p, DevScene sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
+// INST: an instanced scene (trace_instanced); mode is not read
+template <bool COUNT, bool INST = false>
+__global__ void __launch_bounds__(256) k_intersect(FrameParams p, SceneOf<INST> sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t n = *in_count_ptr(ctr, bounce);
@@ -507,7 +550,9 @@ __global__ void __launch_bounds__(256) k_intersect(FrameParams p, DevScene sc, i
     {
         float4 a = q.A[in][i], b = q.B[in][i];
         float bu = 0.0f, bv = 0.0f, bt = 0.0f;
-        uint32_t prim = trace<false, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+        uint32_t prim;
+        if constexpr (INST) prim = trace_instanced<false, COUNT>(sc, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+        else prim = trace<false, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
         q.hits[i] = make_float4(bu, bv, __uint_as_float(prim), bt);
     }
     if (COUNT) { warp_sum64(&ctr->nodes_ext[bounce], nv); warp_sum64(&ctr->tris_ext[bounce], nt); }
@@ -529,8 +574,8 @@ __global__ void __launch_bounds__(256) k_shade_miss(FrameParams p, DevScene sc, 
 }
 
 // ShadeSurfaceHits (stepwise)
-template <bool EMIT>
-__global__ void __launch_bounds__(256) k_shade_hits(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce, AovParams aov)
+template <bool EMIT, bool INST = false>
+__global__ void __launch_bounds__(256) k_shade_hits(FrameParams p, SceneOf<INST> sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce, AovParams aov)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t n = *in_count_ptr(ctr, bounce);
@@ -542,12 +587,12 @@ __global__ void __launch_bounds__(256) k_shade_hits(FrameParams p, DevScene sc, 
         hit = __float_as_uint(h.z) != RT_INVALID_ID;
     }
     uint32_t pixel;
-    shade_hit_group<false, EMIT>(p, sc, aov, q, 0, bounce, hit, h, i, radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
+    shade_hit_group<false, EMIT, INST>(p, sc, aov, q, 0, bounce, hit, h, i, radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
 }
 
 // IntersectShadowRays (stepwise): any-hit -> flags (0 = occluded, INVALID_ID = unoccluded)
-template <bool COUNT>
-__global__ void __launch_bounds__(256) k_intersect_shadow(FrameParams p, DevScene sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
+template <bool COUNT, bool INST = false>
+__global__ void __launch_bounds__(256) k_intersect_shadow(FrameParams p, SceneOf<INST> sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
 {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t n = ctr->emit[bounce].shadow;
@@ -556,7 +601,8 @@ __global__ void __launch_bounds__(256) k_intersect_shadow(FrameParams p, DevScen
     {
         float4 a = q.sA[i], b = q.sB[i];
         float bu, bv, bt;
-        q.shadow_flags[i] = trace<true, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+        if constexpr (INST) q.shadow_flags[i] = trace_instanced<true, COUNT>(sc, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+        else q.shadow_flags[i] = trace<true, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
     }
     if (COUNT) { warp_sum64(&ctr->nodes_shadow[bounce], nv); warp_sum64(&ctr->tris_shadow[bounce], nt); }
 }
@@ -583,7 +629,7 @@ __global__ void __launch_bounds__(256) k_accumulate(FrameParams p, Queues q, Dev
 // mix the two and idle through each other's code.  Every kernel drains its queues through a global atomic
 // cursor (warp_grab).
 template <bool COUNT, int SMEM>
-__device__ __forceinline__ void closest_phase(const DevScene& sc, int mode, const Queues& q, DevCounters* ctr, uint32_t bounce, const float4* s_bvh)
+__device__ __forceinline__ void closest_phase(const SceneOf<SMEM == RT_SMEM_INST>& sc, int mode, const Queues& q, DevCounters* ctr, uint32_t bounce, const float4* s_bvh)
 {
     const uint32_t n = *in_count_ptr(ctr, bounce);
     const int in = bounce & 1;
@@ -601,7 +647,7 @@ __device__ __forceinline__ void closest_phase(const DevScene& sc, int mode, cons
 
 // Fused IntersectShadowRays + AccumulateDirectSamples over the bounce's shadow-ray queue
 template <bool COUNT, int SMEM>
-__device__ __forceinline__ void shadow_phase(const FrameParams& p, const DevScene& sc, int mode, const Queues& q, DevCounters* ctr, float4* radiance,
+__device__ __forceinline__ void shadow_phase(const FrameParams& p, const SceneOf<SMEM == RT_SMEM_INST>& sc, int mode, const Queues& q, DevCounters* ctr, float4* radiance,
                                              uint32_t bounce, const float4* s_bvh)
 {
     const uint32_t n = ctr->emit[bounce].shadow;
@@ -612,7 +658,7 @@ __device__ __forceinline__ void shadow_phase(const FrameParams& p, const DevScen
 }
 
 template <bool COUNT, int SMEM>
-__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_shadow_accumulate(FrameParams p, DevScene sc, int mode, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce)
+__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_shadow_accumulate(FrameParams p, SceneOf<SMEM == RT_SMEM_INST> sc, int mode, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce)
 {
     extern __shared__ __align__(128) float4 s_bvh[];
     __shared__ uint64_t s_mbar;
@@ -622,7 +668,7 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_shadow_accumulate(FrameP
 }
 
 template <bool COUNT, int SMEM>
-__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_closest(FrameParams p, DevScene sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
+__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_closest(FrameParams p, SceneOf<SMEM == RT_SMEM_INST> sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
 {
     extern __shared__ __align__(128) float4 s_bvh[];
     __shared__ uint64_t s_mbar;
@@ -636,7 +682,7 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_closest(FrameParam
 // warp drains the extension queue and then the shadow queue, so the short shadow rays fill the tail of the long
 // extension rays without a second launch, a second staging of the BVH or cross-stream events.
 template <int SMEM>
-__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_both(FrameParams p, DevScene sc, int mode, Queues q, DevCounters* ctr, float4* radiance,
+__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_both(FrameParams p, SceneOf<SMEM == RT_SMEM_INST> sc, int mode, Queues q, DevCounters* ctr, float4* radiance,
                                                                    uint32_t bounce, uint32_t shadow_bounce)
 {
     extern __shared__ __align__(128) float4 s_bvh[];
@@ -686,8 +732,8 @@ __device__ __forceinline__ void flush_continuations(ContStage& st, const Queues&
 // cursor add each, so that their continuation rays leave sorted by ray_key (flush_continuations); the batch shrinks towards 256
 // entries when there are fewer than 4 full batches per CTA, so that the CTAs still finish together.  Misses past the last hit
 // batch are taken 32 at a time by each warp.
-template <bool SORT, bool EMIT = false>
-__global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams p, DevScene sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce,
+template <bool SORT, bool EMIT = false, bool INST = false>
+__global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams p, SceneOf<INST> sc, Queues q, DevCounters* ctr, float4* radiance, uint32_t bounce,
                                                                      AovParams aov, float4 scene_mid)
 {
     extern __shared__ __align__(16) float4 s_dyn[];
@@ -711,7 +757,7 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                 if (hit) h = q.hitq[k];
                 uint32_t pixel;
-                shade_hit_group<false, EMIT>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
+                shade_hit_group<false, EMIT, INST>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
             }
             else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
         }
@@ -736,7 +782,7 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                 if (hit) h = q.hitq[k];
                 uint32_t pixel;
-                shade_hit_group<true, EMIT>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
+                shade_hit_group<true, EMIT, INST>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
             }
             else if (g - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, q.missq[g - hit_span + lane], radiance);
         }
@@ -1185,6 +1231,16 @@ struct rt_ctx
     } lbvh;
     RtCamera camera = {};
     RayGenConsts raygen = {};
+    // instanced scene (rt_upload_instanced_scene): the meshes and the instance buffer in inst_mem, sized for inst_cap instances:
+    // header (2 float4), top-level records, instance records (8 float4 each), previous M rows (3 float4 each), bases (uint32)
+    bool instanced = false;
+    std::vector<rtinst::MeshInfo> meshes;
+    uint32_t inst_cap = 0, n_inst = 0;
+    std::vector<float> inst_last;                  // per instance index ever listed since the upload: its transform in the last
+                                                   // list that had it, 12 floats each (the previous transforms of object motion)
+    std::vector<float4> inst_host;                 // the image of the instance buffer the last rt_set_instances copied
+    float4 *inst_hdr = nullptr, *inst_top = nullptr, *inst_rec = nullptr, *inst_prev = nullptr;
+    uint32_t* inst_base = nullptr;
 
     // adaptive sampling (rt_set_adaptive_sampling): the requested setting, which rt_reset makes the active one; max_error > 0 = on.
     // The per-pixel state exists only while the active setting is on.
@@ -1240,6 +1296,7 @@ struct rt_ctx
     Staging stage;                 // rt_update_triangles' staging
     DevAllocs light_mem;           // the emitter and environment tables
     DevAllocs motion_mem;          // prev_pos: while object motion is on and a scene is uploaded
+    DevAllocs inst_mem;            // the instance buffer of an instanced scene
     std::vector<std::unique_ptr<void, IpcClose>> ipc_opened;
 };
 
@@ -1501,7 +1558,7 @@ struct Stage { int mode; size_t bytes; uint32_t top_k; };
 Stage bvh_stage(const rt_ctx* c, bool octant = true)
 {
     Stage st = { 0, 0, 0 };
-    if (!c->smem_bvh || c->traversal != 1) return st;
+    if (!c->smem_bvh || c->traversal != 1 || c->instanced) return st;
     size_t bytes = ((size_t)c->scene.wnodes_f4 + c->scene.wtris_f4) * 16;
     const size_t oct_bytes = bytes + 8 * (size_t)c->scene.wnodes_f4 * 16 + 16;
     if (octant && c->octant_bvh && oct_bytes <= 40 * 1024) { st.mode = 3; st.bytes = oct_bytes; return st; }
@@ -1509,6 +1566,15 @@ Stage bvh_stage(const rt_ctx* c, bool octant = true)
     uint32_t k = c->top_smem_records < c->scene.top_n ? c->top_smem_records : c->scene.top_n;
     if (k >= 8) { st.mode = 2; st.bytes = (size_t)k * 64; st.top_k = k; }
     return st;
+}
+
+// The kernel argument of an instanced scene's kernels
+DevInstScene inst_scene(const rt_ctx* c)
+{
+    DevInstScene s;
+    static_cast<DevScene&>(s) = c->scene;
+    s.inst_hdr = c->inst_hdr; s.top = c->inst_top; s.irec = c->inst_rec; s.ibase = c->inst_base;
+    return s;
 }
 
 // Launches a staged traversal kernel: calls launch(std::integral_constant<int, SMEM>, the DevScene with this launch's top_k, the
@@ -1523,7 +1589,8 @@ auto launch_staged(const rt_ctx* c, F&& launch, bool octant = true)
     if (sg.mode == 1) return launch(std::integral_constant<int, 1>(), sc, sg.bytes);
     if (sg.mode == 2) return launch(std::integral_constant<int, 2>(), sc, sg.bytes);
     if constexpr (std::is_void_v<decltype(launch(std::integral_constant<int, 1>(), sc, sg.bytes))>)
-    {   // the per-phase kernels (their launchers return nothing); the frame kernels never ask for mode 3
+    {   // the per-phase kernels (their launchers return nothing); the frame kernels never ask for mode 3 or run instanced scenes
+        if (c->instanced) return launch(std::integral_constant<int, RT_SMEM_INST>(), inst_scene(c), (size_t)0);
         if (sg.mode == 3) return launch(std::integral_constant<int, 3>(), sc, sg.bytes);
     }
     return launch(std::integral_constant<int, 0>(), sc, sg.bytes);
@@ -1570,7 +1637,7 @@ AovParams aov_params(const rt_ctx* c)
     memset(&a, 0, sizeof(a));
     a.enabled = (aov_wanted(c) && c->aov_albedo) ? 1 : 0;
     a.albedo = c->aov_albedo; a.depth = c->aov_depth; a.normal = c->aov_normal; a.velocity = c->aov_velocity;
-    a.prev_pos = c->prev_pos;
+    a.prev_pos = c->instanced ? (c->object_motion ? c->inst_prev : nullptr) : c->prev_pos;
     return a;
 }
 
@@ -1632,7 +1699,9 @@ int rt_create(uint32_t width, uint32_t height, int device, rt_ctx** out_ctx)
     if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail("cudaGetDeviceProperties", e);
     c->num_sms = prop.multiProcessorCount;
     if ((e = cudaFuncSetAttribute(k_shade_queues<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess ||
-        (e = cudaFuncSetAttribute(k_shade_queues<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess)
+        (e = cudaFuncSetAttribute(k_shade_queues<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess ||
+        (e = cudaFuncSetAttribute(k_shade_queues<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess ||
+        (e = cudaFuncSetAttribute(k_shade_queues<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ContStage))) != cudaSuccess)
         return fail("cudaFuncSetAttribute(k_shade_queues)", e);
     if ((e = make_stream(c->stream)) != cudaSuccess) return fail("cudaStreamCreate", e);
     if ((e = c->ctx_mem.alloc(c->counters, 1)) != cudaSuccess) return fail("cudaMalloc(counters)", e);
@@ -1790,21 +1859,39 @@ static int set_prev_positions(rt_ctx* c)
     return RT_OK;
 }
 
-int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
+// The instance buffer for `cap` instances (allocated before the old one is freed; the caller has drained the stream)
+static int alloc_instances(rt_ctx* c, uint32_t cap)
 {
-    RT_CHECK_CTX(c); RT_FANOUT(c, rt_upload_scene(k, s));
-    if (!s) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: null scene");
+    DevAllocs g;
+    char* base = nullptr;
+    const size_t top = (size_t)std::max(cap, 2u) - 1u;
+    const size_t f4 = 2 + top * 4 + (size_t)cap * 8 + (size_t)cap * 3 + ((size_t)cap + 3) / 4;
+    RT_CUDA(c, g.alloc(base, f4 * 16));
+    RT_CUDA(c, cudaMemset(base, 0, f4 * 16));
+    float4* p = (float4*)base;
+    c->inst_hdr = p; c->inst_top = p + 2; c->inst_rec = c->inst_top + top * 4; c->inst_prev = c->inst_rec + (size_t)cap * 8;
+    c->inst_base = (uint32_t*)(c->inst_prev + (size_t)cap * 3);
+    c->inst_mem = std::move(g); c->inst_cap = cap;
+    ++c->config_gen;
+    return RT_OK;
+}
+
+// rt_upload_scene (meshes == nullptr) and rt_upload_instanced_scene
+static int upload_scene(rt_ctx* c, const RtSceneDesc* s, const RtMeshDesc* meshes, uint32_t n_meshes)
+{
+    const char* fn = meshes ? "rt_upload_instanced_scene" : "rt_upload_scene";
+    if (!s) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: null scene", fn);
     // cl_pt_integrator.cpp:385,404 assert non-empty triangles/materials; light.h:46 divides by the light count
-    if (!s->triangles || s->n_triangles == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: scene has no triangles");
-    if (!s->materials || s->n_materials == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: scene has no materials");
-    if (!s->nodes || s->n_nodes == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: scene has no BVH nodes");
+    if (!s->triangles || s->n_triangles == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: scene has no triangles", fn);
+    if (!s->materials || s->n_materials == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: scene has no materials", fn);
+    if (!s->nodes || s->n_nodes == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: scene has no BVH nodes", fn);
     if (!s->lights || s->n_lights == 0 || s->scene_info.analytic_light_count == 0)
-        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: at least one analytic light is required (light.h:46 divides by the count)");
-    if (s->scene_info.analytic_light_count > s->n_lights) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: analytic_light_count exceeds n_lights");
-    if (!s->env_image || s->env_width == 0 || s->env_height == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: environment image required");
-    if (s->n_triangles >= 0x7FFFFFFFull || s->n_nodes >= 0x7FFFFFFFull) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: scene too large");
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: at least one analytic light is required (light.h:46 divides by the count)", fn);
+    if (s->scene_info.analytic_light_count > s->n_lights) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: analytic_light_count exceeds n_lights", fn);
+    if (!s->env_image || s->env_width == 0 || s->env_height == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: environment image required", fn);
+    if (s->n_triangles >= 0x7FFFFFFFull || s->n_nodes >= 0x7FFFFFFFull) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: scene too large", fn);
     for (uint64_t i = 0; i < s->n_triangles; ++i)
-        if (s->triangles[i].mtlIndex >= s->n_materials) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: triangle %llu has material index out of range", (unsigned long long)i);
+        if (s->triangles[i].mtlIndex >= s->n_materials) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: triangle %llu has material index out of range", fn, (unsigned long long)i);
 
     for (uint64_t i = 0; i < s->n_materials; ++i)
     {   // texture indices of the packed materials must exist (0xFF = none)
@@ -1812,24 +1899,24 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
         uint32_t idx[6] = { m.diffuse_albedo >> 24, m.specular_albedo >> 24, (m.roughness_metalness >> 8) & 0xFF, m.roughness_metalness >> 24,
                             (m.ior_emission_idx_transparency >> 8) & 0xFF, m.ior_emission_idx_transparency >> 24 };
         for (uint32_t t : idx)
-            if (t != RT_INVALID_TEXTURE_IDX && t >= s->n_textures) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: material %llu references texture %u of %llu", (unsigned long long)i, t, (unsigned long long)s->n_textures);
+            if (t != RT_INVALID_TEXTURE_IDX && t >= s->n_textures) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: material %llu references texture %u of %llu", fn, (unsigned long long)i, t, (unsigned long long)s->n_textures);
     }
     for (uint64_t i = 0; i < s->n_textures; ++i)
     {
         const RtTexture& t = s->textures[i];
         if (t.width <= 0 || t.height <= 0 || t.data_start < 0 || (uint64_t)t.data_start + (uint64_t)t.width * t.height > s->n_texture_data)
-            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: texture %llu lies outside the texel array", (unsigned long long)i);
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: texture %llu lies outside the texel array", fn, (unsigned long long)i);
         // sample_texture (rt_device.cuh) and material.h:259 index texels in int: the last texel must lie below 2^31
         if ((uint64_t)t.data_start + (uint64_t)t.width * t.height > 0x80000000ull)
-            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: texture %llu ends beyond texel 2^31 - 1", (unsigned long long)i);
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: texture %llu ends beyond texel 2^31 - 1", fn, (unsigned long long)i);
     }
     if (c->emitter_sampling)
     {
         if (s->n_emissive && !s->emissive_indices)
-            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: emitter sampling is on and n_emissive > 0 with no emissive_indices");
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: emitter sampling is on and n_emissive > 0 with no emissive_indices", fn);
         std::string err;
         if (!rtemit::check_indices(s->emissive_indices, s->n_emissive, s->n_triangles, err))
-            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: emitter sampling is on and %s", err.c_str());
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: emitter sampling is on and %s", fn, err.c_str());
     }
 
     RT_CUDA(c, cudaSetDevice(c->device));
@@ -1869,11 +1956,37 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     if ((rc = upload(s->env_image, (size_t)s->env_width * s->env_height * 16, (const void**)&ds.env))) return rc;
     ds.env_w = (int)s->env_width; ds.env_h = (int)s->env_height;
     ds.light_count = s->scene_info.analytic_light_count;
+    c->meshes.clear();
+    if (meshes)
+    {   // every mesh's records as rt_upload_scene derives them from that mesh alone, concatenated; references stay mesh-relative
+        std::vector<rtbvh::F4> nodes, tris;
+        for (uint32_t k = 0; k < n_meshes; ++k)
+        {
+            const RtMeshDesc& m = meshes[k];
+            rtbvh::WideLayout wl;
+            std::string err;
+            if (!rtbvh::build_layout(s->nodes + m.first_node, m.n_nodes, s->triangles + m.first_triangle, m.n_triangles, wl, err))
+                RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: malformed BVH of mesh %u: %s", fn, k, err.c_str());
+            const RtLinearBVHNode& r = s->nodes[m.first_node];
+            rtinst::MeshInfo mi = { wl.root_ref, (uint32_t)nodes.size(), (uint32_t)m.first_triangle, (uint32_t)m.n_triangles, (uint32_t)m.first_node,
+                                    { r.bounds_min.x, r.bounds_min.y, r.bounds_min.z }, { r.bounds_max.x, r.bounds_max.y, r.bounds_max.z } };
+            c->meshes.push_back(mi);
+            nodes.insert(nodes.end(), wl.nodes.begin(), wl.nodes.end());
+            tris.resize(std::max<size_t>(tris.size(), (size_t)(m.first_triangle + m.n_triangles) * 3));
+            std::copy(wl.tris.begin(), wl.tris.end(), tris.begin() + (size_t)m.first_triangle * 3);
+        }
+        if (nodes.size() >= 0x7FFFFFFFull) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: scene too large", fn);
+        if ((rc = upload_to(c, c->tree_mem, nodes.data(), nodes.size() * 16, (const void**)&ds.wnodes))) return rc;
+        if ((rc = upload(tris.data(), tris.size() * 16, (const void**)&ds.wtris))) return rc;
+        ds.root_ref = 0; ds.top_n = 0; ds.top_k = 0;
+        ds.wnodes_f4 = (uint32_t)nodes.size(); ds.wtris_f4 = (uint32_t)tris.size();
+    }
+    else
     {   // optimised traversal layout
         rtbvh::WideLayout wl;
         std::string err;
         if (!rtbvh::build_layout(s->nodes, s->n_nodes, s->triangles, s->n_triangles, wl, err))
-            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_scene: malformed BVH: %s", err.c_str());
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: malformed BVH: %s", fn, err.c_str());
         if ((rc = upload_to(c, c->tree_mem, wl.nodes.data(), wl.nodes.size() * 16, (const void**)&ds.wnodes))) return rc;
         if ((rc = upload(wl.tris.data(), wl.tris.size() * 16, (const void**)&ds.wtris))) return rc;
         ds.root_ref = wl.root_ref;
@@ -1885,7 +1998,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
                                (root.bounds_min.z + root.bounds_max.z) * 0.5f, 0.0f);
     // what the emitter table needs is kept only for a scene that lists emitters (a list with a null pointer counts as empty: with
     // the option off the array was never read, and such uploads stay accepted)
-    const uint64_t n_emit = s->emissive_indices ? s->n_emissive : 0;
+    const uint64_t n_emit = (s->emissive_indices && !meshes) ? s->n_emissive : 0;
     c->emit_idx.assign(s->emissive_indices, s->emissive_indices + n_emit);
     c->emit_tris.assign(n_emit, RtTriangle{});
     for (uint64_t i = 0; i < n_emit; ++i)
@@ -1896,10 +2009,84 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
     c->emit_moved = false;
     c->n_tris = s->n_triangles; c->n_nodes = s->n_nodes;
     c->analytic_lit = rtenv::analytic_lit(s->lights, s->scene_info.analytic_light_count);
-    if (c->object_motion && (rc = set_prev_positions(c))) return rc;
+    c->instanced = meshes != nullptr;
+    c->inst_mem.clear(); c->inst_hdr = c->inst_top = c->inst_rec = c->inst_prev = nullptr; c->inst_base = nullptr;
+    c->inst_cap = c->n_inst = 0; c->inst_last.clear();
+    if (c->instanced && (rc = alloc_instances(c, 1))) return rc;          // no instances yet: every ray misses
+    if (!c->instanced && c->object_motion && (rc = set_prev_positions(c))) return rc;
     c->scene_ready = true;
     ++c->config_gen;
     return refresh_lights(c);
+}
+
+int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_upload_scene(k, s));
+    return upload_scene(c, s, nullptr, 0);
+}
+
+int rt_upload_instanced_scene(rt_ctx* c, const RtSceneDesc* s, const RtMeshDesc* meshes, uint32_t n_meshes)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_upload_instanced_scene(k, s, meshes, n_meshes));
+    if (c->emitter_sampling)
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_upload_instanced_scene: emitter sampling (RT_OPT_EMITTER_SAMPLING 1) is not available on instanced scenes");
+    if (!s) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_instanced_scene: null scene");
+    if (!meshes || n_meshes == 0) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_instanced_scene: no meshes");
+    for (uint32_t k = 0; k < n_meshes; ++k)
+    {
+        const RtMeshDesc& m = meshes[k];
+        if (m.n_triangles == 0 || m.n_nodes == 0 || m.first_triangle > s->n_triangles || m.n_triangles > s->n_triangles - m.first_triangle ||
+            m.first_node > s->n_nodes || m.n_nodes > s->n_nodes - m.first_node)
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_instanced_scene: mesh %u is empty or lies outside the scene's arrays", k);
+        if (!s->nodes) break;                      // upload_scene reports the missing nodes
+        const RtLinearBVHNode& r = s->nodes[m.first_node];
+        const float b[6] = { r.bounds_min.x, r.bounds_min.y, r.bounds_min.z, r.bounds_max.x, r.bounds_max.y, r.bounds_max.z };
+        for (float v : b) if (!std::isfinite(v)) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_upload_instanced_scene: mesh %u has a root box that is not finite", k);
+    }
+    return upload_scene(c, s, meshes, n_meshes);
+}
+
+int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_set_instances(k, instances, n));
+    if (!c->scene_ready || !c->instanced) RT_FAIL(c, RT_ERR_NOT_READY, "rt_set_instances: no instanced scene (rt_upload_instanced_scene)");
+    if (n && !instances) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_instances: null instances");
+    rtinst::Prepared pr;
+    std::string err;
+    if (!rtinst::prepare(instances, n, c->meshes, pr, err)) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_set_instances: %s", err.c_str());
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the instances this call rewrites
+    if (n > c->inst_cap)
+    {   // a larger buffer (at least twice the old, so that a list growing one by one re-captures the frame graph log n times):
+        // frames in flight read the old one.  The launch arguments change, so the sort-key origin of the shading pass moves to the
+        // centre of the new top-level root box here (it orders rays only; between growths it stays).
+        RT_CUDA(c, cudaStreamSynchronize(c->stream));
+        int rc = alloc_instances(c, std::max(n, 2u * c->inst_cap)); if (rc) return rc;
+        const rtinst::Box& b = pr.tree.root;
+        c->scene_mid = make_float4((b.lo[0] + b.hi[0]) * 0.5f, (b.lo[1] + b.hi[1]) * 0.5f, (b.lo[2] + b.hi[2]) * 0.5f, 0.0f);
+    }
+    const size_t top = (size_t)std::max(c->inst_cap, 2u) - 1u;
+    const size_t f4 = 2 + top * 4 + (size_t)c->inst_cap * 11 + ((size_t)c->inst_cap + 3) / 4;
+    std::vector<float4>& h = c->inst_host;
+    h.assign(f4, make_float4(0.0f, 0.0f, 0.0f, 0.0f));
+    const rtinst::Box& rb = pr.tree.root;
+    h[0] = make_float4(rb.lo[0], rb.lo[1], rb.lo[2], rtinst::int_bits(pr.tree.root_ref));
+    h[1] = make_float4(rb.hi[0], rb.hi[1], rb.hi[2], rtinst::int_bits((int)n));
+    memcpy(&h[2], pr.tree.records.data(), pr.tree.records.size() * 4);
+    float4* rec = &h[2 + top * 4];
+    memcpy(rec, pr.rec.data(), pr.rec.size() * 4);
+    float4* prev = rec + (size_t)c->inst_cap * 8;
+    // previous transforms: index i's transform in the last earlier list that had index i, else its new one
+    const size_t known = c->inst_last.size() / 12;
+    for (uint32_t i = 0; i < n; ++i)
+        memcpy(prev + (size_t)i * 3, i < known ? &c->inst_last[(size_t)i * 12] : instances[i].object_to_world, 48);
+    memcpy(prev + (size_t)c->inst_cap * 3, pr.base.data(), pr.base.size() * 4);
+    // one copy of the whole image, in render-stream order after the work submitted before (pageable: the call returns once it is staged)
+    RT_CUDA(c, cudaMemcpyAsync(c->inst_hdr, h.data(), f4 * 16, cudaMemcpyHostToDevice, c->stream));
+    if (n > known) c->inst_last.resize((size_t)n * 12);
+    for (uint32_t i = 0; i < n; ++i) memcpy(&c->inst_last[(size_t)i * 12], instances[i].object_to_world, 48);
+    c->n_inst = n;
+    return RT_OK;
 }
 
 // ---- geometry updates: rt_update_triangles[_device], rt_read_bvh (include/rt_b200.h)
@@ -1909,6 +2096,7 @@ int rt_upload_scene(rt_ctx* c, const RtSceneDesc* s)
 static int begin_update(rt_ctx* c, const void* triangles, uint64_t n, const char* what)
 {
     if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "%s: rt_upload_scene has not been called", what);
+    if (c->instanced) RT_FAIL(c, RT_ERR_UNSUPPORTED, "%s: not available on an instanced scene", what);
     if (!triangles) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: null triangles", what);
     if (n != c->n_tris) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: %llu triangles, the upload has %llu", what, (unsigned long long)n, (unsigned long long)c->n_tris);
     RT_CUDA(c, cudaSetDevice(c->device));
@@ -2012,6 +2200,7 @@ int rt_read_bvh(rt_ctx* c, RtLinearBVHNode* nodes, float* records, uint64_t* n_r
 {
     RT_CHECK_CTX(c); RT_NOT_ON_GROUP(c, "rt_read_bvh");
     if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_read_bvh: rt_upload_scene has not been called");
+    if (c->instanced) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_read_bvh: not available on an instanced scene");
     if (records && !n_records) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_read_bvh: records without n_records");
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = join_shadow(c); if (rc) return rc; }
@@ -2169,6 +2358,7 @@ int rt_rebuild_bvh(rt_ctx* c, uint64_t* n_nodes)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_rebuild_bvh(k, n_nodes));
     if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_rebuild_bvh: rt_upload_scene has not been called");
+    if (c->instanced) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_rebuild_bvh: not available on an instanced scene");
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the tree this call rewrites
     if (!c->lbvh.live) { int rc = alloc_lbvh(c); if (rc) return rc; }
@@ -2205,6 +2395,7 @@ int rt_rebuild_bvh_ploc(rt_ctx* c, uint64_t* n_nodes)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_rebuild_bvh_ploc(k, n_nodes));
     if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "rt_rebuild_bvh_ploc: rt_upload_scene has not been called");
+    if (c->instanced) RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_rebuild_bvh_ploc: not available on an instanced scene");
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the tree this call rewrites
     // The first call after an upload builds in a new tree group, which replaces the uploaded tree only once the clustered tree is
@@ -2343,6 +2534,8 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
         return (c->emitter_sampling || c->env_sampling) ? refresh_lights(c) : RT_OK;
     case RT_OPT_EMITTER_SAMPLING:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "emitter sampling must be 0 (off) or 1 (emissive triangles with MIS)");
+        if (value == 1 && c->scene_ready && c->instanced)
+            RT_FAIL(c, RT_ERR_UNSUPPORTED, "emitter sampling is not available on instanced scenes");
         if (value == 1 && c->scene_ready)
         {
             std::string err;
@@ -2368,7 +2561,7 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
             return RT_OK;
         }
         c->object_motion = 1;
-        return c->scene_ready ? set_prev_positions(c) : RT_OK;
+        return (c->scene_ready && !c->instanced) ? set_prev_positions(c) : RT_OK;   // instances keep their previous transforms always
     case RT_OPT_SAMPLER:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "sampler type must be 0 (kRandom) or 1 (kBlueNoise)");
         if (value == 1 && !c->d_bn)
@@ -2599,7 +2792,9 @@ int rt_intersect(rt_ctx* c, uint32_t bounce)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_intersect(k, bounce));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     TimedLaunch t(c, RT_K_INTERSECT);
-    if (c->count_traversal) k_intersect<true><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
+    if (c->instanced)
+        (c->count_traversal ? k_intersect<true, true> : k_intersect<false, true>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, bounce);
+    else if (c->count_traversal) k_intersect<true><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
     else k_intersect<false><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
     return post_launch(c, "k_intersect");
 }
@@ -2633,7 +2828,9 @@ int rt_shade_hits(rt_ctx* c, uint32_t bounce)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     c->cur_bounce = bounce;
     TimedLaunch t(c, RT_K_HIT);
-    (lights_sampled(c) ? k_shade_hits<true> : k_shade_hits<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
+    if (c->instanced)
+        (lights_sampled(c) ? k_shade_hits<true, true> : k_shade_hits<false, true>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->q, c->counters, c->radiance, bounce, aov_params(c));
+    else (lights_sampled(c) ? k_shade_hits<true> : k_shade_hits<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
     return post_launch(c, "k_shade_hits");
 }
 
@@ -2642,7 +2839,9 @@ int rt_intersect_shadow(rt_ctx* c)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_intersect_shadow(k));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, c->cur_bounce);
     TimedLaunch t(c, RT_K_INTERSECT_SHADOW);
-    if (c->count_traversal) k_intersect_shadow<true><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->cur_bounce);
+    if (c->instanced)
+        (c->count_traversal ? k_intersect_shadow<true, true> : k_intersect_shadow<false, true>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, c->cur_bounce);
+    else if (c->count_traversal) k_intersect_shadow<true><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->cur_bounce);
     else k_intersect_shadow<false><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->cur_bounce);
     return post_launch(c, "k_intersect_shadow");
 }
@@ -2689,7 +2888,7 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     {   // this bounce's closest-hit traversal + the previous bounce's shadow pass in one kernel
         c->shadow_deferred = false;
         TimedLaunch t(c, RT_K_TRACE_BOTH);
-        launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) {
+        launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
             auto* k = k_trace_both<smem.value>;
             launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce, c->shadow_deferred_bounce);
         });
@@ -2698,8 +2897,10 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     else
     {
         TimedLaunch t(c, RT_K_TRACE_CLOSEST);
-        if (c->count_traversal) k_trace_closest<true, 0><<<RT_PGRID(c, (k_trace_closest<true, 0>), 0), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
-        else launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) {
+        if (c->count_traversal && c->instanced)
+            k_trace_closest<true, RT_SMEM_INST><<<RT_PGRID(c, (k_trace_closest<true, RT_SMEM_INST>), 0), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, bounce);
+        else if (c->count_traversal) k_trace_closest<true, 0><<<RT_PGRID(c, (k_trace_closest<true, 0>), 0), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
+        else launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
             auto* k = k_trace_closest<false, smem.value>;
             launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
         });
@@ -2708,9 +2909,16 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     { int rc = join_shadow(c); if (rc) return rc; }     // the shading pass accumulates into radiance and refills the shadow queue
     TimedLaunch t(c, RT_K_SHADE_QUEUES);
     const bool sort = sorted_shading(c);
+    const size_t sm = sort ? sizeof(ContStage) : 0;
+    if (c->instanced)
+    {
+        auto* k = lights_sampled(c) ? (sort ? k_shade_queues<true, true, true> : k_shade_queues<false, true, true>)
+                                     : (sort ? k_shade_queues<true, false, true> : k_shade_queues<false, false, true>);
+        launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), inst_scene(c), c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
+        return post_launch(c, "k_shade_queues");
+    }
     auto* k = lights_sampled(c) ? (sort ? k_shade_queues<true, true> : k_shade_queues<false, true>)
                                  : (sort ? k_shade_queues<true> : k_shade_queues<false>);
-    const size_t sm = sort ? sizeof(ContStage) : 0;
     launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
     return post_launch(c, "k_shade_queues");
 }
@@ -2727,8 +2935,10 @@ static int ensure_shadow_stream(rt_ctx* c)
 static int launch_shadow_pass(rt_ctx* c, uint32_t bounce, cudaStream_t st)
 {
     TimedLaunch t(c, RT_K_SHADOW_ACCUMULATE, st);
-    if (c->count_traversal) k_shadow_accumulate<true, 0><<<RT_PGRID(c, (k_shadow_accumulate<true, 0>), 0), 256, 0, st>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->radiance, bounce);
-    else launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) {
+    if (c->count_traversal && c->instanced)
+        k_shadow_accumulate<true, RT_SMEM_INST><<<RT_PGRID(c, (k_shadow_accumulate<true, RT_SMEM_INST>), 0), 256, 0, st>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, c->radiance, bounce);
+    else if (c->count_traversal) k_shadow_accumulate<true, 0><<<RT_PGRID(c, (k_shadow_accumulate<true, 0>), 0), 256, 0, st>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->radiance, bounce);
+    else launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
         auto* k = k_shadow_accumulate<false, smem.value>;
         k<<<RT_PGRID(c, k, sm), 256, sm, st>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce);
     });
@@ -2823,6 +3033,7 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
 // switches at 7168 pixels per SM (0.95 M pixels on 132 SMs).
 static bool frame_kernel_selected(const rt_ctx* c)
 {
+    if (c->instanced) return false;                // instanced scenes always run the per-phase kernels
     if (c->frame_kernel == 2) return (size_t)c->n_local <= (size_t)c->num_sms * 7168u;
     return c->frame_kernel == 1;
 }

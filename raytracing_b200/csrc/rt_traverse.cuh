@@ -22,10 +22,25 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 // L1/L2 (RT_OPT_TOP_SMEM); SMEM 0 stages nothing.  SMEM 3 stages what SMEM 1 does and then builds, behind the triangles, the
 // eight octant-ordered copies of the interior records (rt_octant.h; table s at dst + wnodes_f4 + wtris_f4 + s * wnodes_f4) and
 // one flag word behind them: 1 when every record passed rt_oct_record_ok and the tables exist, 0 when the CTA must not use them.
+// The staging mode of the traversal kernels of instanced scenes (rt_upload_instanced_scene): nothing is staged and the two-level
+// traversal (trace_instanced) runs.  Those kernels take a DevInstScene: DevScene describes the concatenated meshes (nodes_ref,
+// tris_ref, wnodes, wtris, tri_shade) and the fields below the instances.  The flat kernels keep DevScene, so their parameters
+// and code are unchanged.
+#define RT_SMEM_INST 4
+struct DevInstScene : DevScene
+{
+    const float4* inst_hdr;        // 2 float4: (top root box min xyz, root ref), (root box max xyz, instance count) as int bits
+    const float4* top;             // top-level records (rt_bvh_layout.h layout, leaf ref = ~instance), rt_instances.h
+    const float4* irec;            // 8 float4 per instance: W rows, M rows, (mesh root ref, mesh record base in float4, first
+                                   // triangle, base) as int bits, (det sign, first node bits, -, -)
+    const uint32_t* ibase;         // base (first virtual triangle id) per instance, ascending
+};
+template <bool INST> using SceneOf = typename std::conditional<INST, DevInstScene, DevScene>::type;
+
 template <int SMEM>
 __device__ __forceinline__ void stage_bvh(float4* dst, const DevScene& sc, uint64_t* mbar)
 {
-    if (SMEM == 0) return;
+    if (SMEM == 0 || SMEM == RT_SMEM_INST) return;
     const uint32_t bar = smem_u32(mbar);
     constexpr bool WHOLE = SMEM == 1 || SMEM == 3;
     const uint32_t nodes_bytes = (WHOLE ? sc.wnodes_f4 : sc.top_k * 4u) * 16u, tris_bytes = WHOLE ? sc.wtris_f4 * 16u : 0u;
@@ -132,9 +147,11 @@ __device__ __forceinline__ float4 ld_bvh(const float4* p) { return SMEM ? *p : _
 // DFS, 64-entry private stack, far child pushed unconditionally and box-tested when popped,
 // near child chosen by ray_sign[axis], inclusive tests, later equal-t hit overwrites, back-face
 // culling (det < 1e-8 rejects).  ANY = the -D SHADOW_RAYS variant (returns 0 on first hit).
-template <bool ANY, bool COUNT>
+// SIGNED (instanced scenes): the culling test reads det * cull (cull = sign(det M) of a mirrored instance: -1), so that a
+// mirrored instance culls the faces its flattened triangles would; u, v and t still divide by det.
+template <bool ANY, bool COUNT, bool SIGNED = false>
 __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d, float t_min, float t_max,
-                                                  float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
+                                                  float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt, float cull = 1.0f)
 {
     f3 inv = splat(1.0f) / d;
     int sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
@@ -163,7 +180,8 @@ __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d
                     f3 e1 = p2 - p1, e2 = p3 - p1;
                     f3 pvec = cross(d, e2);
                     float det = dot(e1, pvec);
-                    if (det < 1e-8f || -det > 1e-8f) continue;
+                    const float cdet = SIGNED ? det * cull : det;
+                    if (cdet < 1e-8f || -cdet > 1e-8f) continue;
                     float inv_det = 1.0f / det;
                     f3 tvec = o - p1;
                     float u = dot(tvec, pvec) * inv_det;
@@ -214,18 +232,18 @@ __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d
 // branch inside the ordered loop was measured and cost half the gain):
 // exactly what RT_OPT_OCTANT_BVH 0 computes, also where that differs from the literal traversal (a NaN t_max from a triangle
 // with an infinite vertex ends the staged traversal and not the literal one).
-template <bool ANY, bool COUNT, int SMEM, bool PIN = false>
+template <bool ANY, bool COUNT, int SMEM, bool PIN = false, bool SIGNED = false>
 __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4* wnodes, const float4* wtris, f3 o, f3 d, float t_min, float t_max,
-                                               float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
+                                               float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt, float cull = 1.0f)
 {
     constexpr bool OCT = SMEM == 3, PACKED = SMEM == 1 || OCT;
     float fin = ((o.x + o.y) + o.z) + ((d.x + d.y) + d.z);
     if (!(fabsf(fin) <= 3.0e38f) || COUNT)
-        return trace_literal<ANY, COUNT>(sc, o, d, t_min, t_max, bu, bv, bt, nv, nt);
+        return trace_literal<ANY, COUNT, SIGNED>(sc, o, d, t_min, t_max, bu, bv, bt, nv, nt, cull);
 
     f3 inv = splat(1.0f) / d;
     if (OCT && !(rt_oct_ray_ok(inv.x, inv.y, inv.z) && (!ANY || t_max == t_max) && *(const uint32_t*)(wtris + sc.wtris_f4 + 8u * sc.wnodes_f4) != 0u))
-        return trace_fast<ANY, COUNT, OCT ? 1 : SMEM, PIN>(sc, wnodes, wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt);
+        return trace_fast<ANY, COUNT, OCT ? 1 : SMEM, PIN, SIGNED>(sc, wnodes, wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt, cull);
     const bool sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
     uint32_t sign_bits = (sx ? 1u : 0u) | (sy ? 2u : 0u) | (sz ? 4u : 0u);
     if (PIN) asm volatile("" : "+r"(sign_bits));
@@ -377,7 +395,8 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
             f3 pvec = RT_CROSS(d, e2);
             float det = RT_DOT(e1, pvec);
             if (PIN) asm volatile("" : "+f"(det));
-            if (!(det < 1e-8f || -det > 1e-8f))
+            const float cdet = SIGNED ? det * cull : det;
+            if (!(cdet < 1e-8f || -cdet > 1e-8f))
             {
                 float inv_det = 1.0f / det;
                 f3 tvec = o - p1;
@@ -420,13 +439,100 @@ __device__ __forceinline__ uint32_t trace(const DevScene& sc, int mode, f3 o, f3
     return trace_fast<ANY, COUNT, 0>(sc, sc.wnodes, sc.wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt);
 }
 
+// Two-level traversal of an instanced scene (rt_b200.h, instanced scenes).  The top-level tree is walked as trace_fast walks a
+// flat one from L1 (same slab test, near/far order, pop rule and 64-entry stack); at an instance leaf the ray is moved into
+// object space by W and the mesh's tree is traced by trace_fast itself, on a view of DevScene whose arrays start at the mesh's,
+// with the shared t_max and a stack of its own.  A hit stores the instance's virtual id, base + the mesh's triangle index.
+// COUNT counts every node whose box is tested once: the top-level root (the header box) and the two children of each top-level
+// record visited, then the mesh nodes of trace_literal (trace_fast's counting path; it tests the mesh's root box again).
+template <bool ANY, bool COUNT>
+__device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o, f3 d, float t_min, float t_max,
+                                                    float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
+{
+    uint32_t prim = RT_INVALID_ID;
+    const float4 h0 = __ldg(sc.inst_hdr), h1 = __ldg(sc.inst_hdr + 1);
+    if (__float_as_uint(h1.w) == 0u) return prim;                  // no instances: every ray misses
+    const f3 inv = splat(1.0f) / d;
+    const bool sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
+    {   // root box
+        f3 t0 = (mk3(h0) - o) * inv, t1 = (mk3(h1) - o) * inv;
+        float lo = fmaxf(fmaxf(fminf(t0.x, t1.x), fminf(t0.y, t1.y)), fminf(t0.z, t1.z));
+        float hi = fminf(fminf(fmaxf(t0.x, t1.x), fmaxf(t0.y, t1.y)), fmaxf(t0.z, t1.z));
+        if (COUNT) ++nv;
+        if (!(fminf(hi, t_max) >= fmaxf(lo, t_min))) return prim;
+    }
+    int cur = __float_as_int(h0.w);
+    int sp = 0;
+    int stack_ref[64];
+    float stack_t[64];
+    for (;;)
+    {
+        while (cur >= 0)
+        {
+            const float4* np = sc.top + (size_t)cur * 4;
+            float4 a = __ldg(np), b = __ldg(np + 1), c = __ldg(np + 2), m = __ldg(np + 3);
+            if (COUNT) nv += 2;
+            f3 t00 = (mk3(a.x, a.y, a.z) - o) * inv, t01 = (mk3(a.w, b.x, b.y) - o) * inv;
+            f3 t10 = (mk3(b.z, b.w, c.x) - o) * inv, t11 = (mk3(c.y, c.z, c.w) - o) * inv;
+            float lo0 = fmaxf(fmaxf(fmaxf(fminf(t00.x, t01.x), fminf(t00.y, t01.y)), fminf(t00.z, t01.z)), t_min);
+            float hi0 = fminf(fminf(fmaxf(t00.x, t01.x), fmaxf(t00.y, t01.y)), fmaxf(t00.z, t01.z));
+            float lo1 = fmaxf(fmaxf(fmaxf(fminf(t10.x, t11.x), fminf(t10.y, t11.y)), fminf(t10.z, t11.z)), t_min);
+            float hi1 = fminf(fminf(fmaxf(t10.x, t11.x), fmaxf(t10.y, t11.y)), fmaxf(t10.z, t11.z));
+            bool h0b = fminf(hi0, t_max) >= lo0, h1b = fminf(hi1, t_max) >= lo1;
+            int r0 = __float_as_int(m.x), r1 = __float_as_int(m.y);
+            uint32_t axis = __float_as_uint(m.z);
+            bool swap = axis == 0 ? sx : (axis == 1 ? sy : sz);
+            int near_ref = swap ? r1 : r0, far_ref = swap ? r0 : r1;
+            bool near_hit = swap ? h1b : h0b, far_hit = swap ? h0b : h1b;
+            float far_lo = swap ? lo0 : lo1;
+            if (near_hit)
+            {
+                if (far_hit) { stack_ref[sp] = far_ref; stack_t[sp] = far_lo; ++sp; }
+                cur = near_ref;
+            }
+            else if (far_hit) cur = far_ref;
+            else
+            {
+                bool found = false;
+                while (sp > 0) { --sp; if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; } }
+                if (!found) return prim;
+            }
+        }
+        {   // instance leaf: the ray in object space, then the mesh's tree
+            const float4* ir = sc.irec + (size_t)(~cur) * 8;
+            const float4 w0 = __ldg(ir), w1 = __ldg(ir + 1), w2 = __ldg(ir + 2), mi = __ldg(ir + 6), mj = __ldg(ir + 7);
+            const f3 oo = mk3(((w0.x * o.x + w0.y * o.y) + w0.z * o.z) + w0.w, ((w1.x * o.x + w1.y * o.y) + w1.z * o.z) + w1.w,
+                              ((w2.x * o.x + w2.y * o.y) + w2.z * o.z) + w2.w);
+            const f3 od = mk3((w0.x * d.x + w0.y * d.y) + w0.z * d.z, (w1.x * d.x + w1.y * d.y) + w1.z * d.z, (w2.x * d.x + w2.y * d.y) + w2.z * d.z);
+            const uint32_t rec = __float_as_uint(mi.y), first = __float_as_uint(mi.z);
+            DevScene ms = sc;
+            ms.root_ref = __float_as_int(mi.x);
+            ms.wnodes = sc.wnodes + rec; ms.wtris = sc.wtris + (size_t)first * 3;
+            ms.tris_ref = sc.tris_ref + (size_t)first * 3; ms.nodes_ref = sc.nodes_ref + (size_t)__float_as_uint(mj.y) * 3;
+            float u, v, t;
+            const uint32_t p = trace_fast<ANY, COUNT, 0, false, true>(ms, ms.wnodes, ms.wtris, oo, od, t_min, t_max, u, v, t, nv, nt, mj.x);
+            if (p != RT_INVALID_ID)
+            {
+                if (ANY) return 0u;
+                prim = __float_as_uint(mi.w) + p; bu = u; bv = v; bt = t; t_max = t;
+            }
+        }
+        bool found = false;
+        while (sp > 0) { --sp; if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; } }
+        if (!found) return prim;
+    }
+}
+
 // The traversal call of every persistent kernel, for the kernel's staging mode (stage_bvh): ray (a, b) = (origin, -), (dir, t_max).
-// PIN (trace_fast) is applied to the staged modes only.
-template <bool ANY, bool COUNT, int SMEM, bool PIN>
-__device__ __forceinline__ uint32_t trace_staged(const DevScene& sc, int mode, const float4* s_bvh, float4 a, float4 b,
+// PIN (trace_fast) is applied to the staged modes only.  RT_SMEM_INST: sc is a DevInstScene.
+template <bool ANY, bool COUNT, int SMEM, bool PIN, class Scene>
+__device__ __forceinline__ uint32_t trace_staged(const Scene& sc, int mode, const float4* s_bvh, float4 a, float4 b,
                                                  float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
 {
+    if constexpr (SMEM == RT_SMEM_INST) return trace_instanced<ANY, COUNT>(sc, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    else {
     if (SMEM == 1 || SMEM == 3) return trace_fast<ANY, COUNT, SMEM, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
     if (SMEM == 2) return trace_fast<ANY, COUNT, 2, PIN>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
     return trace<ANY, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    }
 }

@@ -155,6 +155,26 @@ void CUDAPathTraceIntegrator::UpdateTriangles(const Triangle* triangles, size_t 
     Check(rt_update_triangles(ctx_, triangles, count), "UpdateTriangles");
 }
 
+void CUDAPathTraceIntegrator::UploadInstancedScene(Scene const& shared, const RtTriangle* triangles, size_t n_triangles,
+                                                   const RtLinearBVHNode* nodes, size_t n_nodes, const RtMeshDesc* meshes, std::uint32_t n_meshes)
+{
+    RtSceneDesc d = {};
+    d.triangles = triangles;                            d.n_triangles = n_triangles;
+    d.nodes = nodes;                                    d.n_nodes = n_nodes;
+    d.materials = shared.GetMaterials().data();         d.n_materials = shared.GetMaterials().size();
+    d.lights = shared.GetLights().data();               d.n_lights = shared.GetLights().size();
+    d.textures = shared.GetTextures().data();           d.n_textures = shared.GetTextures().size();
+    d.texture_data = shared.GetTextureData().data();    d.n_texture_data = shared.GetTextureData().size();
+    d.env_image = shared.GetEnvImage().data.data();     d.env_width = shared.GetEnvImage().width; d.env_height = shared.GetEnvImage().height;
+    d.scene_info = shared.GetSceneInfo();
+    Check(rt_upload_instanced_scene(ctx_, &d, meshes, n_meshes), "UploadInstancedScene");
+}
+
+void CUDAPathTraceIntegrator::SetInstances(const RtInstance* instances, std::uint32_t count)
+{
+    Check(rt_set_instances(ctx_, instances, count), "SetInstances");
+}
+
 std::uint64_t CUDAPathTraceIntegrator::RebuildBvh(BvhBuild build)
 {
     std::uint64_t n_nodes = 0;

@@ -107,6 +107,12 @@ public:
     // triangles, built on the device, when a refit no longer traces well; returns the new node count (2n - 1).  Triangle ids do
     // not change.  No reset, as above.
     std::uint64_t RebuildBvh(BvhBuild build = BvhBuild::kLinear);
+    // instanced scene (rt_upload_instanced_scene): the meshes' triangles (each mesh in its own leaf order) and nodes (each mesh's
+    // own array), concatenated, with the materials, lights, textures and environment of `shared`; replaces the scene.  Place the
+    // meshes with SetInstances (rt_set_instances: the whole list; no reset, as for UpdateTriangles).
+    void UploadInstancedScene(Scene const& shared, const RtTriangle* triangles, size_t n_triangles, const RtLinearBVHNode* nodes,
+                              size_t n_nodes, const RtMeshDesc* meshes, std::uint32_t n_meshes);
+    void SetInstances(const RtInstance* instances, std::uint32_t count);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

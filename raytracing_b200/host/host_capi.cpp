@@ -213,6 +213,17 @@ int rth_render_update_triangles(void* h, const RtTriangle* triangles, size_t cou
     try { ((RenderHandle*)h)->render->UpdateTriangles(reinterpret_cast<const Triangle*>(triangles), count); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_upload_instanced_scene(void* h, const RtTriangle* triangles, size_t n_triangles, const RtLinearBVHNode* nodes, size_t n_nodes,
+                                      const RtMeshDesc* meshes, std::uint32_t n_meshes)
+{
+    try { ((RenderHandle*)h)->render->UploadInstancedScene(triangles, n_triangles, nodes, n_nodes, meshes, n_meshes); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
+int rth_render_set_instances(void* h, const RtInstance* instances, std::uint32_t count)
+{
+    try { ((RenderHandle*)h)->render->SetInstances(instances, count); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_rebuild_bvh(void* h, std::uint64_t* n_nodes)
 {
     try { *n_nodes = ((RenderHandle*)h)->render->RebuildBvh(); return 0; }

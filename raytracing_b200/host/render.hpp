@@ -62,6 +62,14 @@ public:
     // Keeps the accumulation, as above
     using BvhBuild = CUDAPathTraceIntegrator::BvhBuild;
     std::uint64_t RebuildBvh(BvhBuild build = BvhBuild::kLinear) { return Cuda().RebuildBvh(build); }
+    // instanced scene (CUDAPathTraceIntegrator::UploadInstancedScene / SetInstances): shared meshes in place of the scene's
+    // triangles, with the scene's materials, lights and environment; then the instance list
+    void UploadInstancedScene(const RtTriangle* triangles, size_t n_triangles, const RtLinearBVHNode* nodes, size_t n_nodes,
+                              const RtMeshDesc* meshes, std::uint32_t n_meshes)
+    {
+        Cuda().UploadInstancedScene(scene_, triangles, n_triangles, nodes, n_nodes, meshes, n_meshes);
+    }
+    void SetInstances(const RtInstance* instances, std::uint32_t count) { Cuda().SetInstances(instances, count); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

@@ -51,6 +51,8 @@ def load_library():
     L.rth_render_set_light_selection.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float]
     L.rth_render_update_triangles.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.rth_render_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    L.rth_render_upload_instanced_scene.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32]
+    L.rth_render_set_instances.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.rth_render_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
@@ -254,6 +256,30 @@ class HostRender:
         on the device.  Keeps the accumulation (request_reset() starts over)."""
         t = np.ascontiguousarray(triangles, dtype=TRIANGLE_DT)
         if self.L.rth_render_update_triangles(self.h, t.ctypes.data, t.shape[0]) != 0:
+            raise _err(self.L)
+
+    def upload_instanced_scene(self, meshes):
+        """Render::UploadInstancedScene: meshes = a list of dicts with "triangles" (leaf order) and "nodes" (the mesh's own array);
+        the scene's materials, lights and environment are shared."""
+        tris = np.concatenate([np.ascontiguousarray(m["triangles"], dtype=TRIANGLE_DT) for m in meshes])
+        nodes = np.concatenate([np.ascontiguousarray(m["nodes"], dtype=NODE_DT) for m in meshes])
+        desc = np.zeros((len(meshes), 4), dtype="<u8")
+        t0 = n0 = 0
+        for k, m in enumerate(meshes):
+            desc[k] = (t0, len(m["triangles"]), n0, len(m["nodes"]))
+            t0 += len(m["triangles"]); n0 += len(m["nodes"])
+        if self.L.rth_render_upload_instanced_scene(self.h, tris.ctypes.data, len(tris), nodes.ctypes.data, len(nodes), desc.ctypes.data,
+                                                    len(meshes)) != 0:
+            raise _err(self.L)
+
+    def set_instances(self, mesh_ids, transforms):
+        """Render::SetInstances: mesh_ids[i] placed by the row-major 3x4 transforms[i]."""
+        from .capi import INSTANCE_DT
+        ids = np.ascontiguousarray(mesh_ids, dtype="<u4").reshape(-1)
+        rec = np.zeros(len(ids), dtype=INSTANCE_DT)
+        rec["object_to_world"] = np.ascontiguousarray(transforms, dtype="<f4").reshape(-1, 12)
+        rec["mesh"] = ids
+        if self.L.rth_render_set_instances(self.h, rec.ctypes.data if len(rec) else None, len(rec)) != 0:
             raise _err(self.L)
 
     def rebuild_bvh(self, method="linear"):

@@ -40,20 +40,25 @@ def replicate(base_triangles: np.ndarray, copies: int = 183, grid: int = 14, see
         for j, v in enumerate(("v1", "v2", "v3")):
             blk[v]["position"][:, :3] = p[:, j].astype(np.float32)
             blk[v]["normal"][:, :3] = n[:, j].astype(np.float32)
+    bounds = _field_ground(out[copies * len(t):] if ground else None, lo, hi, pitch, copies, grid, t["mtlIndex"][0])
+    return out, bounds
+
+
+def _field_ground(g, lo, hi, pitch, copies, grid, mtl):
+    """The field's bounds (xmin, xmax, ymin, ymax, zmax); writes the ground quad into g (2 triangles) unless g is None."""
     rows = (copies + grid - 1) // grid
     half = pitch * 0.5
     bounds = (-half, (min(copies, grid) - 1) * pitch + half, -half, (rows - 1) * pitch + half, float(hi[2]))
-    if ground:
+    if g is not None:
         gx0, gx1, gy0, gy1 = bounds[0] - pitch, bounds[1] + pitch, bounds[2] - pitch, bounds[3] + pitch
         gz = float(lo[2]) - 0.01 * float(hi[2] - lo[2])           # just below the lowest vertex of the models
         corners = np.array([[gx0, gy0, gz], [gx1, gy0, gz], [gx1, gy1, gz], [gx0, gy1, gz]], dtype=np.float32)
-        g = out[copies * len(t):]
         for tri, idx in zip(g, ((0, 1, 2), (0, 2, 3))):               # counter-clockwise seen from above: front face up
             for v, k in zip(("v1", "v2", "v3"), idx):
                 tri[v]["position"][:3] = corners[k]
                 tri[v]["normal"][:3] = (0.0, 0.0, 1.0)
-        g["mtlIndex"] = t["mtlIndex"][0]
-    return out, bounds
+        g["mtlIndex"] = mtl
+    return bounds
 
 
 def field_camera(width: int, height: int, bounds, pitch_angle: float = 2.2689) -> np.ndarray:
@@ -83,3 +88,36 @@ def bistro_scale_scene(base_scene: dict, copies: int = 183, width: int = 1920, h
     scene["camera_pose"] = field_camera(width, height, bounds)
     scene["bvh_depth"] = depth
     return scene
+
+
+
+def instanced_field(base_scene: dict, copies: int = 183, grid: int = 14, seed: int = 1234, width: int = 1920, height: int = 1080) -> dict:
+    """replicate()'s field as an instanced scene (Context.upload_instanced_scene / set_instances): the base model as mesh 0, the
+    ground quad as mesh 1, and copies + 1 instances with replicate()'s placements (the rotation about Z and the grid cell as one
+    matrix rounded to float; the ground at identity).  Each mesh's BVH comes from the host builder.  Keys: meshes, shared (the
+    base scene, for its materials, lights, textures and environment), mesh_ids, transforms (n, 3, 4), camera_pose."""
+    from . import hostapi
+    t = np.ascontiguousarray(base_scene["triangles"], dtype=TRIANGLE_DT)
+    pos = np.stack([t[v]["position"][:, :3] for v in ("v1", "v2", "v3")], axis=1).astype(np.float64)
+    lo, hi = pos.reshape(-1, 3).min(0), pos.reshape(-1, 3).max(0)
+    centre = (lo + hi) * 0.5
+    pitch = 1.1 * max(hi[0] - lo[0], hi[1] - lo[1])
+    ground = np.zeros(2, dtype=TRIANGLE_DT)
+    bounds = _field_ground(ground, lo, hi, pitch, copies, grid, t["mtlIndex"][0])
+    meshes = []
+    for tris in (t, ground):
+        ordered, nodes, _ = hostapi.build_bvh(tris)
+        meshes.append({"triangles": ordered, "nodes": nodes})
+    transforms = np.zeros((copies + 1, 3, 4), dtype=np.float32)
+    x = seed
+    for k in range(copies):
+        x = (1103515245 * x + 12345) & 0xFFFFFFFF
+        ang = (x / 4294967296.0) * 2.0 * math.pi
+        c, s = math.cos(ang), math.sin(ang)
+        rot = np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
+        cell = np.array([(k % grid) * pitch, (k // grid) * pitch, 0.0])
+        transforms[k, :, :3] = rot
+        transforms[k, :, 3] = cell - rot @ (centre * [1, 1, 0])
+    transforms[copies, :, :3] = np.eye(3)
+    return {"meshes": meshes, "shared": base_scene, "mesh_ids": np.array([0] * copies + [1], dtype="<u4"), "transforms": transforms,
+            "camera_pose": field_camera(width, height, bounds)}

@@ -1,0 +1,105 @@
+"""
+Instanced against flattened Synthetic10M (C5): replicate()'s 183 rotated ShaderBalls copies and the ground quad, once as 10 M
+flattened triangles under the host SAH tree (bench.py's secondary workload) and once as two meshes and 184 instances
+(synthetic.instanced_field, rt_upload_instanced_scene / rt_set_instances).
+
+  python tools/instance_probe.py [--width 1920 --height 1080 --bounces 8 --frames 20 --warmup 5] [--out FILE]
+
+Per arm: ms per frame (rt_reset + rt_integrate) from CUDA events on the render stream after --warmup frames, the device memory the
+scene holds (free memory before the context's upload minus after it, cudaMemGetInfo), and for the instanced arm the cost of one
+rt_set_instances with the 184 instances (host clock around 50 calls, each followed by rt_sync, warm buffer).  Prints one JSON line
+per arm, headed by the GPU's name and power limit read in the same run.  Frames of the two arms are not equal: the instanced matrices
+round differently from the flattened vertices (tests/test_instancing_cpu.py bounds the difference).
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from raytracing_b200 import capi, scene_io, synthetic  # noqa: E402
+
+
+def gpu_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
+
+
+def timed_frames(c, bounces, frames, warmup):
+    import torch
+    for _ in range(warmup):
+        c.reset(); c.integrate(bounces)
+    c.sync()
+    stream = torch.cuda.ExternalStream(c.stream_handle())
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record(stream)
+    for _ in range(frames):
+        c.reset(); c.integrate(bounces)
+    b.record(stream)
+    b.synchronize()
+    return a.elapsed_time(b) / frames
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--width", type=int, default=1920)
+    ap.add_argument("--height", type=int, default=1080)
+    ap.add_argument("--bounces", type=int, default=8)
+    ap.add_argument("--frames", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--copies", type=int, default=183)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    import torch
+    torch.cuda.init()
+    base = scene_io.load_scene("ShaderBalls")
+    lines = [{"gpu": gpu_info()}]
+
+    def free():
+        torch.cuda.synchronize()
+        return torch.cuda.mem_get_info()[0]
+
+    fld = synthetic.instanced_field(base, copies=args.copies, width=args.width, height=args.height)
+    cam = fld["camera_pose"]
+    c = capi.Context(args.width, args.height)
+    c.set_camera(cam)
+    f0 = free()
+    c.upload_instanced_scene(fld["meshes"], fld["shared"])
+    c.set_instances(fld["mesh_ids"], fld["transforms"])
+    c.sync()
+    mem = f0 - free()
+    ms = timed_frames(c, args.bounces, args.frames, args.warmup)
+    t = time.perf_counter()
+    for _ in range(50):
+        c.set_instances(fld["mesh_ids"], fld["transforms"]); c.sync()
+    set_ms = (time.perf_counter() - t) * 1e3 / 50
+    c.destroy()
+    lines.append({"arm": "instanced", "instances": len(fld["mesh_ids"]), "mesh_triangles": [len(m["triangles"]) for m in fld["meshes"]],
+                  "ms_per_frame": ms, "scene_device_bytes": int(mem), "set_instances_ms": set_ms,
+                  "frame": f"{args.width}x{args.height}x{args.bounces}"})
+
+    flat = synthetic.bistro_scale_scene(base, copies=args.copies, width=args.width, height=args.height)
+    c = capi.Context(args.width, args.height)
+    c.set_camera(cam)
+    f0 = free()
+    c.upload_scene(flat)
+    c.sync()
+    mem = f0 - free()
+    ms = timed_frames(c, args.bounces, args.frames, args.warmup)
+    c.destroy()
+    lines.append({"arm": "flattened", "triangles": len(flat["triangles"]), "ms_per_frame": ms, "scene_device_bytes": int(mem),
+                  "frame": f"{args.width}x{args.height}x{args.bounces}"})
+    text = "\n".join(json.dumps(x) for x in lines)
+    print(text)
+    if args.out:
+        with open(args.out, "w") as f:
+            f.write(text + "\n")
+
+
+if __name__ == "__main__":
+    main()
