@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                     const uint32_t n_alive = s.ext_n[in];
                     for (uint32_t k = threadIdx.x; k < n_alive; k += blockDim.x)
                     {
-                        const uint32_t li = local_index(p, __float_as_uint(q.A[in][base + k].w));
+                        const uint32_t li = local_index(p, __float_as_uint(q.B[in][base + k].w));
                         p.gather[li] = radiance[li];
                     }
                 }
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                     float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                     if (hit) h = q.hitq[base + k];
                     uint32_t pixel;
-                    const bool ends = shade_hit_group<false, EMIT>(p, sc, aov, q, base, b, hit, h, __float_as_uint(h.w), radiance, &s.emit[in], &s.n_emissive, pixel);
+                    const bool ends = shade_hit_group<false, EMIT, false, EMIT>(p, sc, aov, q, base, b, hit, h, __float_as_uint(h.w), radiance, &s.emit[in], &s.n_emissive, pixel);
                     if (p.gather)
                     {   // paths that end at this hit (no continuation ray): final once their shadow ray is accumulated in T(b+1)
                         const unsigned dmask = __ballot_sync(0xffffffffu, ends);
@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame(FrameParams p
                         }
                     }
                 }
-                else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, base + q.missq[base + at - hit_span + lane], radiance);
+                else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, b, base + q.missq[base + at - hit_span + lane], radiance);
             }
             __syncthreads();
             if (threadIdx.x == 0)
@@ -255,7 +255,7 @@ __device__ __forceinline__ bool shade_hit_regen(const FrameParams& p, const DevS
     if (hit)
     {
         const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
-        pixel = __float_as_uint(a.w); state = __float_as_uint(c.w); bounce = state & 0xFFu;
+        pixel = __float_as_uint(b.w); state = __float_as_uint(c.w); bounce = state & 0xFFu;
         shade_hit(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), 0.0f, __float_as_uint(h.z), h.x, h.y, state >> 8, so);
         li = local_index(p, pixel);
         if (so.emissive) add_radiance(radiance, li, so.emission_add);
@@ -286,8 +286,8 @@ __device__ __forceinline__ bool shade_hit_regen(const FrameParams& p, const DevS
     {
         const int out = in ^ 1;
         const uint32_t ni = base + (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
-        q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
-        q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
+        q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, 0.0f);
+        q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, __uint_as_float(pixel));
         q.C[out][ni] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, __uint_as_float(state + 1u));
     }
     return hit && !cont;
@@ -399,9 +399,9 @@ __global__ void __launch_bounds__(RT_FRAME_MAX_THREADS, 1) k_frame_regen(FramePa
                     if (miss)
                     {
                         const uint32_t slot = base + q.missq[base + k];
-                        const float4 a = q.A[in][slot], b = q.B[in][slot], c = q.C[in][slot];
+                        const float4 b = q.B[in][slot], c = q.C[in][slot];
                         const f3 sky = p.white_furnace ? splat(0.5f) : sample_sky(sc, mk3(b));
-                        li = local_index(p, __float_as_uint(a.w)); state = __float_as_uint(c.w);
+                        li = local_index(p, __float_as_uint(b.w)); state = __float_as_uint(c.w);
                         const float4 rr = add_radiance(radiance, li, sky * mk3(c));
                         if (p.gather && (state >> 8) + 1u == n_samples) p.gather[li] = rr;
                     }

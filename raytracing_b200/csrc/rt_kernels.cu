@@ -107,12 +107,15 @@ struct ShadeOut
 // kernels/cl/miss.cl:41-77: radiance += sky * throughput, for the ray in slot `slot` of ray queue `in`.
 // EMIT (the sampled-light instance, shade_hit): with an environment table, a BSDF-sampled ray (C.w = p_b > 0) adds
 // (sky * throughput) * mis(p_b, p_v(dir)), weighted against the environment strategy that could have drawn its direction.
+// Plane A is not read: a miss needs the direction and the pixel (B) and the throughput (C); at bounce 0 the throughput of every
+// path is (1, 1, 1) with C.w = 0, so C is not read either.
 template <bool EMIT = false>
-__device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams& p, const Queues& q, int in, uint32_t slot, float4* radiance)
+__device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams& p, const Queues& q, uint32_t bounce, uint32_t slot, float4* radiance)
 {
-    const float4 a = q.A[in][slot], b = q.B[in][slot], c = q.C[in][slot];
+    const int in = bounce & 1;
+    const float4 b = q.B[in][slot], c = bounce == 0 ? make_float4(1.0f, 1.0f, 1.0f, 0.0f) : q.C[in][slot];
     f3 sky = p.white_furnace ? splat(0.5f) : sample_sky(sc, mk3(b));
-    uint32_t li = local_index(p, __float_as_uint(a.w));
+    uint32_t li = local_index(p, __float_as_uint(b.w));
     f3 add = sky * mk3(c);
     if (EMIT && c.w > 0.0f && sc.env_pdf)
         add = add * mis_power(c.w, rtenv::pdf_dir(sc.env_pdf, sc.env_w, sc.env_h, b.x, b.y, b.z));
@@ -364,17 +367,15 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
 // kernels and the CTA's region of every queue for k_frame.  The slot and statistics counters are global memory (DevCounters)
 // for the per-phase kernels and shared memory (CtaFrame) for k_frame.
 
-// RayGeneration (raygeneration.cl:65-139): the primary ray (a, b) of local pixel li for sample `sample_idx`, stored in slot `slot`
-// of ray queue `in` with `state` in C.w (the path state of the regenerating frame kernel; 0 everywhere else)
-__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, int in, uint32_t slot, uint32_t li,
-                                            uint32_t sample_idx, uint32_t state, float4& a, float4& b)
+// RayGeneration (raygeneration.cl:65-139): the primary ray (a, b) of local pixel li for sample `sample_idx` in queue-plane layout
+// (a = origin, b = direction + packed pixel); clears the pixel's AOVs
+__device__ __forceinline__ void make_primary_ray(const FrameParams& p, const AovParams& aov, uint32_t li, uint32_t sample_idx, float4& a, float4& b)
 {
     const uint32_t px = li % p.width, py = (li / p.width) * p.world + p.rank;
     f3 o, d;
     generate_primary_ray(p.dyn->raygen, py * p.width + px, px, py, sample_idx, o, d);
-    a = make_float4(o.x, o.y, o.z, __uint_as_float(pack_pixel(px, py)));
-    b = make_float4(d.x, d.y, d.z, RT_MAX_RENDER_DIST);
-    q.A[in][slot] = a; q.B[in][slot] = b; q.C[in][slot] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(state));
+    a = make_float4(o.x, o.y, o.z, 0.0f);
+    b = make_float4(d.x, d.y, d.z, __uint_as_float(pack_pixel(px, py)));
     if (aov.enabled)
     {   // raygeneration.cl:129-133
         aov.albedo[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -382,6 +383,15 @@ __device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& 
         aov.normal[li] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         aov.velocity[li] = make_float2(0.0f, 0.0f);
     }
+}
+
+// make_primary_ray, stored in slot `slot` of ray queue `in` with throughput 1 and `state` in C.w (the path state of the
+// regenerating frame kernel; 0 everywhere else)
+__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, int in, uint32_t slot, uint32_t li,
+                                            uint32_t sample_idx, uint32_t state, float4& a, float4& b)
+{
+    make_primary_ray(p, aov, li, sample_idx, a, b);
+    q.A[in][slot] = a; q.B[in][slot] = b; q.C[in][slot] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(state));
 }
 
 // Closest hit of the ray (a, b) of entry i (live lanes) and hit/miss stream compaction: __ballot + __popc give every lane its
@@ -451,7 +461,9 @@ __device__ __forceinline__ uint32_t ray_key(f3 o, f3 d, float4 mid)
 // of both queues (shadow rays in the low word, continuation rays in the high).  With STAGE the continuation rays go to the CTA's
 // staging area `st` instead (flush_continuations writes them out and counts them) and the atomic reserves shadow-ray slots only.
 // Returns whether the lane's path ends at this hit (no continuation ray); `pixel` is the packed pixel of the ray.
-template <bool STAGE = false, bool EMIT = false, bool INST = false>
+// ALL_PLANES (the one-kernel frame with EMIT, whose primary rays are stored whole): read planes A and C of every hit; at its 64
+// registers the two uniform branches below cost it spills.
+template <bool STAGE = false, bool EMIT = false, bool INST = false, bool ALL_PLANES = false>
 __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const SceneOf<INST>& sc, const AovParams& aov, const Queues& q, uint32_t base, uint32_t bounce,
                                                 bool hit, float4 h, uint32_t i, float4* radiance, unsigned long long* emit, uint32_t* n_emissive, uint32_t& pixel,
                                                 ContStage* st = nullptr)
@@ -461,9 +473,13 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
     so.emissive = so.spawn_next = so.spawn_shadow = false;
     pixel = 0;
     if (hit)
-    {
-        const float4 a = q.A[in][base + i], b = q.B[in][base + i], c = q.C[in][base + i];
-        pixel = __float_as_uint(a.w);
+    {   // plane A (the origin) only where shade_hit reads it: the depth AOV of bounce 0 and, with EMIT, the MIS weight of an emitter
+        // hit by a BSDF-sampled ray (never at bounce 0: C.w of a primary ray is 0).  Plane C is (1, 1, 1, 0) at bounce 0.
+        const bool origin = ALL_PLANES || (bounce == 0 ? aov.enabled != 0 : EMIT);
+        const float4 b = q.B[in][base + i];
+        const float4 c = bounce == 0 && !ALL_PLANES ? make_float4(1.0f, 1.0f, 1.0f, 0.0f) : q.C[in][base + i];
+        const float4 a = origin ? q.A[in][base + i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        pixel = __float_as_uint(b.w);
         shade_hit<EMIT, INST>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, 0u, so);
         if (so.emissive) add_radiance(radiance, local_index(p, pixel), so.emission_add);
     }
@@ -500,8 +516,8 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
         }
         if (sn)
         {
-            st->A[j] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
-            st->B[j] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
+            st->A[j] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, 0.0f);
+            st->B[j] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, __uint_as_float(pixel));
             st->C[j] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, so.n_pdf);
             const uint32_t key = ray_key(so.n_origin, so.n_dir, st->mid);
             st->key[j] = (uint8_t)key;
@@ -511,8 +527,8 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
     else if (sn)
     {
         const uint32_t ni = base + (uint32_t)(slot >> 32) + __popc(nmask & lt_mask);
-        q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, __uint_as_float(pixel));
-        q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, RT_MAX_RENDER_DIST);
+        q.A[out][ni] = make_float4(so.n_origin.x, so.n_origin.y, so.n_origin.z, 0.0f);
+        q.B[out][ni] = make_float4(so.n_dir.x, so.n_dir.y, so.n_dir.z, __uint_as_float(pixel));
         q.C[out][ni] = make_float4(so.n_throughput.x, so.n_throughput.y, so.n_throughput.z, so.n_pdf);
     }
     return hit && !so.spawn_next;
@@ -551,8 +567,8 @@ __global__ void __launch_bounds__(256) k_intersect(FrameParams p, SceneOf<INST> 
         float4 a = q.A[in][i], b = q.B[in][i];
         float bu = 0.0f, bv = 0.0f, bt = 0.0f;
         uint32_t prim;
-        if constexpr (INST) prim = trace_instanced<false, COUNT>(sc, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-        else prim = trace<false, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+        if constexpr (INST) prim = trace_instanced<false, COUNT>(sc, mk3(a), mk3(b), 0.0f, RT_MAX_RENDER_DIST, bu, bv, bt, nv, nt);
+        else prim = trace<false, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, RT_MAX_RENDER_DIST, bu, bv, bt, nv, nt);
         q.hits[i] = make_float4(bu, bv, __uint_as_float(prim), bt);
     }
     if (COUNT) { warp_sum64(&ctr->nodes_ext[bounce], nv); warp_sum64(&ctr->tris_ext[bounce], nt); }
@@ -568,7 +584,7 @@ __global__ void __launch_bounds__(256) k_shade_miss(FrameParams p, DevScene sc, 
     if (i < n)
     {
         miss = __float_as_uint(q.hits[i].z) == RT_INVALID_ID;
-        if (miss) shade_miss<EMIT>(sc, p, q, bounce & 1, i, radiance);
+        if (miss) shade_miss<EMIT>(sc, p, q, bounce, i, radiance);
     }
     warp_count(&ctr->hm[bounce].miss, miss);
 }
@@ -677,6 +693,36 @@ __global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_closest(FrameParam
     closest_phase<COUNT, SMEM>(sc, mode, q, ctr, bounce, s_bvh);
 }
 
+// Bounce 0 of the per-phase frame: k_raygen and k_trace_closest(0) in one kernel.  Entry i is generated in registers (local pixel
+// i, or active[i] with adaptive sampling), traced, and only the planes the bounce-0 shading pass reads are stored: B (direction,
+// pixel), and A (origin) when the AOVs are on.  That pass takes C as (1, 1, 1, 0).  Sets n_primary as k_raygen does.
+template <bool COUNT, int SMEM>
+__global__ void __launch_bounds__(256, RT_MINB_TRACE) k_trace_primary(FrameParams p, SceneOf<SMEM == RT_SMEM_INST> sc, int mode, Queues q, DevCounters* ctr,
+                                                                      AovParams aov)
+{
+    extern __shared__ __align__(128) float4 s_bvh[];
+    __shared__ uint64_t s_mbar;
+    stage_bvh<SMEM>(s_bvh, sc, &s_mbar);
+    pdl_wait(); pdl_launch_dependents();
+    const uint32_t n = p.active ? *p.n_active : p.n_local;
+    if (blockIdx.x == 0 && threadIdx.x == 0) ctr->n_primary = n;
+    uint32_t nv = 0, nt = 0;
+    for (uint32_t at; (at = warp_grab(&ctr->work_ext[0])) < n;)
+    {
+        const uint32_t i = at + (threadIdx.x & 31);
+        const bool live = i < n;
+        float4 a, b;
+        if (live)
+        {
+            make_primary_ray(p, aov, p.active ? p.active[i] : i, p.dyn->sample_idx, a, b);
+            q.B[0][i] = b;
+            if (aov.enabled) q.A[0][i] = a;
+        }
+        closest_group<COUNT, SMEM, false>(sc, mode, s_bvh, q, 0, i, live, a, b, (unsigned long long*)&ctr->hm[0], nv, nt);
+    }
+    if (COUNT) { warp_sum64(&ctr->nodes_ext[0], nv); warp_sum64(&ctr->tris_ext[0], nt); }
+}
+
 // Closest-hit traversal of bounce b and the shadow pass of bounce b-1 in ONE persistent kernel (RT_OPT_OVERLAP = 2, the
 // default): the two are independent (the shadow pass only shares the radiance buffer with LATER shading passes), every
 // warp drains the extension queue and then the shadow queue, so the short shadow rays fill the tail of the long
@@ -759,7 +805,7 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 uint32_t pixel;
                 shade_hit_group<false, EMIT, INST>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel);
             }
-            else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, bounce & 1, q.missq[at - hit_span + lane], radiance);
+            else if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, bounce, q.missq[at - hit_span + lane], radiance);
         }
         return;
     }
@@ -784,13 +830,13 @@ __global__ void __launch_bounds__(256, RT_MINB_SHADE) k_shade_queues(FrameParams
                 uint32_t pixel;
                 shade_hit_group<true, EMIT, INST>(p, sc, aov, q, 0, bounce, hit, h, __float_as_uint(h.w), radiance, (unsigned long long*)&ctr->emit[bounce], &ctr->n_emissive[bounce], pixel, &st);
             }
-            else if (g - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, q.missq[g - hit_span + lane], radiance);
+            else if (g - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, bounce, q.missq[g - hit_span + lane], radiance);
         }
         if (at < hit_span) flush_continuations(st, q, in ^ 1, &ctr->emit[bounce].next);
         if (at + batch >= hit_span) break;                      // every later entry is a miss
     }
     for (uint32_t at; (at = warp_grab(&ctr->work_shade[bounce])) < total;)
-        if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, in, q.missq[at - hit_span + lane], radiance);
+        if (at - hit_span + lane < n_miss) shade_miss<EMIT>(sc, p, q, bounce, q.missq[at - hit_span + lane], radiance);
 }
 
 #include "rt_frame_kernel.cuh"
@@ -1116,8 +1162,8 @@ __global__ void k_unpack_rays(const float4* A, const float4* B, const uint32_t* 
     if (i >= *count) return;
     float4 a = A[i], b = B[i];
     rays[i].origin = RtFloat3{ a.x, a.y, a.z, 0.0f };
-    rays[i].direction = RtFloat3{ b.x, b.y, b.z, b.w };
-    uint32_t pxy = __float_as_uint(a.w);
+    rays[i].direction = RtFloat3{ b.x, b.y, b.z, RT_MAX_RENDER_DIST };      // every extension ray's t_max
+    uint32_t pxy = __float_as_uint(b.w);
     pixels[i] = (pxy >> 16) * width + (pxy & 0xFFFFu);
 }
 
@@ -1274,6 +1320,7 @@ struct rt_ctx
     uint32_t sample_count = 0;
     uint32_t cur_bounce = 0;
     bool frame_started = false;
+    bool primary_fused = false;    // the frame was begun without k_raygen: rt_extend_shade(0) generates its primary rays (k_trace_primary)
     uint64_t launches = 0;
 
     // kernel timing
@@ -2759,9 +2806,10 @@ int rt_read_active_pixels(rt_ctx* c, uint32_t* n_active)
     return RT_OK;
 }
 
-int rt_generate_rays(rt_ctx* c)
+// A frame starts on one device: counters cleared, the frame constants set, and with `raygen` the full primary-ray queue (k_raygen).
+// Without it the bounce-0 traversal of rt_extend_shade generates the primary rays itself (k_trace_primary).
+static int begin_frame(rt_ctx* c, bool raygen)
 {
-    RT_CHECK_CTX(c); RT_FANOUT(c, rt_generate_rays(k));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; }
     int rc = require_ready(c); if (rc) return rc;
     RT_CUDA(c, cudaSetDevice(c->device));
@@ -2773,10 +2821,17 @@ int rt_generate_rays(rt_ctx* c)
         k_set_frame<<<1, 1, 0, c->stream>>>(c->d_dyn, dyn);
         ++c->launches;
     }
-    k_raygen<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->q, c->counters, aov_params(c));
+    if (raygen) k_raygen<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->q, c->counters, aov_params(c));
     note_frame_aovs(c);
     c->frame_started = true;
-    return post_launch(c, "k_raygen");
+    c->primary_fused = !raygen;
+    return post_launch(c, raygen ? "k_raygen" : "k_set_frame");
+}
+
+int rt_generate_rays(rt_ctx* c)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_generate_rays(k));
+    return begin_frame(c, true);
 }
 
 #define RT_BOUNCE_CHECK(c, b)                                                                                   \
@@ -2894,6 +2949,19 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
         });
         int rc = post_launch(c, "k_trace_both"); if (rc) return rc;
     }
+    else if (bounce == 0 && c->primary_fused)
+    {   // the frame's primary rays are generated here (begin_frame without k_raygen)
+        c->primary_fused = false;
+        TimedLaunch t(c, RT_K_TRACE_CLOSEST);
+        if (c->count_traversal && c->instanced)
+            k_trace_primary<true, RT_SMEM_INST><<<RT_PGRID(c, (k_trace_primary<true, RT_SMEM_INST>), 0), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, aov_params(c));
+        else if (c->count_traversal) k_trace_primary<true, 0><<<RT_PGRID(c, (k_trace_primary<true, 0>), 0), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, aov_params(c));
+        else launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
+            auto* k = k_trace_primary<false, smem.value>;
+            launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, aov_params(c));
+        });
+        int rc = post_launch(c, "k_trace_primary"); if (rc) return rc;
+    }
     else
     {
         TimedLaunch t(c, RT_K_TRACE_CLOSEST);
@@ -2971,7 +3039,7 @@ int rt_shadow_accumulate(rt_ctx* c, uint32_t bounce)
 
 static int integrate_body(rt_ctx* c, uint32_t max_bounces)
 {
-    int rc = rt_generate_rays(c); if (rc) return rc;
+    int rc = begin_frame(c, false); if (rc) return rc;      // rt_extend_shade(0) generates the primary rays
     for (uint32_t b = 0; b <= max_bounces; ++b)          // inclusive, integrator.cpp:37
     {
         if ((rc = rt_extend_shade(c, b))) return rc;
@@ -2997,7 +3065,7 @@ static int capture_frame_graph(rt_ctx* c, uint32_t max_bounces)
     c->graph_launches = c->launches - saved_launches;
     c->sample_count = saved_samples; c->cur_bounce = saved_bounce; c->launches = saved_launches; c->frame_started = saved_started;
     c->aov_ready = saved_aov_ready; c->ad_fresh = saved_ad_fresh;
-    c->shadow_pending = false; c->shadow_deferred = false;
+    c->shadow_pending = false; c->shadow_deferred = false; c->primary_fused = false;
     if (rc) return rc;
     if (e != cudaSuccess) RT_FAIL(c, RT_ERR_CUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(e));
     size_t n_nodes = 0;
@@ -3450,7 +3518,7 @@ int rt_read_hits(rt_ctx* c, uint32_t bounce, RtHit* hits, uint32_t* pixels, uint
     if (pixels && n)
     {
         std::vector<float4> a(n);
-        RT_CUDA(c, cudaMemcpy(a.data(), c->q.A[bounce & 1], (size_t)n * 16, cudaMemcpyDeviceToHost));
+        RT_CUDA(c, cudaMemcpy(a.data(), c->q.B[bounce & 1], (size_t)n * 16, cudaMemcpyDeviceToHost));     // B.w: the packed pixel
         for (uint32_t i = 0; i < n; ++i) { uint32_t pxy; memcpy(&pxy, &a[i].w, 4); pixels[i] = (pxy >> 16) * c->width + (pxy & 0xFFFFu); }
     }
     return RT_OK;

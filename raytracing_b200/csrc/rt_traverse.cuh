@@ -523,16 +523,18 @@ __device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o
     }
 }
 
-// The traversal call of every persistent kernel, for the kernel's staging mode (stage_bvh): ray (a, b) = (origin, -), (dir, t_max).
+// The traversal call of every persistent kernel, for the kernel's staging mode (stage_bvh): ray (a, b) = (origin, -), (dir, w).
+// A shadow ray (ANY) carries its t_max in b.w; an extension ray carries its pixel there, and its t_max is RT_MAX_RENDER_DIST.
 // PIN (trace_fast) is applied to the staged modes only.  RT_SMEM_INST: sc is a DevInstScene.
 template <bool ANY, bool COUNT, int SMEM, bool PIN, class Scene>
 __device__ __forceinline__ uint32_t trace_staged(const Scene& sc, int mode, const float4* s_bvh, float4 a, float4 b,
                                                  float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
 {
-    if constexpr (SMEM == RT_SMEM_INST) return trace_instanced<ANY, COUNT>(sc, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    const float t_max = ANY ? b.w : RT_MAX_RENDER_DIST;
+    if constexpr (SMEM == RT_SMEM_INST) return trace_instanced<ANY, COUNT>(sc, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
     else {
-    if (SMEM == 1 || SMEM == 3) return trace_fast<ANY, COUNT, SMEM, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-    if (SMEM == 2) return trace_fast<ANY, COUNT, 2, PIN>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-    return trace<ANY, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+    if (SMEM == 1 || SMEM == 3) return trace_fast<ANY, COUNT, SMEM, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
+    if (SMEM == 2) return trace_fast<ANY, COUNT, 2, PIN>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
+    return trace<ANY, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
     }
 }
