@@ -290,14 +290,19 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
             {   // the wide node at slot `cur` of this ray's table: 2..4 slots of (entry xyz, exit | exit yz, ref, count), in visiting order
                 // The children are tested last to first: each hit defers the one found before it, so the first child that hits
                 // is continued into and the other hit children are deferred in reverse order, with no per-child state kept.
+                // An any-hit ray tests them first to last instead and so walks the tree far to near: its t_max never changes,
+                // so every box test has the same outcome in any order and the ray reaches the same leaves, but a shadow ray
+                // that starts on a surface is usually stopped by what lies far from its origin (a wall, the ceiling), and
+                // the near subtrees, which hold the surface it leaves, are then never walked.
                 const float4* np = wnodes + (oct_at + (uint32_t)cur * 2u);
                 const uint32_t cnt = __float_as_uint(np[1].w);
                 bool found = false;
                 int next_ref = 0;
                 float next_lo = 0.0f;
 #pragma unroll
-                for (int j = 3; j >= 0; --j)
+                for (int k = 0; k < 4; ++k)
                 {
+                    const int j = ANY ? k : 3 - k;
                     if (j >= 2 && (uint32_t)j >= cnt) continue;
                     const float4 p = np[2 * j], q = np[2 * j + 1];
                     float lo, hi;

@@ -21,6 +21,7 @@
 
 #include "rt_types.h"
 #include "../raytracing_b200/csrc/rt_bvh_layout.h"
+#include "../raytracing_b200/csrc/rt_octant.h"
 
 namespace
 {
@@ -253,5 +254,175 @@ extern "C" int simt_model(const RtLinearBVHNode* nodes, uint32_t n_nodes, const 
     double n_node = 0, n_tri = 0;
     for (auto& v : ops) for (uint8_t op : v) { if (op == OP_NODE) ++n_node; else if (op != OP_LEAF_END) ++n_tri; }
     out[0] = slots; out[1] = work; out[2] = n_node; out[3] = n_tri;
+    return 0;
+}
+
+// ------------------------------------------------------------------ any-hit rays on the 4-wide octant tables (SMEM 3)
+// trace_fast<true, false, 3> walks the tables of its ray's octant (rt_octant.h: wide nodes of 2..4 slots, children tested last
+// to first, the first hit child continued into, the others kept as references on a 4-byte stack that is popped without a test).
+// A lane's walk is a state machine here because the postponed loop changes which step a lane takes next depending on the warp:
+//   variant 0  the while-while loop walking near to far: interior steps while any lane has an interior record, then the leaves of every lane
+//              that reached one, one triangle per slot, then the pop
+//   variant 1  postponed leaves: a lane that reaches a leaf with its pending slot empty keeps the leaf there and pops its next
+//              entry; with the slot full it stops.  The interior loop ends when no lane has an interior record, or when the vote of
+//              the lanes still in it finds at least `trigger` of them (0: all; -1: no vote) holding a leaf.  The leaf loop then runs every
+//              pending leaf; a lane whose leaf ends while it stands on another leaf takes that one in the same loop.
+//   variant 2  the while-while loop of variant 0 with the wide step walking far to near: the children are tested first to last
+//              and the last that hits is continued into (the order trace_fast<true, false, 3> uses)
+// Only rays that take the table walk are modelled (rt_oct_ray_ok, finite t_max); the others run the SMEM 1 loop in both builds.
+namespace
+{
+const int EMPTY = INT32_MIN;                                   // no interior or leaf reference left
+struct AnyLane
+{
+    const float* base; float o[3], d[3], inv[3], t_max;
+    int cur = EMPTY, pending = 0, sp = 0, stack[128];
+    bool live = false;
+};
+
+uint32_t fbits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+
+void pop(AnyLane& l) { l.cur = l.sp ? l.stack[--l.sp] : EMPTY; }
+
+void wide_step(AnyLane& l, bool far_first)
+{
+    const float* np = l.base + (size_t)l.cur * 8;
+    const uint32_t cnt = fbits(np[7]);
+    bool found = false; int next_ref = 0;
+    for (int k = 0; k < (int)cnt; ++k)
+    {
+        const int j = far_first ? k : (int)cnt - 1 - k;
+        const float* q = np + 8 * j;
+        float lo, hi;
+        rt_slab_ordered(q[0], q[1], q[2], q[3], q[4], q[5], l.o[0], l.o[1], l.o[2], l.inv[0], l.inv[1], l.inv[2], 0.0f, lo, hi);
+        if (rt_oct_min(hi, l.t_max) >= lo)
+        {
+            if (found) l.stack[l.sp++] = next_ref;
+            next_ref = (int)fbits(q[6]); found = true;
+        }
+    }
+    if (found) l.cur = next_ref; else pop(l);
+}
+
+// one triangle test of trace_fast: the exit stage (OP_TRI1..4), *hit and *last
+uint8_t tri_step(const float* tris, const AnyLane& l, uint32_t ti, bool* hit, bool* last)
+{
+    const float* q = tris + 12 * (size_t)ti;
+    *last = fbits(q[9]) != 0u; *hit = false;
+    V3 p1{ q[0], q[1], q[2] }, e1{ q[3], q[4], q[5] }, e2{ q[6], q[7], q[8] }, d{ l.d[0], l.d[1], l.d[2] }, o{ l.o[0], l.o[1], l.o[2] };
+    V3 pvec = cross(d, e2);
+    float det = dot(e1, pvec);
+    if (det < 1e-8f || -det > 1e-8f) return OP_TRI1;
+    float inv_det = 1.0f / det;
+    V3 tvec = o - p1;
+    float u = dot(tvec, pvec) * inv_det;
+    if (u < 0.0f || u > 1.0f) return OP_TRI2;
+    V3 qvec = cross(tvec, e1);
+    float v = dot(d, qvec) * inv_det;
+    if (v < 0.0f || u + v > 1.0f) return OP_TRI3;
+    float t = dot(e2, qvec) * inv_det;
+    *hit = !(t < 0.0f || t > l.t_max);
+    return OP_TRI4;
+}
+
+// costs: wide step, tri1..tri4, ray fetch, postponing overhead per interior step (postpone test + vote)
+Result simulate_any_warp(const float* tables, uint32_t n, const float* tris, int root_ref, const float* root_box, const float* rays,
+                         size_t first, size_t count, int variant, int trigger, const double* c, uint64_t* unoccluded)
+{
+    Result r; r.rays = count;
+    for (size_t b = first; b < first + count; b += 32)
+    {
+        AnyLane lane[32];
+        int m = (int)std::min<size_t>(32, first + count - b);
+        r.slots += c[5]; r.thread_work += c[5] * m;
+        for (int i = 0; i < m; ++i)
+        {
+            AnyLane& l = lane[i];
+            const float* ray = rays + 7 * (b + i);
+            for (int k = 0; k < 3; ++k) { l.o[k] = ray[k]; l.d[k] = ray[3 + k]; l.inv[k] = 1.0f / ray[3 + k]; }
+            l.t_max = ray[6];
+            if (!rt_oct_ray_ok(l.inv[0], l.inv[1], l.inv[2]) || l.t_max != l.t_max) continue;
+            l.base = tables + (size_t)rt_oct_octant(l.inv[0], l.inv[1], l.inv[2]) * 2 * n * 8;
+            float lo, hi;
+            rt_slab_pairwise(root_box, l.o[0], l.o[1], l.o[2], l.inv[0], l.inv[1], l.inv[2], 0.0f, lo, hi);
+            if (!(rt_oct_min(hi, l.t_max) >= lo)) continue;
+            l.live = true; l.cur = root_ref;
+            if (variant == 1 && l.cur < 0) { l.pending = l.cur; l.cur = EMPTY; }
+        }
+        auto is_leaf = [](int ref) { return ref < 0 && ref != EMPTY; };
+        for (;;)
+        {
+            bool any_live = false;
+            for (int i = 0; i < m; ++i) any_live |= lane[i].live;
+            if (!any_live) break;
+            for (;;)
+            {   // interior loop
+                int n_in = 0, n_pend = 0;
+                for (int i = 0; i < m; ++i)
+                {
+                    AnyLane& l = lane[i];
+                    if (!l.live || l.cur < 0) continue;
+                    ++n_in;
+                    wide_step(l, variant == 2);
+                    if (variant == 1 && is_leaf(l.cur) && l.pending == 0) { l.pending = l.cur; pop(l); }
+                    if (variant == 1 && l.pending != 0) ++n_pend;
+                    if (variant != 1 && l.cur == EMPTY) { l.live = false; ++*unoccluded; }
+                }
+                if (!n_in) break;
+                const double step = c[0] + (variant == 1 ? c[6] : 0.0);
+                r.slots += step; r.thread_work += step * n_in;
+                if (variant == 1 && trigger >= 0 && n_pend >= (trigger ? std::min(trigger, n_in) : n_in)) break;
+            }
+            for (;;)
+            {   // leaf loop: lane state ti = ~leaf
+                int n_in = 0; double worst = 0, sum = 0;
+                for (int i = 0; i < m; ++i)
+                {
+                    AnyLane& l = lane[i];
+                    int* leaf = variant == 1 ? &l.pending : &l.cur;
+                    if (!l.live || !is_leaf(*leaf)) continue;
+                    ++n_in;
+                    bool hit, last;
+                    const uint8_t st = tri_step(tris, l, (uint32_t)~*leaf, &hit, &last);
+                    worst = std::max(worst, c[st]); sum += c[st];
+                    if (hit) { l.live = false; continue; }
+                    if (!last) { --*leaf; continue; }
+                    if (variant != 1) { l.cur = EMPTY; l.pending = 1; continue; }   // pops after the loop
+                    if (is_leaf(l.cur)) { l.pending = l.cur; pop(l); } else l.pending = 0;
+                }
+                if (!n_in) break;
+                r.slots += worst; r.thread_work += sum;
+            }
+            for (int i = 0; i < m; ++i)
+            {
+                AnyLane& l = lane[i];
+                if (!l.live) continue;
+                if (variant != 1 && l.pending == 1) { l.pending = 0; pop(l); }
+                if (l.cur == EMPTY && l.pending == 0) { l.live = false; ++*unoccluded; }
+            }
+        }
+    }
+    return r;
+}
+} // namespace
+
+// The SMEM 3 any-hit loop over rays (7 floats: origin, direction, t_max): tables of n records (tests/wide_octant_host.cpp,
+// wide_tables), triangle records of rt_bvh_layout.h.  costs: wide step, tri1..tri4, fetch, postponing overhead.
+// out: slots, thread work, rays walked to the end without a hit.
+extern "C" int simt_any_model(const float* tables, uint32_t n, const float* tris, int root_ref, const float* root_box, const float* rays,
+                              uint32_t n_rays, int variant, int trigger, const double* costs, double* out)
+{
+    double slots = 0, work = 0; uint64_t unocc = 0;
+    const uint32_t per = 32 * 64;
+    const long long n_chunks = (long long)((n_rays + per - 1) / per);
+#pragma omp parallel for schedule(dynamic, 16) reduction(+ : slots, work, unocc)
+    for (long long w = 0; w < n_chunks; ++w)
+    {
+        size_t first = (size_t)w * per, count = std::min<size_t>(per, (size_t)n_rays - first);
+        uint64_t u = 0;
+        Result r = simulate_any_warp(tables, n, tris, root_ref, root_box, rays, first, count, variant, trigger, costs, &u);
+        slots += r.slots; work += r.thread_work; unocc += u;
+    }
+    out[0] = slots; out[1] = work; out[2] = (double)unocc;
     return 0;
 }
