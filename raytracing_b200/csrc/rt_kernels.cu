@@ -554,7 +554,7 @@ __global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCoun
 }
 
 // IntersectRays (stepwise): closest hit of every live ray of bounce b -> hits[]
-// INST: an instanced scene (trace_instanced); mode is not read
+// INST: an instanced scene (trace_instanced); mode is not read.  Nothing is staged.
 template <bool COUNT, bool INST = false>
 __global__ void __launch_bounds__(256) k_intersect(FrameParams p, SceneOf<INST> sc, int mode, Queues q, DevCounters* ctr, uint32_t bounce)
 {
@@ -566,9 +566,7 @@ __global__ void __launch_bounds__(256) k_intersect(FrameParams p, SceneOf<INST> 
     {
         float4 a = q.A[in][i], b = q.B[in][i];
         float bu = 0.0f, bv = 0.0f, bt = 0.0f;
-        uint32_t prim;
-        if constexpr (INST) prim = trace_instanced<false, COUNT>(sc, mk3(a), mk3(b), 0.0f, RT_MAX_RENDER_DIST, bu, bv, bt, nv, nt);
-        else prim = trace<false, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, RT_MAX_RENDER_DIST, bu, bv, bt, nv, nt);
+        const uint32_t prim = trace_staged<false, COUNT, INST ? RT_SMEM_INST : 0, false>(sc, mode, nullptr, a, b, bu, bv, bt, nv, nt);
         q.hits[i] = make_float4(bu, bv, __uint_as_float(prim), bt);
     }
     if (COUNT) { warp_sum64(&ctr->nodes_ext[bounce], nv); warp_sum64(&ctr->tris_ext[bounce], nt); }
@@ -617,8 +615,7 @@ __global__ void __launch_bounds__(256) k_intersect_shadow(FrameParams p, SceneOf
     {
         float4 a = q.sA[i], b = q.sB[i];
         float bu, bv, bt;
-        if constexpr (INST) q.shadow_flags[i] = trace_instanced<true, COUNT>(sc, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
-        else q.shadow_flags[i] = trace<true, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, b.w, bu, bv, bt, nv, nt);
+        q.shadow_flags[i] = trace_staged<true, COUNT, INST ? RT_SMEM_INST : 0, false>(sc, mode, nullptr, a, b, bu, bv, bt, nv, nt);
     }
     if (COUNT) { warp_sum64(&ctr->nodes_shadow[bounce], nv); warp_sum64(&ctr->tris_shadow[bounce], nt); }
 }
@@ -1624,23 +1621,39 @@ DevInstScene inst_scene(const rt_ctx* c)
     return s;
 }
 
-// Launches a staged traversal kernel: calls launch(std::integral_constant<int, SMEM>, the DevScene with this launch's top_k, the
-// dynamic shared-memory bytes) once, for the launch's staging mode, and returns its result.  At most 40 KB are staged, under the
-// 48 KB that every kernel may take without raising its shared-memory limit.
-template <class F>
-auto launch_staged(const rt_ctx* c, F&& launch, bool octant = true)
+// Calls f(INST, scene) with the context's scene as a kernel argument: (std::true_type, inst_scene(c)) or (std::false_type,
+// c->scene), the latter always when the caller's kernels have no instanced variant (HAS_INST false).
+template <bool HAS_INST = true, class F>
+auto with_scene(const rt_ctx* c, F&& f)
 {
-    const Stage sg = bvh_stage(c, octant);
-    DevScene sc = c->scene;
-    sc.top_k = sg.top_k;
-    if (sg.mode == 1) return launch(std::integral_constant<int, 1>(), sc, sg.bytes);
-    if (sg.mode == 2) return launch(std::integral_constant<int, 2>(), sc, sg.bytes);
-    if constexpr (std::is_void_v<decltype(launch(std::integral_constant<int, 1>(), sc, sg.bytes))>)
-    {   // the per-phase kernels (their launchers return nothing); the frame kernels never ask for mode 3 or run instanced scenes
-        if (c->instanced) return launch(std::integral_constant<int, RT_SMEM_INST>(), inst_scene(c), (size_t)0);
-        if (sg.mode == 3) return launch(std::integral_constant<int, 3>(), sc, sg.bytes);
-    }
-    return launch(std::integral_constant<int, 0>(), sc, sg.bytes);
+    if constexpr (HAS_INST) if (c->instanced) return f(std::true_type(), inst_scene(c));
+    return f(std::false_type(), c->scene);
+}
+
+// The traversal kernel families and the variants each is instantiated for (COUNT: RT_OPT_COUNT_TRAVERSAL, which stages nothing):
+//   PER_PHASE  k_trace_closest, k_trace_primary, k_shadow_accumulate: staging modes 0-3 and RT_SMEM_INST, COUNT on 0 and INST;
+//   MERGED     k_trace_both: modes 0-3 and RT_SMEM_INST, no COUNT (merged_trace_available);
+//   STEPWISE   k_intersect, k_intersect_shadow: 0 and RT_SMEM_INST, COUNT on both;
+//   FRAME      k_frame, k_frame_regen: modes 0-2 (bvh_stage without the octant tables) on flat scenes, no COUNT.
+enum Family { PER_PHASE, MERGED, STEPWISE, FRAME };
+
+// Launches a traversal kernel of family F: calls launch(COUNT, SMEM, scene, dynamic shared-memory bytes) once with this launch's
+// COUNT (std::bool_constant) and staging mode SMEM (std::integral_constant), and the DevScene with its top_k or the DevInstScene;
+// returns launch's result.  At most 40 KB are staged, under the 48 KB that every kernel may take without raising its limit.
+template <Family F, class L>
+auto launch_traversal(const rt_ctx* c, L&& launch)
+{
+    return with_scene<F != FRAME>(c, [&](auto inst, auto sc) {
+        using Unstaged = std::integral_constant<int, inst.value ? RT_SMEM_INST : 0>;
+        if constexpr (F == PER_PHASE || F == STEPWISE) if (c->count_traversal) return launch(std::true_type(), Unstaged(), sc, (size_t)0);
+        constexpr int MAX_MODE = inst.value || F == STEPWISE ? 0 : F == FRAME ? 2 : 3;
+        const Stage sg = MAX_MODE ? bvh_stage(c, MAX_MODE == 3) : Stage{ 0, 0, 0 };
+        sc.top_k = sg.top_k;
+        if constexpr (MAX_MODE >= 1) if (sg.mode == 1) return launch(std::false_type(), std::integral_constant<int, 1>(), sc, sg.bytes);
+        if constexpr (MAX_MODE >= 2) if (sg.mode == 2) return launch(std::false_type(), std::integral_constant<int, 2>(), sc, sg.bytes);
+        if constexpr (MAX_MODE >= 3) if (sg.mode == 3) return launch(std::false_type(), std::integral_constant<int, 3>(), sc, sg.bytes);
+        return launch(std::false_type(), Unstaged(), sc, (size_t)0);
+    });
 }
 
 AovCam aov_cam(const RtCamera& cam);
@@ -2847,10 +2860,9 @@ int rt_intersect(rt_ctx* c, uint32_t bounce)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_intersect(k, bounce));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     TimedLaunch t(c, RT_K_INTERSECT);
-    if (c->instanced)
-        (c->count_traversal ? k_intersect<true, true> : k_intersect<false, true>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, bounce);
-    else if (c->count_traversal) k_intersect<true><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
-    else k_intersect<false><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
+    launch_traversal<STEPWISE>(c, [&](auto count, auto smem, const auto& sc, size_t) {
+        k_intersect<count.value, smem.value == RT_SMEM_INST><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
+    });
     return post_launch(c, "k_intersect");
 }
 
@@ -2883,9 +2895,9 @@ int rt_shade_hits(rt_ctx* c, uint32_t bounce)
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, bounce);
     c->cur_bounce = bounce;
     TimedLaunch t(c, RT_K_HIT);
-    if (c->instanced)
-        (lights_sampled(c) ? k_shade_hits<true, true> : k_shade_hits<false, true>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->q, c->counters, c->radiance, bounce, aov_params(c));
-    else (lights_sampled(c) ? k_shade_hits<true> : k_shade_hits<false>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c));
+    with_scene(c, [&](auto inst, const auto& sc) {
+        (lights_sampled(c) ? k_shade_hits<true, inst.value> : k_shade_hits<false, inst.value>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), sc, c->q, c->counters, c->radiance, bounce, aov_params(c));
+    });
     return post_launch(c, "k_shade_hits");
 }
 
@@ -2894,10 +2906,9 @@ int rt_intersect_shadow(rt_ctx* c)
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_intersect_shadow(k));
     { int rt_j_ = join_shadow(c); if (rt_j_) return rt_j_; } RT_BOUNCE_CHECK(c, c->cur_bounce);
     TimedLaunch t(c, RT_K_INTERSECT_SHADOW);
-    if (c->instanced)
-        (c->count_traversal ? k_intersect_shadow<true, true> : k_intersect_shadow<false, true>)<<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, c->cur_bounce);
-    else if (c->count_traversal) k_intersect_shadow<true><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->cur_bounce);
-    else k_intersect_shadow<false><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->cur_bounce);
+    launch_traversal<STEPWISE>(c, [&](auto count, auto smem, const auto& sc, size_t) {
+        k_intersect_shadow<count.value, smem.value == RT_SMEM_INST><<<grid_for(c->n_local), 256, 0, c->stream>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->cur_bounce);
+    });
     return post_launch(c, "k_intersect_shadow");
 }
 
@@ -2943,7 +2954,7 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     {   // this bounce's closest-hit traversal + the previous bounce's shadow pass in one kernel
         c->shadow_deferred = false;
         TimedLaunch t(c, RT_K_TRACE_BOTH);
-        launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
+        launch_traversal<MERGED>(c, [&](auto, auto smem, const auto& sc, size_t sm) {
             auto* k = k_trace_both<smem.value>;
             launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce, c->shadow_deferred_bounce);
         });
@@ -2953,24 +2964,20 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     {   // the frame's primary rays are generated here (begin_frame without k_raygen)
         c->primary_fused = false;
         TimedLaunch t(c, RT_K_TRACE_CLOSEST);
-        if (c->count_traversal && c->instanced)
-            k_trace_primary<true, RT_SMEM_INST><<<RT_PGRID(c, (k_trace_primary<true, RT_SMEM_INST>), 0), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, aov_params(c));
-        else if (c->count_traversal) k_trace_primary<true, 0><<<RT_PGRID(c, (k_trace_primary<true, 0>), 0), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, aov_params(c));
-        else launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
-            auto* k = k_trace_primary<false, smem.value>;
-            launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, aov_params(c));
+        launch_traversal<PER_PHASE>(c, [&](auto count, auto smem, const auto& sc, size_t sm) {
+            auto* k = k_trace_primary<count.value, smem.value>;
+            if (count) k<<<RT_PGRID(c, k, sm), 256, sm, c->stream>>>(frame_params(c), sc, c->traversal, c->q, c->counters, aov_params(c));
+            else launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, aov_params(c));
         });
         int rc = post_launch(c, "k_trace_primary"); if (rc) return rc;
     }
     else
     {
         TimedLaunch t(c, RT_K_TRACE_CLOSEST);
-        if (c->count_traversal && c->instanced)
-            k_trace_closest<true, RT_SMEM_INST><<<RT_PGRID(c, (k_trace_closest<true, RT_SMEM_INST>), 0), 256, 0, c->stream>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, bounce);
-        else if (c->count_traversal) k_trace_closest<true, 0><<<RT_PGRID(c, (k_trace_closest<true, 0>), 0), 256, 0, c->stream>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, bounce);
-        else launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
-            auto* k = k_trace_closest<false, smem.value>;
-            launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
+        launch_traversal<PER_PHASE>(c, [&](auto count, auto smem, const auto& sc, size_t sm) {
+            auto* k = k_trace_closest<count.value, smem.value>;
+            if (count) k<<<RT_PGRID(c, k, sm), 256, sm, c->stream>>>(frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
+            else launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->traversal, c->q, c->counters, bounce);
         });
         int rc = post_launch(c, "k_trace_closest"); if (rc) return rc;
     }
@@ -2978,16 +2985,11 @@ int rt_extend_shade(rt_ctx* c, uint32_t bounce)
     TimedLaunch t(c, RT_K_SHADE_QUEUES);
     const bool sort = sorted_shading(c);
     const size_t sm = sort ? sizeof(ContStage) : 0;
-    if (c->instanced)
-    {
-        auto* k = lights_sampled(c) ? (sort ? k_shade_queues<true, true, true> : k_shade_queues<false, true, true>)
-                                     : (sort ? k_shade_queues<true, false, true> : k_shade_queues<false, false, true>);
-        launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), inst_scene(c), c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
-        return post_launch(c, "k_shade_queues");
-    }
-    auto* k = lights_sampled(c) ? (sort ? k_shade_queues<true, true> : k_shade_queues<false, true>)
-                                 : (sort ? k_shade_queues<true> : k_shade_queues<false>);
-    launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), c->scene, c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
+    with_scene(c, [&](auto inst, const auto& sc) {
+        auto* k = lights_sampled(c) ? (sort ? k_shade_queues<true, true, inst.value> : k_shade_queues<false, true, inst.value>)
+                                     : (sort ? k_shade_queues<true, false, inst.value> : k_shade_queues<false, false, inst.value>);
+        launch_chain(c, k, RT_PGRID(c, k, sm), sm, c->stream, frame_params(c), sc, c->q, c->counters, c->radiance, bounce, aov_params(c), c->scene_mid);
+    });
     return post_launch(c, "k_shade_queues");
 }
 
@@ -3003,11 +3005,8 @@ static int ensure_shadow_stream(rt_ctx* c)
 static int launch_shadow_pass(rt_ctx* c, uint32_t bounce, cudaStream_t st)
 {
     TimedLaunch t(c, RT_K_SHADOW_ACCUMULATE, st);
-    if (c->count_traversal && c->instanced)
-        k_shadow_accumulate<true, RT_SMEM_INST><<<RT_PGRID(c, (k_shadow_accumulate<true, RT_SMEM_INST>), 0), 256, 0, st>>>(frame_params(c), inst_scene(c), c->traversal, c->q, c->counters, c->radiance, bounce);
-    else if (c->count_traversal) k_shadow_accumulate<true, 0><<<RT_PGRID(c, (k_shadow_accumulate<true, 0>), 0), 256, 0, st>>>(frame_params(c), c->scene, c->traversal, c->q, c->counters, c->radiance, bounce);
-    else launch_staged(c, [&](auto smem, const auto& sc, size_t sm) {
-        auto* k = k_shadow_accumulate<false, smem.value>;
+    launch_traversal<PER_PHASE>(c, [&](auto count, auto smem, const auto& sc, size_t sm) {
+        auto* k = k_shadow_accumulate<count.value, smem.value>;
         k<<<RT_PGRID(c, k, sm), 256, sm, st>>>(frame_params(c), sc, c->traversal, c->q, c->counters, c->radiance, bounce);
     });
     return post_launch(c, "k_shadow_accumulate");
@@ -3164,14 +3163,14 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
     const FrameDyn dyn = frame_dyn(c);
     FrameParams fp = frame_params(c);
     fp.gather = push ? c->gather_slab : nullptr;
-    rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
+    rc = launch_traversal<FRAME>(c, [&](auto, auto smem, const DevScene& sc, size_t sm) -> int {
         auto* k = lights_sampled(c) ? k_frame<smem.value, true> : k_frame<smem.value>;
         uint32_t grid, slots_per_cta;
         int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
         TimedLaunch t(c, RT_K_MISC);
         k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters, c->radiance, aov_params(c), max_bounces, slots_per_cta, dyn);
         return RT_OK;
-    }, false);
+    });
     if (rc || (rc = post_launch(c, "k_frame"))) return rc;
     note_frame_aovs(c);
     if (adaptive_on(c) && (rc = launch_adaptive_update(c))) return rc;
@@ -3188,7 +3187,7 @@ static int integrate_regen_kernel(rt_ctx* c, uint32_t max_bounces, uint32_t n_sa
     const FrameDyn dyn = frame_dyn(c);
     FrameParams fp = frame_params(c);
     fp.gather = c->gather_slab;
-    int rc = launch_staged(c, [&](auto smem, const DevScene& sc, size_t sm) -> int {
+    int rc = launch_traversal<FRAME>(c, [&](auto, auto smem, const DevScene& sc, size_t sm) -> int {
         auto* k = k_frame_regen<smem.value>;
         uint32_t grid, slots_per_cta;
         int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
@@ -3196,7 +3195,7 @@ static int integrate_regen_kernel(rt_ctx* c, uint32_t max_bounces, uint32_t n_sa
         k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters_sum, c->radiance, aov_params(c), max_bounces, n_samples,
                                             slots_per_cta, dyn);
         return RT_OK;
-    }, false);
+    });
     if (rc || (rc = post_launch(c, "k_frame_regen"))) return rc;
     note_frame_aovs(c);
     c->frame_started = true; c->cur_bounce = max_bounces;

@@ -1,6 +1,7 @@
 /*
- * rt_traverse.cuh — BVH staging (TMA bulk copies) and the traversal functions: literal reference-order traversal, the child-box layout
- * traversal, and trace_staged, the traversal call of a kernel that staged the BVH.
+ * rt_traverse.cuh — BVH staging (TMA bulk copies), the traversal steps, and the traversal functions built from them: literal
+ * reference-order traversal, the child-box layout traversal, the two-level instanced traversal, and trace_staged, the traversal call
+ * of every kernel.
  * Part of the single translation unit rt_kernels.cu (included there, inside its anonymous namespace).
  */
 #pragma once
@@ -142,13 +143,119 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 template <int SMEM>
 __device__ __forceinline__ float4 ld_bvh(const float4* p) { return SMEM ? *p : __ldg(p); }
 
+// ------------------------------------------------------------------------------------ traversal steps
+// The steps every traversal loop below is made of: the slab test of a box, the binary child-pair step, the pop of a deferred far
+// child and the ray-triangle test.  One expression order each, shared by the literal, child-box and instanced traversals, which
+// is what keeps them bit-identical.
+// RT_FMA_TRAVERSAL (an experiment build, tools/build_variant.py; NOT bit-exact): contracted slab, cross and dot products.
+#ifdef RT_FMA_TRAVERSAL
+#define RT_CROSS(a, b) mk3(__fmaf_rn((a).y, (b).z, -((a).z * (b).y)), __fmaf_rn((a).z, (b).x, -((a).x * (b).z)), __fmaf_rn((a).x, (b).y, -((a).y * (b).x)))
+#define RT_DOT(a, b) __fmaf_rn((a).x, (b).x, __fmaf_rn((a).y, (b).y, (a).z * (b).z))
+#else
+#define RT_CROSS(a, b) cross(a, b)
+#define RT_DOT(a, b) dot(a, b)
+#endif
+
+// Slab interval [lo, hi] of the ray (o, inv = 1 / d) in the box (bmin, bmax), lo clamped below by t_min; the box is hit when
+// fminf(hi, t_max) >= lo (inclusive).
+__device__ __forceinline__ void slab(f3 bmin, f3 bmax, f3 o, f3 inv, float t_min, float& lo, float& hi)
+{
+#ifdef RT_FMA_TRAVERSAL
+    // plane * inv - origin * inv in one FFMA per plane
+    const f3 noi = mk3(-(o.x * inv.x), -(o.y * inv.y), -(o.z * inv.z));
+    const f3 t0 = mk3(__fmaf_rn(bmin.x, inv.x, noi.x), __fmaf_rn(bmin.y, inv.y, noi.y), __fmaf_rn(bmin.z, inv.z, noi.z));
+    const f3 t1 = mk3(__fmaf_rn(bmax.x, inv.x, noi.x), __fmaf_rn(bmax.y, inv.y, noi.y), __fmaf_rn(bmax.z, inv.z, noi.z));
+#else
+    const f3 t0 = (bmin - o) * inv, t1 = (bmax - o) * inv;
+#endif
+    lo = fmaxf(fmaxf(fmaxf(fminf(t0.x, t1.x), fminf(t0.y, t1.y)), fminf(t0.z, t1.z)), t_min);
+    hi = fminf(fminf(fmaxf(t0.x, t1.x), fmaxf(t0.y, t1.y)), fmaxf(t0.z, t1.z));
+}
+
+// Does the ray hit the box (bmin, bmax) within [t_min, t_max]?
+__device__ __forceinline__ bool box_hit(f3 bmin, f3 bmax, f3 o, f3 inv, float t_min, float t_max)
+{
+    float lo, hi;
+    slab(bmin, bmax, o, inv, t_min, lo, hi);
+    return fminf(hi, t_max) >= lo;
+}
+
+// Binary child-pair step on a child-box record (a, b, c, m) (rt_bvh_layout.h): both children's boxes tested, near and far
+// child chosen by the ray's sign on the record's split axis (the second child is near iff inv[axis] < 0), and the far child's
+// entry distance.  PACKED: the sign-bit form (sign_bits bit k: inv[k] < 0), for records in shared memory; otherwise predicate
+// selects on the signs of inv (sign_bits unused), for records behind L1/L2 (trace_fast says why).
+struct ChildPair { int near_ref, far_ref; bool near_hit, far_hit; float far_lo; };
+template <bool PACKED>
+__device__ __forceinline__ ChildPair child_pair(float4 a, float4 b, float4 c, float4 m, f3 o, f3 inv, uint32_t sign_bits, float t_min, float t_max)
+{
+    // child 0 box: min (a.x,a.y,a.z) max (a.w,b.x,b.y); child 1 box: min (b.z,b.w,c.x) max (c.y,c.z,c.w)
+    float lo0, hi0, lo1, hi1;
+    slab(mk3(a.x, a.y, a.z), mk3(a.w, b.x, b.y), o, inv, t_min, lo0, hi0);
+    slab(mk3(b.z, b.w, c.x), mk3(c.y, c.z, c.w), o, inv, t_min, lo1, hi1);
+    const bool h0 = fminf(hi0, t_max) >= lo0, h1 = fminf(hi1, t_max) >= lo1;
+    const int r0 = __float_as_int(m.x), r1 = __float_as_int(m.y);
+    const uint32_t axis = __float_as_uint(m.z);
+    const bool swap = PACKED ? ((sign_bits >> axis) & 1u) != 0u : (axis == 0 ? inv.x < 0 : (axis == 1 ? inv.y < 0 : inv.z < 0));
+    ChildPair s;
+    s.near_ref = swap ? r1 : r0; s.far_ref = swap ? r0 : r1;
+    s.near_hit = swap ? h1 : h0; s.far_hit = swap ? h0 : h1;
+    s.far_lo = swap ? lo0 : lo1;
+    return s;
+}
+
+// Pop: the deferred far child on top of the stack, as (reference, entry distance).  A pushed child is re-tested against the
+// (possibly shrunk) t_max, as the reference does when it pops it; its slab interval was already valid at push time.  Entries
+// that fail are dropped.  Returns false when the stack runs empty.  Two stack shapes: packed 64-bit entries, or two arrays.
+__device__ __forceinline__ bool pop(const int2* stack, int& sp, float t_max, int& cur)
+{
+    while (sp > 0)
+    {
+        --sp;
+        const int2 e = stack[sp];
+        if (t_max >= __int_as_float(e.y)) { cur = e.x; return true; }
+    }
+    return false;
+}
+__device__ __forceinline__ bool pop(const int* stack_ref, const float* stack_t, int& sp, float t_max, int& cur)
+{
+    while (sp > 0) { --sp; if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; return true; } }
+    return false;
+}
+
+// Ray-triangle test (Möller-Trumbore) of the triangle (p1, e1 = p2 - p1, e2 = p3 - p1), inclusive, with back-face culling:
+// det < 1e-8 rejects.  SIGNED (instanced scenes): the culling test reads det * cull (cull = sign(det M) of a mirrored instance:
+// -1), so that a mirrored instance culls the faces its flattened triangles would; u, v and t still divide by det.  A hit with t
+// in [t_min, t_max] calls hit(u, v, t) and returns true.  PIN: see trace_fast.
+// The hit is handed to a callable rather than returned through references: a returned (u, v, t) joins the miss paths before
+// the caller's branch, and ptxas then spills the closest-hit kernels at their 48 registers.
+template <bool SIGNED, bool PIN = false, class Hit>
+__device__ __forceinline__ bool tri_hit(f3 p1, f3 e1, f3 e2, f3 o, f3 d, float cull, float t_min, float t_max, Hit&& hit)
+{
+    const f3 pvec = RT_CROSS(d, e2);
+    float det = RT_DOT(e1, pvec);
+    if (PIN) asm volatile("" : "+f"(det));
+    const float cdet = SIGNED ? det * cull : det;
+    if (cdet < 1e-8f || -cdet > 1e-8f) return false;
+    const float inv_det = 1.0f / det;
+    const f3 tvec = o - p1;
+    const float u = RT_DOT(tvec, pvec) * inv_det;
+    if (u < 0.0f || u > 1.0f) return false;
+    const f3 qvec = RT_CROSS(tvec, e1);
+    const float v = RT_DOT(d, qvec) * inv_det;
+    if (v < 0.0f || u + v > 1.0f) return false;
+    const float t = RT_DOT(e2, qvec) * inv_det;
+    if (t < t_min || t > t_max) return false;
+    hit(u, v, t);
+    return true;
+}
+#undef RT_CROSS
+#undef RT_DOT
+
 // ------------------------------------------------------------------------------------ traversal
 // Literal restatement of kernels/cl/trace_bvh.cl:99-211 on the reference node layout: per-ray
 // DFS, 64-entry private stack, far child pushed unconditionally and box-tested when popped,
 // near child chosen by ray_sign[axis], inclusive tests, later equal-t hit overwrites, back-face
-// culling (det < 1e-8 rejects).  ANY = the -D SHADOW_RAYS variant (returns 0 on first hit).
-// SIGNED (instanced scenes): the culling test reads det * cull (cull = sign(det M) of a mirrored instance: -1), so that a
-// mirrored instance culls the faces its flattened triangles would; u, v and t still divide by det.
+// culling (det < 1e-8 rejects, tri_hit).  ANY = the -D SHADOW_RAYS variant (returns 0 on first hit).
 template <bool ANY, bool COUNT, bool SIGNED = false>
 __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d, float t_min, float t_max,
                                                   float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt, float cull = 1.0f)
@@ -162,10 +269,7 @@ __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d
     {
         float4 n0 = __ldg(sc.nodes_ref + (size_t)cur * 3), n1 = __ldg(sc.nodes_ref + (size_t)cur * 3 + 1), n2 = __ldg(sc.nodes_ref + (size_t)cur * 3 + 2);
         if (COUNT) ++nv;
-        f3 t0 = (mk3(n0) - o) * inv, t1 = (mk3(n1) - o) * inv;
-        float lo = fmaxf(fmaxf(fminf(t0.x, t1.x), fminf(t0.y, t1.y)), fminf(t0.z, t1.z));
-        float hi = fminf(fminf(fmaxf(t0.x, t1.x), fmaxf(t0.y, t1.y)), fmaxf(t0.z, t1.z));
-        bool box = fminf(hi, t_max) >= fmaxf(lo, t_min);
+        bool box = box_hit(mk3(n0), mk3(n1), o, inv, t_min, t_max);
         uint32_t offset = __float_as_uint(n2.x), npa = __float_as_uint(n2.y);
         if (box)
         {
@@ -177,24 +281,12 @@ __device__ __forceinline__ uint32_t trace_literal(const DevScene& sc, f3 o, f3 d
                     const float4* tp = sc.tris_ref + (size_t)(offset + i) * 3;
                     f3 p1 = mk3(__ldg(tp)), p2 = mk3(__ldg(tp + 1)), p3 = mk3(__ldg(tp + 2));
                     if (COUNT) ++nt;
-                    f3 e1 = p2 - p1, e2 = p3 - p1;
-                    f3 pvec = cross(d, e2);
-                    float det = dot(e1, pvec);
-                    const float cdet = SIGNED ? det * cull : det;
-                    if (cdet < 1e-8f || -cdet > 1e-8f) continue;
-                    float inv_det = 1.0f / det;
-                    f3 tvec = o - p1;
-                    float u = dot(tvec, pvec) * inv_det;
-                    if (u < 0.0f || u > 1.0f) continue;
-                    f3 qvec = cross(tvec, e1);
-                    float v = dot(d, qvec) * inv_det;
-                    if (v < 0.0f || u + v > 1.0f) continue;
-                    float t = dot(e2, qvec) * inv_det;
-                    if (t < t_min || t > t_max) continue;
-                    bu = u; bv = v; bt = t;
-                    prim = offset + i;
-                    t_max = t;
-                    if (ANY) return 0u;
+                    const bool hit = tri_hit<SIGNED>(p1, p2 - p1, p3 - p1, o, d, cull, t_min, t_max, [&](float u, float v, float t) {
+                        bu = u; bv = v; bt = t;
+                        prim = offset + i;
+                        t_max = t;
+                    });
+                    if (ANY && hit) return 0u;
                 }
                 if (to_visit == 0) break;
                 cur = stack[--to_visit];
@@ -266,22 +358,8 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
     // being re-derived from the sign bits and the two sizes on every step
     uint32_t oct_at = OCT ? sc.wnodes_f4 + sc.wtris_f4 + sign_bits * sc.wnodes_f4 : 0u;
     if (OCT) asm volatile("" : "+r"(oct_at));
-    if (cur < 0)
-    {   // single-leaf tree: the root box is tested like any visited node
-        float4 r0 = __ldg(sc.nodes_ref), r1 = __ldg(sc.nodes_ref + 1);
-        f3 t0 = (mk3(r0) - o) * inv, t1 = (mk3(r1) - o) * inv;
-        float lo = fmaxf(fmaxf(fminf(t0.x, t1.x), fminf(t0.y, t1.y)), fminf(t0.z, t1.z));
-        float hi = fminf(fminf(fmaxf(t0.x, t1.x), fmaxf(t0.y, t1.y)), fmaxf(t0.z, t1.z));
-        if (!(fminf(hi, t_max) >= fmaxf(lo, t_min))) return prim;
-    }
-    else
-    {   // root box test (the reference tests every node it visits, including the root)
-        float4 r0 = __ldg(sc.nodes_ref), r1 = __ldg(sc.nodes_ref + 1);
-        f3 t0 = (mk3(r0) - o) * inv, t1 = (mk3(r1) - o) * inv;
-        float lo = fmaxf(fmaxf(fminf(t0.x, t1.x), fminf(t0.y, t1.y)), fminf(t0.z, t1.z));
-        float hi = fminf(fminf(fmaxf(t0.x, t1.x), fmaxf(t0.y, t1.y)), fmaxf(t0.z, t1.z));
-        if (!(fminf(hi, t_max) >= fmaxf(lo, t_min))) return prim;
-    }
+    // root box (the reference tests every node it visits, including the root; a single-leaf tree has nothing else to test)
+    if (!box_hit(mk3(__ldg(sc.nodes_ref)), mk3(__ldg(sc.nodes_ref + 1)), o, inv, t_min, t_max)) return prim;
     for (;;)
     {
         while (cur >= 0)
@@ -319,68 +397,25 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
                 }
                 if (found) { cur = next_ref; continue; }
                 if (ANY) { if (sp == 0) return prim; cur = any_stack[--sp]; continue; }
-                while (sp > 0)
-                {
-                    --sp;
-                    int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; }
-                }
-                if (!found) return prim;
+                if (!pop(stack, sp, t_max, cur)) return prim;
                 continue;
             }
             // SMEM == 2: `wnodes` is the staged top of the tree (records [0, sc.top_k)), deeper records come from sc.wnodes
             const float4* np = (SMEM == 2 && (uint32_t)cur >= sc.top_k) ? sc.wnodes + (size_t)cur * 4 : wnodes + (size_t)cur * 4;
-            float4 a = ld_bvh<SMEM>(np), b = ld_bvh<SMEM>(np + 1), c = ld_bvh<SMEM>(np + 2), m = ld_bvh<SMEM>(np + 3);
-            int near_ref, far_ref;
-            bool near_hit, far_hit;
-            float far_lo;
+            const ChildPair s = child_pair<PACKED>(ld_bvh<SMEM>(np), ld_bvh<SMEM>(np + 1), ld_bvh<SMEM>(np + 2), ld_bvh<SMEM>(np + 3),
+                                                   o, inv, sign_bits, t_min, t_max);
+            if (s.near_hit)
             {
-                // child 0 box: min (a.x,a.y,a.z) max (a.w,b.x,b.y); child 1 box: min (b.z,b.w,c.x) max (c.y,c.z,c.w)
-#ifdef RT_FMA_TRAVERSAL
-                // experiment (NOT bit-exact): contracted slab test, plane * inv - origin * inv in one FFMA per plane
-                const f3 noi = mk3(-(o.x * inv.x), -(o.y * inv.y), -(o.z * inv.z));
-                f3 t00 = mk3(__fmaf_rn(a.x, inv.x, noi.x), __fmaf_rn(a.y, inv.y, noi.y), __fmaf_rn(a.z, inv.z, noi.z));
-                f3 t01 = mk3(__fmaf_rn(a.w, inv.x, noi.x), __fmaf_rn(b.x, inv.y, noi.y), __fmaf_rn(b.y, inv.z, noi.z));
-                f3 t10 = mk3(__fmaf_rn(b.z, inv.x, noi.x), __fmaf_rn(b.w, inv.y, noi.y), __fmaf_rn(c.x, inv.z, noi.z));
-                f3 t11 = mk3(__fmaf_rn(c.y, inv.x, noi.x), __fmaf_rn(c.z, inv.y, noi.y), __fmaf_rn(c.w, inv.z, noi.z));
-#else
-                f3 t00 = (mk3(a.x, a.y, a.z) - o) * inv, t01 = (mk3(a.w, b.x, b.y) - o) * inv;
-                f3 t10 = (mk3(b.z, b.w, c.x) - o) * inv, t11 = (mk3(c.y, c.z, c.w) - o) * inv;
-#endif
-                float lo0 = fmaxf(fmaxf(fmaxf(fminf(t00.x, t01.x), fminf(t00.y, t01.y)), fminf(t00.z, t01.z)), t_min);
-                float hi0 = fminf(fminf(fmaxf(t00.x, t01.x), fmaxf(t00.y, t01.y)), fmaxf(t00.z, t01.z));
-                float lo1 = fmaxf(fmaxf(fmaxf(fminf(t10.x, t11.x), fminf(t10.y, t11.y)), fminf(t10.z, t11.z)), t_min);
-                float hi1 = fminf(fminf(fmaxf(t10.x, t11.x), fmaxf(t10.y, t11.y)), fmaxf(t10.z, t11.z));
-                bool h0 = fminf(hi0, t_max) >= lo0, h1 = fminf(hi1, t_max) >= lo1;
-                int r0 = __float_as_int(m.x), r1 = __float_as_int(m.y);
-                uint32_t axis = __float_as_uint(m.z);
-                bool swap = PACKED ? ((sign_bits >> axis) & 1u) != 0u : (axis == 0 ? sx : (axis == 1 ? sy : sz));   // near child = second iff inv_dir[axis] < 0
-                near_ref = swap ? r1 : r0; far_ref = swap ? r0 : r1;
-                near_hit = swap ? h1 : h0; far_hit = swap ? h0 : h1;
-                far_lo = swap ? lo0 : lo1;
-            }
-            if (near_hit)
-            {
-                if (far_hit)
+                if (s.far_hit)
                 {
-                    if (PACKED) stack[sp] = make_int2(far_ref, __float_as_int(far_lo));
-                    else { stack_ref[sp] = far_ref; stack_t[sp] = far_lo; }
+                    if (PACKED) stack[sp] = make_int2(s.far_ref, __float_as_int(s.far_lo));
+                    else { stack_ref[sp] = s.far_ref; stack_t[sp] = s.far_lo; }
                     ++sp;
                 }
-                cur = near_ref;
+                cur = s.near_ref;
             }
-            else if (far_hit) cur = far_ref;
-            else
-            {   // pop: a pushed far child is re-tested against the (possibly shrunk) t_max, as the
-                // reference does when it pops it; its slab interval was already valid at push time
-                bool found = false;
-                while (sp > 0)
-                {
-                    --sp;
-                    if (PACKED) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
-                    else if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; }
-                }
-                if (!found) return prim;
-            }
+            else if (s.far_hit) cur = s.far_ref;
+            else if (!(PACKED ? pop(stack, sp, t_max, cur) : pop(stack_ref, stack_t, sp, t_max, cur))) return prim;
         }
         // leaf: triangles [~cur ...] until the end-of-leaf flag
         uint32_t ti = (uint32_t)(~cur);
@@ -388,60 +423,16 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
         {
             const float4* tp = wtris + (size_t)ti * 3;
             float4 q0 = ld_bvh<PACKED>(tp), q1 = ld_bvh<PACKED>(tp + 1), q2 = ld_bvh<PACKED>(tp + 2);
-            f3 p1 = mk3(q0.x, q0.y, q0.z), e1 = mk3(q0.w, q1.x, q1.y), e2 = mk3(q1.z, q1.w, q2.x);
             bool last = __float_as_uint(q2.y) != 0u;
-#ifdef RT_FMA_TRAVERSAL
-#define RT_CROSS(a, b) mk3(__fmaf_rn((a).y, (b).z, -((a).z * (b).y)), __fmaf_rn((a).z, (b).x, -((a).x * (b).z)), __fmaf_rn((a).x, (b).y, -((a).y * (b).x)))
-#define RT_DOT(a, b) __fmaf_rn((a).x, (b).x, __fmaf_rn((a).y, (b).y, (a).z * (b).z))
-#else
-#define RT_CROSS(a, b) cross(a, b)
-#define RT_DOT(a, b) dot(a, b)
-#endif
-            f3 pvec = RT_CROSS(d, e2);
-            float det = RT_DOT(e1, pvec);
-            if (PIN) asm volatile("" : "+f"(det));
-            const float cdet = SIGNED ? det * cull : det;
-            if (!(cdet < 1e-8f || -cdet > 1e-8f))
-            {
-                float inv_det = 1.0f / det;
-                f3 tvec = o - p1;
-                float u = RT_DOT(tvec, pvec) * inv_det;
-                if (!(u < 0.0f || u > 1.0f))
-                {
-                    f3 qvec = RT_CROSS(tvec, e1);
-                    float v = RT_DOT(d, qvec) * inv_det;
-                    if (!(v < 0.0f || u + v > 1.0f))
-                    {
-                        float t = RT_DOT(e2, qvec) * inv_det;
-                        if (!(t < t_min || t > t_max))
-                        {
-                            bu = u; bv = v; bt = t; prim = ti; t_max = t;
-                            if (ANY) return 0u;
-                        }
-                    }
-                }
-            }
+            const bool hit = tri_hit<SIGNED, PIN>(mk3(q0.x, q0.y, q0.z), mk3(q0.w, q1.x, q1.y), mk3(q1.z, q1.w, q2.x), o, d, cull, t_min, t_max,
+                                                  [&](float u, float v, float t) { bu = u; bv = v; bt = t; prim = ti; t_max = t; });
+            if (ANY && hit) return 0u;
             if (last) break;
             ++ti;
         }
         if (OCT && ANY) { if (sp == 0) return prim; cur = any_stack[--sp]; continue; }
-        bool found = false;
-        while (sp > 0)
-                {
-                    --sp;
-                    if (PACKED) { int2 e = stack[sp]; if (t_max >= __int_as_float(e.y)) { cur = e.x; found = true; break; } }
-                    else if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; }
-                }
-        if (!found) return prim;
+        if (!(PACKED ? pop(stack, sp, t_max, cur) : pop(stack_ref, stack_t, sp, t_max, cur))) return prim;
     }
-}
-
-template <bool ANY, bool COUNT>
-__device__ __forceinline__ uint32_t trace(const DevScene& sc, int mode, f3 o, f3 d, float t_min, float t_max,
-                                          float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
-{
-    if (mode == 0) return trace_literal<ANY, COUNT>(sc, o, d, t_min, t_max, bu, bv, bt, nv, nt);
-    return trace_fast<ANY, COUNT, 0>(sc, sc.wnodes, sc.wtris, o, d, t_min, t_max, bu, bv, bt, nv, nt);
 }
 
 // Two-level traversal of an instanced scene (rt_b200.h, instanced scenes).  The top-level tree is walked as trace_fast walks a
@@ -458,14 +449,8 @@ __device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o
     const float4 h0 = __ldg(sc.inst_hdr), h1 = __ldg(sc.inst_hdr + 1);
     if (__float_as_uint(h1.w) == 0u) return prim;                  // no instances: every ray misses
     const f3 inv = splat(1.0f) / d;
-    const bool sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
-    {   // root box
-        f3 t0 = (mk3(h0) - o) * inv, t1 = (mk3(h1) - o) * inv;
-        float lo = fmaxf(fmaxf(fminf(t0.x, t1.x), fminf(t0.y, t1.y)), fminf(t0.z, t1.z));
-        float hi = fminf(fminf(fmaxf(t0.x, t1.x), fmaxf(t0.y, t1.y)), fmaxf(t0.z, t1.z));
-        if (COUNT) ++nv;
-        if (!(fminf(hi, t_max) >= fmaxf(lo, t_min))) return prim;
-    }
+    if (COUNT) ++nv;
+    if (!box_hit(mk3(h0), mk3(h1), o, inv, t_min, t_max)) return prim;       // root box
     int cur = __float_as_int(h0.w);
     int sp = 0;
     int stack_ref[64];
@@ -475,33 +460,15 @@ __device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o
         while (cur >= 0)
         {
             const float4* np = sc.top + (size_t)cur * 4;
-            float4 a = __ldg(np), b = __ldg(np + 1), c = __ldg(np + 2), m = __ldg(np + 3);
             if (COUNT) nv += 2;
-            f3 t00 = (mk3(a.x, a.y, a.z) - o) * inv, t01 = (mk3(a.w, b.x, b.y) - o) * inv;
-            f3 t10 = (mk3(b.z, b.w, c.x) - o) * inv, t11 = (mk3(c.y, c.z, c.w) - o) * inv;
-            float lo0 = fmaxf(fmaxf(fmaxf(fminf(t00.x, t01.x), fminf(t00.y, t01.y)), fminf(t00.z, t01.z)), t_min);
-            float hi0 = fminf(fminf(fmaxf(t00.x, t01.x), fmaxf(t00.y, t01.y)), fmaxf(t00.z, t01.z));
-            float lo1 = fmaxf(fmaxf(fmaxf(fminf(t10.x, t11.x), fminf(t10.y, t11.y)), fminf(t10.z, t11.z)), t_min);
-            float hi1 = fminf(fminf(fmaxf(t10.x, t11.x), fmaxf(t10.y, t11.y)), fmaxf(t10.z, t11.z));
-            bool h0b = fminf(hi0, t_max) >= lo0, h1b = fminf(hi1, t_max) >= lo1;
-            int r0 = __float_as_int(m.x), r1 = __float_as_int(m.y);
-            uint32_t axis = __float_as_uint(m.z);
-            bool swap = axis == 0 ? sx : (axis == 1 ? sy : sz);
-            int near_ref = swap ? r1 : r0, far_ref = swap ? r0 : r1;
-            bool near_hit = swap ? h1b : h0b, far_hit = swap ? h0b : h1b;
-            float far_lo = swap ? lo0 : lo1;
-            if (near_hit)
+            const ChildPair s = child_pair<false>(__ldg(np), __ldg(np + 1), __ldg(np + 2), __ldg(np + 3), o, inv, 0u, t_min, t_max);
+            if (s.near_hit)
             {
-                if (far_hit) { stack_ref[sp] = far_ref; stack_t[sp] = far_lo; ++sp; }
-                cur = near_ref;
+                if (s.far_hit) { stack_ref[sp] = s.far_ref; stack_t[sp] = s.far_lo; ++sp; }
+                cur = s.near_ref;
             }
-            else if (far_hit) cur = far_ref;
-            else
-            {
-                bool found = false;
-                while (sp > 0) { --sp; if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; } }
-                if (!found) return prim;
-            }
+            else if (s.far_hit) cur = s.far_ref;
+            else if (!pop(stack_ref, stack_t, sp, t_max, cur)) return prim;
         }
         {   // instance leaf: the ray in object space, then the mesh's tree
             const float4* ir = sc.irec + (size_t)(~cur) * 8;
@@ -522,15 +489,14 @@ __device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o
                 prim = __float_as_uint(mi.w) + p; bu = u; bv = v; bt = t; t_max = t;
             }
         }
-        bool found = false;
-        while (sp > 0) { --sp; if (t_max >= stack_t[sp]) { cur = stack_ref[sp]; found = true; break; } }
-        if (!found) return prim;
+        if (!pop(stack_ref, stack_t, sp, t_max, cur)) return prim;
     }
 }
 
 // The traversal call of every persistent kernel, for the kernel's staging mode (stage_bvh): ray (a, b) = (origin, -), (dir, w).
 // A shadow ray (ANY) carries its t_max in b.w; an extension ray carries its pixel there, and its t_max is RT_MAX_RENDER_DIST.
-// PIN (trace_fast) is applied to the staged modes only.  RT_SMEM_INST: sc is a DevInstScene.
+// SMEM 0: mode 0 (RT_OPT_TRAVERSAL 0) is the literal traversal, otherwise trace_fast from L1/L2; s_bvh is not read.  PIN
+// (trace_fast) is applied to the staged modes only.  RT_SMEM_INST: sc is a DevInstScene, and mode and s_bvh are not read.
 template <bool ANY, bool COUNT, int SMEM, bool PIN, class Scene>
 __device__ __forceinline__ uint32_t trace_staged(const Scene& sc, int mode, const float4* s_bvh, float4 a, float4 b,
                                                  float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
@@ -540,6 +506,7 @@ __device__ __forceinline__ uint32_t trace_staged(const Scene& sc, int mode, cons
     else {
     if (SMEM == 1 || SMEM == 3) return trace_fast<ANY, COUNT, SMEM, PIN>(sc, s_bvh, s_bvh + sc.wnodes_f4, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
     if (SMEM == 2) return trace_fast<ANY, COUNT, 2, PIN>(sc, s_bvh, sc.wtris, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
-    return trace<ANY, COUNT>(sc, mode, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
+    if (mode == 0) return trace_literal<ANY, COUNT>(sc, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
+    return trace_fast<ANY, COUNT, 0>(sc, sc.wnodes, sc.wtris, mk3(a), mk3(b), 0.0f, t_max, bu, bv, bt, nv, nt);
     }
 }
