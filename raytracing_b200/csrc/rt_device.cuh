@@ -199,6 +199,19 @@ struct Material
     float transparency;
 };
 
+// The BSDF constants of a material (derive_bsdf): the values evaluate_material, sample_bxdf and bxdf_eval_sampled rebuilt from it
+// on every hit, computed once per call by derive_bsdf so that the three cannot drift apart.  They are derived, not loaded from a
+// per-material table: the shading pass waits on memory latency, and loading them at any of the call sites measured slower on an
+// H100 than the arithmetic it saves (DESIGN.md section 4).
+struct Bsdf
+{
+    f3 f0;                         // mix(ior_to_f0(1, ior), specular_albedo, metalness)
+    f3 diffuse_mix;                // (1 - metalness) * diffuse_albedo
+    f3 specular_mix;               // mix(specular_albedo, 1, metalness)
+    f3 diffuse_lambert;            // diffuse_mix * (1 / pi)
+    float diffuse_weight;          // luma(diffuse_mix): sample_bxdf's diffuse lobe weight when the Fresnel term is 0
+};
+
 // kernels/common/material.h:319-369
 __device__ __forceinline__ f3 sample_texture(const DevScene& sc, uint32_t tex_idx, f2 uv)
 {
@@ -217,6 +230,21 @@ __device__ __forceinline__ f3 pow3(f3 a, float e) { return mk3(rt_powf(a.x, e), 
 __device__ __forceinline__ f3 unpack_rgb8(uint32_t d)
 {
     return mk3((float)(d & 0xFF), (float)((d >> 8) & 0xFF), (float)((d >> 16) & 0xFF)) / 255.0f;
+}
+
+__device__ __forceinline__ float luma(f3 c) { return dot(c, mk3(0.299f, 0.587f, 0.114f)); }
+__device__ __forceinline__ float ior_to_f0(float a, float b) { float r = (b - a) / (b + a); return r * r; }
+
+// The per-material values of material.h:132-241 that do not depend on the hit's directions, in the reference's operation order.
+__device__ __forceinline__ Bsdf derive_bsdf(const Material& m)
+{
+    Bsdf d;
+    d.f0 = mix(splat(ior_to_f0(1.0f, m.ior)), m.specular_albedo, m.metalness);
+    d.diffuse_mix = (1.0f - m.metalness) * m.diffuse_albedo;
+    d.specular_mix = mix(m.specular_albedo, splat(1.0f), m.metalness);
+    d.diffuse_lambert = d.diffuse_mix * RT_INV_PI;
+    d.diffuse_weight = luma(d.diffuse_mix);
+    return d;
 }
 
 // kernels/common/material.h:251-264 (OpenCL branch), utils.h:123-190
@@ -263,7 +291,6 @@ __device__ __forceinline__ Material load_material(const DevScene& sc, uint32_t m
 }
 
 // kernels/common/bxdf.h:57-61, 71-74, 90-95, 104-119; utils.h:83-86, 99-111
-__device__ __forceinline__ float ior_to_f0(float a, float b) { float r = (b - a) / (b + a); return r * r; }
 __device__ __forceinline__ f3 fresnel_schlick(f3 f0, float h_dot_o) { return f0 + (1.0f - f0) * rt_powf(1.0f - h_dot_o, 5.0f); }
 __device__ __forceinline__ float ggx_d(float alpha, float n_dot_h)
 {
@@ -278,7 +305,6 @@ __device__ __forceinline__ float v_smith_ggx_correlated(float n_dot_i, float n_d
     float ll = n_dot_i * sqrtf((-n_dot_o * a2 + n_dot_o) * n_dot_o + a2);
     return 0.5f / (lv + ll);
 }
-__device__ __forceinline__ float luma(f3 c) { return dot(c, mk3(0.299f, 0.587f, 0.114f)); }
 __device__ __forceinline__ f3 reflect(f3 v, f3 n) { return v - 2.0f * dot(v, n) * n; }
 
 // tangent frame of utils.h:99-106 / bxdf.h:163-165
@@ -290,7 +316,7 @@ __device__ __forceinline__ void tangent_frame(f3 n, f3& t, f3& b)
 }
 
 // kernels/common/material.h:132-169
-__device__ __forceinline__ f3 evaluate_material(const Material& m, f3 normal, f3 incoming, f3 outgoing)
+__device__ __forceinline__ f3 evaluate_material(const Material& m, const Bsdf& d, f3 normal, f3 incoming, f3 outgoing)
 {
     if (m.transparency < 0.5f) return mk3(0.0f, 0.0f, 0.0f);
     f3 half_vec = normalize(incoming + outgoing);
@@ -299,33 +325,46 @@ __device__ __forceinline__ f3 evaluate_material(const Material& m, f3 normal, f3
     float n_dot_h = fmaxf(dot(normal, half_vec), RT_EPS);
     float h_dot_o = fmaxf(dot(half_vec, outgoing), RT_EPS);
     float alpha = m.roughness * m.roughness;
-    float f0_dielectric = ior_to_f0(1.0f, m.ior);
-    f3 f0 = mix(splat(f0_dielectric), m.specular_albedo, m.metalness);
-    f3 diffuse_color = (1.0f - m.metalness) * m.diffuse_albedo;
-    f3 fresnel = fresnel_schlick(f0, h_dot_o);
+    f3 fresnel = fresnel_schlick(d.f0, h_dot_o);
     float specular = ggx_d(alpha, n_dot_h) * v_smith_ggx_correlated(n_dot_i, n_dot_o, alpha);
-    f3 diffuse = diffuse_color * RT_INV_PI;
+    f3 diffuse = d.diffuse_lambert;
     return fresnel * specular + (1.0f - fresnel) * diffuse;
 }
 
 // kernels/common/material.h:171-241 with SampleDiffuse :51-64, SampleSpecular :66-103,
 // SampleTransparency :105-117, SampleHemisphereCosine bxdf.h:33-54, GGX_Sample bxdf.h:157-168
 // (cos_theta's fp64 sub-expression kept in double).
-__device__ __forceinline__ f3 sample_bxdf(float s1, f2 s, Material m, f3 normal, f3 incoming, bool white_furnace,
+__device__ __forceinline__ f3 sample_bxdf(float s1, f2 s, Material m, Bsdf d, f3 normal, f3 incoming, bool white_furnace,
                                           f3& outgoing, float& pdf, float& offset)
 {
-    if (white_furnace) { m.diffuse_albedo = splat(1.0f); m.specular_albedo = splat(1.0f); }
+    if (white_furnace) { m.diffuse_albedo = splat(1.0f); m.specular_albedo = splat(1.0f); d = derive_bsdf(m); }
     float alpha = m.roughness * m.roughness;
-    float f0_dielectric = ior_to_f0(1.0f, m.ior);
-    f3 f0 = mix(splat(f0_dielectric), m.specular_albedo, m.metalness);
-    f3 diffuse_albedo = (1.0f - m.metalness) * m.diffuse_albedo;
-    f3 specular_albedo = mix(m.specular_albedo, splat(1.0f), m.metalness);
-    f3 fresnel = fresnel_schlick(f0, dot(normal, incoming)) * specular_albedo;
-    float specular_weight = luma(specular_albedo * fresnel);
-    float diffuse_weight = luma(diffuse_albedo * (1.0f - fresnel));
-    float weight_sum = diffuse_weight + specular_weight;
-    float specular_pdf = specular_weight / weight_sum;
-    float diffuse_pdf = diffuse_weight / weight_sum;
+    const float n_dot_in = dot(normal, incoming);
+    // Lobe weights without specular (every CornellBox material): when specular_mix is exactly (0, 0, 0) the general rule below gives
+    // fresnel = +-0, specular_pdf = +-0 and diffuse_pdf = 1, bit for bit, as long as
+    //   - fresnel_schlick(f0, n.i) is finite: f0 is in [0, 1] and |n.i| <= 2 keeps (1 - n.i)^5 below 243, so x * 0 is +-0 for it;
+    //   - diffuse_weight = luma(diffuse_mix * (1 - +-0)) = luma(diffuse_mix): 1 - +-0 = 1, and x * 1 = x;
+    //   - specular_weight = luma(0 * +-0) = +-0, so weight_sum = w + +-0 = w, specular_pdf = +-0 / w = +-0 and diffuse_pdf = w / w = 1
+    //     for a finite nonzero w.
+    // The fast path takes +0 for fresnel and specular_pdf.  The sign of a zero changes nothing: s1 <= +-0 is the same test for
+    // every s1 (s1 = 0 takes the specular lobe in both), and that lobe's pdf is then pdf * +-0, never > 0, so neither its bxdf
+    // nor its pdf reaches a continuation ray; in the diffuse lobe 1 - +-0 = 1.  A NaN n.i, or a zero or non-finite diffuse
+    // weight, takes the general path.
+    const bool no_specular = d.specular_mix.x == 0.0f && d.specular_mix.y == 0.0f && d.specular_mix.z == 0.0f &&
+                             fabsf(n_dot_in) <= 2.0f && d.diffuse_weight > 0.0f && d.diffuse_weight <= 3.402823466e38f;
+    f3 fresnel;
+    float specular_pdf, diffuse_pdf;
+    if (no_specular)
+    { fresnel = splat(0.0f); specular_pdf = 0.0f; diffuse_pdf = 1.0f; }
+    else
+    {
+        fresnel = fresnel_schlick(d.f0, n_dot_in) * d.specular_mix;
+        float specular_weight = luma(d.specular_mix * fresnel);
+        float diffuse_weight = luma(d.diffuse_mix * (1.0f - fresnel));
+        float weight_sum = diffuse_weight + specular_weight;
+        specular_pdf = specular_weight / weight_sum;
+        diffuse_pdf = diffuse_weight / weight_sum;
+    }
     offset = 1.0f;
     if (m.transparency < 0.5f)
     {
@@ -376,7 +415,7 @@ __device__ __forceinline__ f3 sample_bxdf(float s1, f2 s, Material m, f3 normal,
         f3 t, b;
         tangent_frame(normal, t, b);
         outgoing = normalize(b * tbn.x + t * tbn.y + normal * tbn.z);
-        bxdf = (1.0f - fresnel) * (diffuse_albedo * RT_INV_PI) * fmaxf(dot(outgoing, normal), 0.0f);
+        bxdf = (1.0f - fresnel) * d.diffuse_lambert * fmaxf(dot(outgoing, normal), 0.0f);
         pdf *= diffuse_pdf;
     }
     return bxdf;
@@ -391,23 +430,19 @@ __device__ __forceinline__ f3 sample_bxdf(float s1, f2 s, Material m, f3 normal,
 //   p_b  = (n.h > 0 and h.o > 0 ? specular_pdf * (D * n.h / (4 * h.o)) : 0) + diffuse_pdf * (max(n.o, 0) * (1 / pi))
 // The specular terms are 0 when alpha <= 1e-4 (a delta lobe, left to BSDF sampling).  `spec_pdf` and `alpha` let the caller tell
 // whether the lobe sample_bxdf picked with s1 was a delta.
-__device__ __forceinline__ f3 bxdf_eval_sampled(const Material& m, f3 normal, f3 incoming, f3 o, float& p_b, float& spec_pdf, float& alpha)
+__device__ __forceinline__ f3 bxdf_eval_sampled(const Material& m, const Bsdf& d, f3 normal, f3 incoming, f3 o, float& p_b, float& spec_pdf, float& alpha)
 {
     alpha = m.roughness * m.roughness;
-    float f0_dielectric = ior_to_f0(1.0f, m.ior);
-    f3 f0 = mix(splat(f0_dielectric), m.specular_albedo, m.metalness);
-    f3 diffuse_albedo = (1.0f - m.metalness) * m.diffuse_albedo;
-    f3 specular_albedo = mix(m.specular_albedo, splat(1.0f), m.metalness);
-    f3 fresnel = fresnel_schlick(f0, dot(normal, incoming)) * specular_albedo;
-    float specular_weight = luma(specular_albedo * fresnel);
-    float diffuse_weight = luma(diffuse_albedo * (1.0f - fresnel));
+    f3 fresnel = fresnel_schlick(d.f0, dot(normal, incoming)) * d.specular_mix;
+    float specular_weight = luma(d.specular_mix * fresnel);
+    float diffuse_weight = luma(d.diffuse_mix * (1.0f - fresnel));
     float weight_sum = diffuse_weight + specular_weight;
     spec_pdf = specular_weight / weight_sum;
     float diffuse_pdf = diffuse_weight / weight_sum;
     p_b = 0.0f;
     if (m.transparency < 0.5f) return splat(0.0f);
     const float cos_o = fmaxf(dot(o, normal), 0.0f);
-    f3 g = (1.0f - fresnel) * (diffuse_albedo * RT_INV_PI) * cos_o;
+    f3 g = (1.0f - fresnel) * d.diffuse_lambert * cos_o;
     float ps = 0.0f;
     if (alpha > 1e-4f)
     {
@@ -438,8 +473,9 @@ __device__ __forceinline__ float mis_power(float p, float q)
 
 // kernels/common/light.h:30-65 followed by hit_surface.cl:122-123 (length + normalize of the direction).
 // For directional lights `outgoing = origin * MAX_RENDER_DIST`, its length and its normalisation are constants
-// of the light: computed once at upload with the same operations (rt_bvh_layout.h).
-__device__ __forceinline__ f3 light_sample(const DevScene& sc, f3 position, float s, f3& outgoing_n, float& distance, float& pdf)
+// of the light: computed once at upload with the same operations (rt_bvh_layout.h).  `directional` is the index of the
+// light's record when the light is directional (its record holds outgoing_n and distance), else -1.
+__device__ __forceinline__ f3 light_sample(const DevScene& sc, f3 position, float s, f3& outgoing_n, float& distance, float& pdf, int& directional)
 {
     int n = (int)sc.light_count;
     int idx = (int)(s * (float)sc.light_count);
@@ -453,9 +489,11 @@ __device__ __forceinline__ f3 light_sample(const DevScene& sc, f3 position, floa
         radiance = radiance / dot(to_light, to_light);
         distance = length(to_light);
         outgoing_n = normalize(to_light);
+        directional = -1;
     }
     else
     {
+        directional = idx;
         outgoing_n = mk3(l0);
         distance = l0.w;
     }

@@ -228,13 +228,15 @@ __device__ __forceinline__ void shadow_group_regen(const FrameParams& p, const D
     uint32_t bounce = 0;
     if (i < n)
     {
-        const float4 a = q.sA[base + i], b = q.sB[base + i];
+        const float4 a = q.sA[base + i];
+        uint32_t li;
+        const float4 b = shadow_dir(p, sc, q, base + i, __float_as_uint(a.w), li);
         float bu, bv, bt;
         un = trace_staged<true, false, SMEM, true>(sc, mode, s_bvh, a, b, bu, bv, bt, nv, nt) == RT_INVALID_ID;
         if (un)
         {
             const float4 c = q.sC[base + i];
-            add_radiance(radiance, local_index(p, __float_as_uint(a.w)), mk3(c));
+            add_radiance(radiance, li, mk3(c));
             bounce = __float_as_uint(c.w) & 0xFFu;
         }
     }
@@ -278,9 +280,7 @@ __device__ __forceinline__ bool shade_hit_regen(const FrameParams& p, const DevS
     if (ss)
     {
         const uint32_t si = base + (uint32_t)slot + __popc(smask & lt_mask);
-        q.sA[si] = make_float4(so.s_origin.x, so.s_origin.y, so.s_origin.z, __uint_as_float(pixel));
-        q.sB[si] = make_float4(so.s_dir.x, so.s_dir.y, so.s_dir.z, so.s_tmax);
-        q.sC[si] = make_float4(so.s_sample.x, so.s_sample.y, so.s_sample.z, __uint_as_float(state));
+        put_shadow(p, q, si, li, so.s_light, so.s_origin, so.s_dir, so.s_tmax, so.s_sample, state);
     }
     if (cont)
     {

@@ -125,6 +125,39 @@ __device__ __forceinline__ uint32_t warp_grab(uint32_t* cursor)
     return __shfl_sync(0xffffffffu, at, 0);
 }
 
+// Shadow-ray records.  sA = (origin.xyz, word), sC = (light sample.xyz, path state or 0), and sB = (dir.xyz, t_max) only where the
+// light does not fix them: for a directional light they are its record light_rec[2 * l] (light_sample), which the shadow pass
+// reads in place of sB.  The word is the local pixel index (low 24 bits) and the light byte l (high 8 bits); RT_SHADOW_3PLANE
+// marks every other ray (point lights, emitter and environment samples, lights from index 255 on), whose sB is stored.  Partitions
+// of 2^24 local pixels or more store every ray with three planes and the whole local index in the word.
+#define RT_SHADOW_3PLANE 0xFFu
+__device__ __forceinline__ bool shadow_two_plane(const FrameParams& p) { return p.n_local <= (1u << 24); }
+__device__ __forceinline__ uint32_t shadow_word(const FrameParams& p, uint32_t li, uint32_t light)
+{
+    return shadow_two_plane(p) ? li | (light << 24) : li;
+}
+// Writes the shadow ray of local pixel li in slot si; sB only for a three-plane record
+__device__ __forceinline__ void put_shadow(const FrameParams& p, const Queues& q, uint32_t si, uint32_t li, uint32_t light, f3 o, f3 d, float t_max,
+                                           f3 sample, uint32_t c_w)
+{
+    q.sA[si] = make_float4(o.x, o.y, o.z, __uint_as_float(shadow_word(p, li, light)));
+    if (!shadow_two_plane(p) || light == RT_SHADOW_3PLANE) q.sB[si] = make_float4(d.x, d.y, d.z, t_max);
+    q.sC[si] = make_float4(sample.x, sample.y, sample.z, __uint_as_float(c_w));
+}
+// The (dir.xyz, t_max) plane of the shadow ray in slot si whose sA word is w, and its local pixel li
+__device__ __forceinline__ float4 shadow_dir(const FrameParams& p, const DevScene& sc, const Queues& q, uint32_t si, uint32_t w, uint32_t& li)
+{
+    if (shadow_two_plane(p))
+    {
+        li = w & 0xFFFFFFu;
+        const uint32_t light = w >> 24;
+        if (light != RT_SHADOW_3PLANE) return __ldg(sc.light_rec + (size_t)light * 2);
+        return q.sB[si];
+    }
+    li = w;
+    return q.sB[si];
+}
+
 __device__ __forceinline__ float4 add_radiance(float4* radiance, uint32_t li, f3 v)
 {
     float4 r = radiance[li];

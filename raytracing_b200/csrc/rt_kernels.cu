@@ -10,9 +10,9 @@
  *   extension-ray queue q[b&1]:  A = (origin.xyz, pixel_idx bits)
  *                                B = (dir.xyz, t_max)
  *                                C = (path throughput.xyz, -)
- *   shadow-ray queue:            A = (origin.xyz, pixel_idx bits)
- *                                B = (dir.xyz, t_max = distance to light)
- *                                C = (light sample.xyz, -)
+ *   shadow-ray queue:            A = (origin.xyz, local pixel index | light byte << 24)
+ *                                B = (dir.xyz, t_max = distance to light), not stored for a directional light
+ *                                C = (light sample.xyz, 0 or path state)          (rt_kernel_types.cuh, put_shadow)
  *   hit queue:                   (bc.x, bc.y, primitive_id bits, ray slot bits)   — rays that hit, compacted
  *   miss queue:                  ray slot (uint32)                                — rays that missed, compacted
  *   hits (stepwise path only):   (bc.x, bc.y, primitive_id bits, t)
@@ -100,6 +100,7 @@ struct ShadeOut
     bool spawn_shadow, spawn_next, emissive;
     f3 emission_add;
     f3 s_origin, s_dir, s_sample; float s_tmax;
+    uint32_t s_light;              // the shadow ray's light record when s_dir and s_tmax are those of a directional light, else RT_SHADOW_3PLANE
     f3 n_origin, n_dir, n_throughput;
     float n_pdf;                   // C.w of the continuation ray: its p_b with emitter or environment sampling on, else 0
 };
@@ -151,6 +152,8 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         out.emissive = false;
         out.spawn_shadow = out.spawn_next = true;
         out.s_origin = position; out.s_dir = mk3(q3) + mk3(q4) + mk3(q5) + mk3(q1.w, q2.w, q3.w); out.s_tmax = s + m2.x;
+        // a scene whose first light is directional stores two planes, as the renderer does
+        out.s_light = __float_as_uint(__ldg(sc.light_rec + 1).w) == RT_LIGHT_TYPE_DIRECTIONAL ? 0u : RT_SHADOW_3PLANE;
         out.s_sample = hit_throughput * mk3(m0);
         out.n_origin = position; out.n_dir = -ray_dir; out.n_throughput = hit_throughput * mk3(m0); out.n_pdf = prev_pdf + q4.w + q5.w;
         (void)ray_origin; (void)aov;
@@ -239,6 +242,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
     }
     uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx + sample_offset);
     out.spawn_shadow = false;
+    out.s_light = RT_SHADOW_3PLANE;
     bool pick_emitter = false, pick_env = false;
     if (EMIT && emit_on)
     {   // light kind (rt_set_light_selection): emitter iff P_e >= 1 or c < P_e, else environment iff the analytic weight is 0 or
@@ -283,7 +287,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         {
             const float p_l = __ldg(sc.emit_pdfA + t) * d2 / cos_e;
             float p_b, spec_pdf, alpha;
-            const f3 g = bxdf_eval_sampled(material, normal, incoming, w, p_b, spec_pdf, alpha);
+            const f3 g = bxdf_eval_sampled(material, derive_bsdf(material), normal, incoming, w, p_b, spec_pdf, alpha);
             const f3 ls = hit_throughput * g * le * (mis_power(p_l, p_b) / p_l);
             out.spawn_shadow = (p_l > 0.0f) && (dot(ls, ls) > 0.0f);
             out.s_origin = o;
@@ -301,7 +305,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         const float p_v = rtenv::pdf_dir(sc.env_pdf, sc.env_w, sc.env_h, w.x, w.y, w.z);
         const f3 le = sample_sky(sc, w);
         float p_b, spec_pdf, alpha;
-        const f3 g = bxdf_eval_sampled(material, normal, incoming, w, p_b, spec_pdf, alpha);
+        const f3 g = bxdf_eval_sampled(material, derive_bsdf(material), normal, incoming, w, p_b, spec_pdf, alpha);
         const f3 ls = hit_throughput * g * le * (mis_power(p_v, p_b) / p_v);
         out.spawn_shadow = (p_v > 0.0f) && (dot(ls, ls) > 0.0f);
         out.s_origin = position + geometry_normal * RT_EPS;
@@ -312,19 +316,25 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx + sample_offset, bounce * 5u + SAMPLE_LIGHT)
                              : sample_random(pixel_seed, bounce, SAMPLE_LIGHT);
         f3 outgoing; float pdf, distance_to_light;
-        f3 light_radiance = light_sample(sc, position, s_light, outgoing, distance_to_light, pdf);
+        int directional;
+        f3 light_radiance = light_sample(sc, position, s_light, outgoing, distance_to_light, pdf, directional);
         // light_sample = L * throughput * brdf / pdf * max(n.l, 0); a shadow ray is spawned iff pdf > 0 and
         // dot(sample, sample) > 0 (hit_surface.cl:127-129).  When max(n.l, 0) is 0 every component of the sample is
         // +-0 or NaN whatever the BRDF evaluates to, so the ray is never spawned: the BRDF evaluation is skipped then.
         const float cos_l = fmaxf(dot(outgoing, normal), 0.0f);
         if (cos_l > 0.0f)
         {
-            f3 brdf = evaluate_material(material, normal, incoming, outgoing);
-            f3 ls = light_radiance * hit_throughput * brdf / pdf * cos_l;
+            f3 brdf = evaluate_material(material, derive_bsdf(material), normal, incoming, outgoing);
+            // one light: pdf = 1 / 1 = 1 and x / 1 = x for every x but a NaN, whose quotient may carry other NaN bits; a sample with a
+            // NaN component is never stored (dot(ls, ls) > 0 is false), so the division is skipped
+            f3 ls = light_radiance * hit_throughput * brdf;
+            if (sc.light_count != 1u) ls = ls / pdf;
+            ls = ls * cos_l;
             if (EMIT && emit_on) ls = ls / (1.0f - sc.light_pev);
             out.spawn_shadow = (pdf > 0.0f) && (dot(ls, ls) > 0.0f);
             out.s_origin = position + normal * RT_EPS;
             out.s_dir = outgoing; out.s_tmax = distance_to_light; out.s_sample = ls;
+            out.s_light = directional >= 0 && directional < (int)RT_SHADOW_3PLANE ? (uint32_t)directional : RT_SHADOW_3PLANE;
         }
     }
     {   // BSDF sampling
@@ -343,7 +353,8 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         }
         float pdf = 0.0f, offset = 1.0f;
         f3 outgoing = mk3(0.0f, 0.0f, 0.0f);
-        f3 bxdf = sample_bxdf(s1, s, material, normal, incoming, p.white_furnace != 0, outgoing, pdf, offset);
+        // (derived here, not loaded: holding loaded constants from here on costs k_shade_queues spills at its 80 registers)
+        f3 bxdf = sample_bxdf(s1, s, material, derive_bsdf(material), normal, incoming, p.white_furnace != 0, outgoing, pdf, offset);
         f3 throughput = splat(0.0f);
         if (pdf > 0.0f) throughput = bxdf / pdf;
         out.n_throughput = hit_throughput * throughput;
@@ -354,7 +365,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         if (EMIT && emit_on)
         {   // the continuation's p_b for the MIS weight of an emitter it hits or of the sky it misses into (0 after a delta lobe)
             float p_b, spec_pdf, alpha;
-            bxdf_eval_sampled(material, normal, incoming, outgoing, p_b, spec_pdf, alpha);
+            bxdf_eval_sampled(material, derive_bsdf(material), normal, incoming, outgoing, p_b, spec_pdf, alpha);
             const bool delta = material.transparency < 0.5f || (s1 <= spec_pdf && alpha <= 1e-4f);
             out.n_pdf = delta ? 0.0f : p_b;
         }
@@ -428,10 +439,12 @@ __device__ __forceinline__ void shadow_group(const FrameParams& p, const Scene& 
     bool un = false;
     if (i < n)
     {
-        const float4 a = q.sA[base + i], b = q.sB[base + i];
+        const float4 a = q.sA[base + i];
+        uint32_t li;
+        const float4 b = shadow_dir(p, sc, q, base + i, __float_as_uint(a.w), li);
         float bu, bv, bt;
         un = trace_staged<true, COUNT, SMEM, PIN>(sc, mode, s_bvh, a, b, bu, bv, bt, nv, nt) == RT_INVALID_ID;
-        if (un) add_radiance(radiance, local_index(p, __float_as_uint(a.w)), mk3(q.sC[base + i]));
+        if (un) add_radiance(radiance, li, mk3(q.sC[base + i]));
     }
     warp_count(n_unoccluded, un);
 }
@@ -472,6 +485,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
     ShadeOut so;
     so.emissive = so.spawn_next = so.spawn_shadow = false;
     pixel = 0;
+    uint32_t li = 0;
     if (hit)
     {   // plane A (the origin) only where shade_hit reads it: the depth AOV of bounce 0 and, with EMIT, the MIS weight of an emitter
         // hit by a BSDF-sampled ray (never at bounce 0: C.w of a primary ray is 0).  Plane C is (1, 1, 1, 0) at bounce 0.
@@ -481,7 +495,8 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
         const float4 a = origin ? q.A[in][base + i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         pixel = __float_as_uint(b.w);
         shade_hit<EMIT, INST>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, 0u, so);
-        if (so.emissive) add_radiance(radiance, local_index(p, pixel), so.emission_add);
+        li = local_index(p, pixel);
+        if (so.emissive) add_radiance(radiance, li, so.emission_add);
     }
     const bool ss = hit && so.spawn_shadow, sn = hit && so.spawn_next;
     const unsigned smask = __ballot_sync(0xffffffffu, ss), nmask = __ballot_sync(0xffffffffu, sn);
@@ -502,9 +517,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
     if (ss)
     {
         const uint32_t si = base + (uint32_t)slot + __popc(smask & lt_mask);
-        q.sA[si] = make_float4(so.s_origin.x, so.s_origin.y, so.s_origin.z, __uint_as_float(pixel));
-        q.sB[si] = make_float4(so.s_dir.x, so.s_dir.y, so.s_dir.z, so.s_tmax);
-        q.sC[si] = make_float4(so.s_sample.x, so.s_sample.y, so.s_sample.z, 0.0f);
+        put_shadow(p, q, si, li, so.s_light, so.s_origin, so.s_dir, so.s_tmax, so.s_sample, 0u);
     }
     if (STAGE)
     {
@@ -613,7 +626,9 @@ __global__ void __launch_bounds__(256) k_intersect_shadow(FrameParams p, SceneOf
     uint32_t nv = 0, nt = 0;
     if (i < n)
     {
-        float4 a = q.sA[i], b = q.sB[i];
+        const float4 a = q.sA[i];
+        uint32_t li;
+        const float4 b = shadow_dir(p, sc, q, i, __float_as_uint(a.w), li);
         float bu, bv, bt;
         q.shadow_flags[i] = trace_staged<true, COUNT, INST ? RT_SMEM_INST : 0, false>(sc, mode, nullptr, a, b, bu, bv, bt, nv, nt);
     }
@@ -629,7 +644,7 @@ __global__ void __launch_bounds__(256) k_accumulate(FrameParams p, Queues q, Dev
     if (i < n)
     {
         un = q.shadow_flags[i] == RT_INVALID_ID;
-        if (un) add_radiance(radiance, local_index(p, __float_as_uint(q.sA[i].w)), mk3(q.sC[i]));
+        if (un) add_radiance(radiance, shadow_two_plane(p) ? __float_as_uint(q.sA[i].w) & 0xFFFFFFu : __float_as_uint(q.sA[i].w), mk3(q.sC[i]));
     }
     warp_count(&ctr->n_unoccluded[bounce], un);
 }

@@ -1,8 +1,13 @@
 """
-Extension-ray queue bytes per frame, pass by pass: the layout before the pixel moved from plane A to plane B (every primary ray
-written whole by k_raygen, every shaded entry reading planes A, B and C) against the current one (primary rays generated in the
-bounce-0 traversal, which stores plane B only; the shading pass reads B, and C after bounce 0, and A only for the depth AOV at
-bounce 0 or the emitter MIS term after it).  A byte model from the per-bounce counters, not a measurement: queue planes are 16 B
+Ray queue bytes per frame, pass by pass, for three layouts:
+  - "raygen": before the pixel moved from plane A to plane B (every primary ray written whole by k_raygen, every shaded entry
+    reading planes A, B and C, every shadow ray three planes);
+  - "3-plane": primary rays generated in the bounce-0 traversal, which stores plane B only; the shading pass reads B, and C after
+    bounce 0, and A only for the depth AOV at bounce 0 or the emitter MIS term after it; shadow rays still three planes;
+  - "now": as "3-plane", but a shadow ray toward a directional light stores planes sA and sC only, and the shadow pass reads sA
+    (and sC for an unoccluded ray), taking direction and t_max from the light's record.  Every light of the shipped scenes is
+    directional, so the model counts every shadow ray as two-plane.
+A byte model from the per-bounce counters, not a measurement: queue planes are 16 B
 float4s, hit-queue entries 16 B, miss-queue entries 4 B; BVH, material and radiance traffic is left out (the same in both).
 
     python tools/stream_bytes.py                          # the oracle's counters on the CPU (CornellBox, ShaderBalls)
@@ -38,8 +43,9 @@ def counters(name, device):
     return mb, {k: np.asarray(st[k][: mb + 1], dtype=np.int64) for k in ("n_ext", "n_miss", "n_shadow", "n_cont", "n_unoccluded")}
 
 
-def passes(mb, s, fused, aov=False, emit=False):
+def passes(mb, s, fused, aov=False, emit=False, two_plane=False):
     """Bytes per pass of one frame: (pass name, bytes read, bytes written)."""
+    shadow_planes = 2 if two_plane else 3
     out = []
     n0 = int(s["n_ext"][0])
     if not fused:
@@ -56,10 +62,10 @@ def passes(mb, s, fused, aov=False, emit=False):
             miss_planes = 1 if b == 0 else 2
         else:
             hit_planes = miss_planes = 3
-        written = 3 * PLANE * (int(s["n_shadow"][b]) + int(s["n_cont"][b]))
+        written = shadow_planes * PLANE * int(s["n_shadow"][b]) + 3 * PLANE * int(s["n_cont"][b])
         out.append(("shade %d" % b, (HITQ + hit_planes * PLANE) * hit + (MISSQ + miss_planes * PLANE) * miss, written))
         sh = int(s["n_shadow"][b])
-        out.append(("shadow %d" % b, 2 * PLANE * sh + PLANE * int(s["n_unoccluded"][b]), 0))
+        out.append(("shadow %d" % b, (shadow_planes - 1) * PLANE * sh + PLANE * int(s["n_unoccluded"][b]), 0))
     return out
 
 
@@ -71,25 +77,26 @@ def main():
     args = ap.parse_args()
     for name in args.scenes:
         mb, s = counters(name, args.device)
-        old, new = passes(mb, s, False), passes(mb, s, True)
-        print("%s (max_bounces %d, %s counters): extension rays per bounce %s" % (name, mb, "device" if args.device else "oracle",
-                                                                               s["n_ext"].tolist()))
-        print("  %-10s %14s %14s %14s" % ("pass", "before MB", "now MB", "saved MB"))
-        kinds = {}
-        for (p, r0, w0), (_, r1, w1) in zip([x for x in old if x[0] != "raygen"], new):
+        arms = (("raygen", passes(mb, s, False)), ("3-plane", passes(mb, s, True)), ("now", passes(mb, s, True, two_plane=True)))
+        print("%s (max_bounces %d, %s counters): extension rays per bounce %s, shadow rays %d (%d unoccluded)"
+              % (name, mb, "device" if args.device else "oracle", s["n_ext"].tolist(), int(s["n_shadow"].sum()), int(s["n_unoccluded"].sum())))
+        print("  %-10s" % "pass" + "".join("%14s" % (a + " MB") for a, _ in arms))
+        kinds, order = {}, []
+        for rows in zip(*[[x for x in ps if x[0] != "raygen"] for _, ps in arms]):
+            p = rows[0][0]
             k = p.split()[0] if not p.endswith(" 0") else p
-            a = kinds.setdefault(k, [0, 0])
-            a[0] += r0 + w0; a[1] += r1 + w1
+            if k not in kinds: kinds[k] = [0] * len(arms); order.append(k)
+            for j, (_, r, w) in enumerate(rows):
+                kinds[k][j] += r + w
             if args.per_pass:
-                print("  %-10s %14.1f %14.1f %14.1f" % (p, (r0 + w0) / 1e6, (r1 + w1) / 1e6, (r0 + w0 - r1 - w1) / 1e6))
-        rg = sum(r + w for p, r, w in old if p == "raygen")
-        print("  %-10s %14.1f %14.1f %14.1f" % ("raygen", rg / 1e6, 0.0, rg / 1e6))
-        for k, (a, b) in kinds.items():
-            print("  %-10s %14.1f %14.1f %14.1f" % (k, a / 1e6, b / 1e6, (a - b) / 1e6))
-        to = sum(r + w for _, r, w in old); tn = sum(r + w for _, r, w in new)
-        print("  %-10s %14.1f %14.1f %14.1f  (%.1f %% of the queue bytes)" % ("frame", to / 1e6, tn / 1e6, (to - tn) / 1e6,
-                                                                               100.0 * (to - tn) / to))
-
+                print("  %-10s" % p + "".join("%14.1f" % ((r + w) / 1e6) for _, r, w in rows))
+        rg = sum(r + w for p, r, w in arms[0][1] if p == "raygen")
+        print("  %-10s" % "raygen" + "%14.1f" % (rg / 1e6) + "%14.1f" % 0.0 * (len(arms) - 1))
+        for k in order:
+            print("  %-10s" % k + "".join("%14.1f" % (v / 1e6) for v in kinds[k]))
+        tot = [sum(r + w for _, r, w in ps) for _, ps in arms]
+        print("  %-10s" % "frame" + "".join("%14.1f" % (t / 1e6) for t in tot)
+              + "   (now saves %.1f MB = %.1f %% of the 3-plane layout's queue bytes)" % ((tot[1] - tot[2]) / 1e6, 100.0 * (tot[1] - tot[2]) / tot[1]))
 
 if __name__ == "__main__":
     main()
