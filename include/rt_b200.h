@@ -560,7 +560,8 @@ int rt_rebuild_bvh_ploc(rt_ctx* ctx, uint64_t* n_nodes);
  * uploaded flat, except where a signed zero or a NaN coordinate meets the matrix arithmetic (0 * x, -0 + 0).
  * Object motion (RT_OPT_OBJECT_MOTION): the previous transform M_prev of instance index i is its transform in the last earlier
  * rt_set_instances (since the upload) whose list had index i, or its current one if none had; the velocity AOV of a bounce-0 hit is
- * project(M * p) - project(M_prev * p), both points from the same object-space p, all float as the shading position.
+ * project(M * p) - project(M_prev * q), all float as the shading position, with q the hit's point on the mesh triangle's previous
+ * positions (the mesh-update block below; q = p until the mesh's first rt_update_mesh_triangles*).
  * Schedules: always the per-phase kernels (RT_OPT_FRAME_KERNEL has no effect), nothing staged (rt_bvh_staging reports mode 0;
  * RT_OPT_SMEM_BVH, RT_OPT_TOP_SMEM, RT_OPT_OCTANT_BVH and RT_OPT_TRAVERSAL have no effect).  Overlap modes, graphs, PDL, kernel
  * timing, traversal counting, the stepwise calls and rt_integrate_samples work.  Traversal counting counts each top-level box
@@ -577,6 +578,43 @@ typedef struct RtMeshDesc { uint64_t first_triangle, n_triangles, first_node, n_
 typedef struct RtInstance { float object_to_world[12]; uint32_t mesh; uint32_t padding[3]; } RtInstance;
 int rt_upload_instanced_scene(rt_ctx* ctx, const RtSceneDesc* scene, const RtMeshDesc* meshes, uint32_t n_meshes);
 int rt_set_instances(rt_ctx* ctx, const RtInstance* instances, uint32_t n_instances);
+
+/* ---- mesh updates in instanced scenes (new capability): deform one shared mesh in place, its tree refit on the device ----------
+ * triangles[i] replaces triangle first_triangle + i of mesh `mesh` (RtMeshDesc of the upload), in the mesh's own leaf order;
+ * n_triangles must equal the mesh's count.  The mesh's records (tris_ref, wtris, tri_shade) become what the upload derives, as
+ * rt_update_triangles defines them: mtlIndex and the padding are not read, the materials and end-of-leaf flags are kept.  The
+ * mesh's tree keeps its topology and is refit by the refit rule of the geometry-update block, over the mesh's nodes only; no other
+ * mesh's records are touched.  The refit root box is read back (32 bytes, so both variants block once for it) and becomes the
+ * mesh's root box: if an instance of the current list uses the mesh, the top-level tree is rebuilt from it by rt_set_instances'
+ * rule (raytracing_b200/csrc/rt_instances.h) for the current list, and only the header and the top-level records are rewritten.
+ * The instance records (W, M, bases), the previous transforms of object motion and the sort-key origin of the shading pass stay
+ * as they were.  So every output of a later frame is, bit for bit, that of rt_upload_instanced_scene with the refit nodes and the
+ * new triangles followed by the same rt_set_instances; only the order of the continuation rays may differ.  If no instance uses
+ * the mesh, only the mesh is written.
+ * Object motion (RT_OPT_OBJECT_MOTION): the context keeps the previous positions Q of every mesh triangle, by the flat rule of the
+ * object-motion block: Q = the positions before the last rt_update_mesh_triangles* of that mesh, the current ones after an upload
+ * and after turning the option on; rt_set_instances, frames, rt_reset and camera changes leave Q alone.  The velocity AOV of a
+ * bounce-0 hit on mesh triangle t of instance i at barycentrics (u, v), w0 = 1 - u - v, all float as the shading position:
+ *     q = (q1 * w0 + q2 * u) + q3 * v;  velocity = project(M_i * p) - project(M_prev,i * q)
+ * With Q equal to the current positions, q is the object-space hit point p bit for bit: nothing changes until a mesh update.
+ * Memory: 48 B per mesh triangle while the option is on.
+ * Validation: a position coordinate (xyz of v1, v2, v3) that is not finite is RT_ERR_INVALID_ARGUMENT and nothing is written
+ * (the upload refuses a mesh root box that is not finite).  rt_update_mesh_triangles checks on the host;
+ * rt_update_mesh_triangles_device runs a check kernel and reads back its flag (blocking) before anything is written.
+ * Ordering and buffers as for rt_update_triangles: a deferred shadow pass is launched first and the update is enqueued on the
+ * render stream; no buffer moves, so a captured frame graph stays valid; the refit kernels never trigger dependent launches.
+ * rt_update_mesh_triangles reads the caller's array before it returns, through rt_update_triangles' staging (at most 2 x 32 MB,
+ * allocated at the first host update of either kind); rt_update_mesh_triangles_device reads `device_triangles` (RtTriangle
+ * layout, 16-byte aligned device memory of the context's device) on the render stream, and the caller keeps it unchanged until
+ * the call returns.  The first update of a mesh builds its refit map (blocking; 12 B per node and 4 B per leaf of the mesh, plus
+ * one 4-byte flag for the device variant), which lives until the next upload.
+ * Errors: RT_ERR_NOT_READY without an instanced scene (none, or a flat one); RT_ERR_INVALID_ARGUMENT for a mesh index out of
+ * range, a count mismatch, a null pointer or a position that is not finite, and for the device variant a pointer that is not
+ * 16-byte aligned device memory of the context's device; RT_ERR_UNSUPPORTED for rt_update_mesh_triangles_device on a
+ * multi-device context (rt_update_mesh_triangles fans out).  The launches count under RT_K_MISC (RT_OPT_KERNEL_TIMING) and in
+ * rt_launch_count.  rt_update_triangles*, the rebuilds and rt_read_bvh stay RT_ERR_UNSUPPORTED on instanced scenes. */
+int rt_update_mesh_triangles(rt_ctx* ctx, uint32_t mesh, const RtTriangle* triangles, uint64_t n_triangles);
+int rt_update_mesh_triangles_device(rt_ctx* ctx, uint32_t mesh, const void* device_triangles, uint64_t n_triangles);
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

@@ -39,7 +39,8 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_gather_buffer", "rt_ipc_export", "rt_ipc_open", "rt_set_gather_target", "rt_gather_wait",
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
            "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh",
-           "rt_rebuild_bvh", "rt_bvh_staging", "rt_rebuild_bvh_ploc", "rt_upload_instanced_scene", "rt_set_instances"]
+           "rt_rebuild_bvh", "rt_bvh_staging", "rt_rebuild_bvh_ploc", "rt_upload_instanced_scene", "rt_set_instances",
+           "rt_update_mesh_triangles", "rt_update_mesh_triangles_device"]
 
 
 class RtSceneDesc(C.Structure):
@@ -132,6 +133,8 @@ def load_library():
     L.rt_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rt_upload_instanced_scene.argtypes = [C.c_void_p, C.POINTER(RtSceneDesc), C.c_void_p, C.c_uint32]
     L.rt_set_instances.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.rt_update_mesh_triangles.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64]
+    L.rt_update_mesh_triangles_device.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64]
     _lib = L
     return L
 
@@ -190,7 +193,8 @@ class Context:
         if world != 1:
             self._ck(self.lib.rt_set_partition(self.h, rank, world))
         self._keep = None
-        self._update_srcs = []              # (tensor, event on the render stream after its update): update_triangles
+        self._update_srcs = []              # (tensor, event on the render stream after its update): update_triangles,
+                                            # update_mesh_triangles
 
     def gather_radiance(self):
         self._ck(self.lib.rt_gather_radiance(self.h))
@@ -329,6 +333,17 @@ class Context:
         self._ck(self.lib.rt_set_light_selection(self.h, float(analytic), float(emitters), float(environment)))
 
     # ---- geometry updates
+    def update_mesh_triangles(self, mesh, tris):
+        """Replace the triangles of mesh `mesh` of an instanced scene (its leaf order, same count), refit its tree on the device and
+        rebuild the top-level tree (rt_update_mesh_triangles*).  `tris` is taken as by update_triangles: a TRIANGLE_DT array
+        through the host variant, or a contiguous CUDA torch tensor uint8 (n, 160) / float32 (n, 40), held as update_triangles
+        holds it.  The accumulation is kept: call reset()."""
+        if isinstance(tris, np.ndarray):
+            t = np.ascontiguousarray(tris, dtype=TRIANGLE_DT)
+            self._ck(self.lib.rt_update_mesh_triangles(self.h, int(mesh), t.ctypes.data, t.shape[0]))
+            return
+        self._device_update(tris, "update_mesh_triangles", lambda p, n: self.lib.rt_update_mesh_triangles_device(self.h, int(mesh), p, n))
+
     def update_triangles(self, tris):
         """Replace the uploaded triangles (leaf order, same count) and refit the BVH on the device (rt_update_triangles*).
         A TRIANGLE_DT numpy array goes through the host variant; a contiguous CUDA torch tensor (uint8 (n, 160) or float32
@@ -341,13 +356,18 @@ class Context:
             t = np.ascontiguousarray(tris, dtype=TRIANGLE_DT)
             self._ck(self.lib.rt_update_triangles(self.h, t.ctypes.data, t.shape[0]))
             return
+        self._device_update(tris, "update_triangles", lambda p, n: self.lib.rt_update_triangles_device(self.h, p, n))
+
+    def _device_update(self, tris, what, call):
+        """The device variant of an update: call(device pointer, n) on the render stream after torch's current stream, the tensor
+        held until an event after the call has completed (update_triangles)."""
         import torch
         if not (isinstance(tris, torch.Tensor) and tris.is_cuda and tris.is_contiguous() and tris.dim() == 2 and
                 ((tris.dtype == torch.uint8 and tris.shape[1] == 160) or (tris.dtype == torch.float32 and tris.shape[1] == 40))):
-            raise TypeError("update_triangles: a TRIANGLE_DT array, or a contiguous CUDA tensor uint8 (n, 160) / float32 (n, 40)")
+            raise TypeError(what + ": a TRIANGLE_DT array, or a contiguous CUDA tensor uint8 (n, 160) / float32 (n, 40)")
         render = torch.cuda.ExternalStream(self.stream_handle(), device=tris.device)
         render.wait_stream(torch.cuda.current_stream(tris.device))
-        self._ck(self.lib.rt_update_triangles_device(self.h, C.c_void_p(tris.data_ptr()), tris.shape[0]))
+        self._ck(call(C.c_void_p(tris.data_ptr()), tris.shape[0]))
         read = torch.cuda.Event()
         read.record(render)
         self._update_srcs = [(x, e) for x, e in self._update_srcs if not e.query()] + [(tris, read)]

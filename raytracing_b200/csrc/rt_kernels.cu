@@ -129,8 +129,8 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
 // EMIT: the scene has an active emitter table (sc.emit_*, RT_OPT_EMITTER_SAMPLING) or environment table (sc.env_*,
 // RT_OPT_ENV_SAMPLING), each read only while it exists; a template flag, so that the kernels without it are the code of both options off.
 // INST: an instanced scene (rt_b200.h): prim is a virtual id; the hit is shaded on its mesh triangle and moved to world space by the
-// instance's M (position) and W^T (normals); the AOV's previous position uses the instance's previous M (aov.prev_pos, 3 float4 per
-// instance) when object motion is on.
+// instance's M (position) and W^T (normals); the AOV's previous position places the mesh triangle's previous positions
+// (sc.prev_tri) by the instance's previous M (aov.prev_pos, 3 float4 per instance) when object motion is on.
 template <bool EMIT = false, bool INST = false>
 __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
                                           f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
@@ -184,6 +184,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
     f3 position = p1 * w0 + p2 * u + p3 * v;
     f3 normal;
     f3 obj_position = position;
+    f3 inst_prev = position;                          // INST: the velocity AOV's previous position (object motion)
     if constexpr (INST)
     {   // world space: position = M * p; normals = normalize(W^T * n), the geometric one from the unnormalised cross product (the
         // upload's normalize of it, when W is the identity) times sign(det M)
@@ -192,6 +193,15 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         position = xform_point(__ldg(ir + 3), __ldg(ir + 4), __ldg(ir + 5), obj_position);
         normal = normalize(xform_normal(wr0, wr1, wr2, n1 * w0 + n2 * u + n3 * v));
         geometry_normal = normalize(xform_normal(wr0, wr1, wr2, cross(p2 - p1, p3 - p1))) * __ldg(ir + 7).x;
+        if (bounce == 0 && aov.enabled && aov.prev_pos)
+        {   // object motion, for the AOV block below (here, where tri, u and v are live anyway: carrying them to the block costs the
+            // shading kernels spills): the mesh triangle's previous positions at the same barycentrics, placed by the instance's
+            // previous transform
+            const float4* qt = sc.prev_tri + (size_t)tri * 3;
+            const f3 q = mk3(__ldg(qt)) * w0 + mk3(__ldg(qt + 1)) * u + mk3(__ldg(qt + 2)) * v;
+            const float4* qp = aov.prev_pos + (size_t)inst * 3;
+            inst_prev = xform_point(__ldg(qp), __ldg(qp + 1), __ldg(qp + 2), q);
+        }
     }
     else normal = normalize(n1 * w0 + n2 * u + n3 * v);
     f2 texcoord; texcoord.x = 0.0f; texcoord.y = 0.0f;
@@ -210,11 +220,13 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         aov.normal[li] = make_float4(normal.x, normal.y, normal.z, 0.0f);
         f3 prev = position;
         if (aov.prev_pos)
-        {   // object motion: the same barycentrics on the triangle's previous positions (INST: the same object-space point under
-            // the instance's previous transform)
-            const float4* qp = aov.prev_pos + (size_t)(INST ? inst : prim) * 3;
-            if (INST) prev = xform_point(__ldg(qp), __ldg(qp + 1), __ldg(qp + 2), obj_position);
-            else prev = mk3(__ldg(qp)) * w0 + mk3(__ldg(qp + 1)) * u + mk3(__ldg(qp + 2)) * v;
+        {   // object motion: the same barycentrics on the triangle's previous positions (INST: computed above)
+            if constexpr (INST) prev = inst_prev;
+            else
+            {
+                const float4* qp = aov.prev_pos + (size_t)prim * 3;
+                prev = mk3(__ldg(qp)) * w0 + mk3(__ldg(qp + 1)) * u + mk3(__ldg(qp + 2)) * v;
+            }
         }
         f2 s0 = project_screen(position, p.dyn->cam), s1 = project_screen(prev, p.dyn->prev);
         aov.velocity[li] = make_float2(s0.x - s1.x, s0.y - s1.y);
@@ -1299,6 +1311,12 @@ struct rt_ctx
     std::vector<float4> inst_host;                 // the image of the instance buffer the last rt_set_instances copied
     float4 *inst_hdr = nullptr, *inst_top = nullptr, *inst_rec = nullptr, *inst_prev = nullptr;
     uint32_t* inst_base = nullptr;
+    std::vector<RtInstance> inst_list;             // the list of the last rt_set_instances (rt_update_mesh_triangles rebuilds its tree)
+    // rt_update_mesh_triangles: per mesh, its node count and its refit map (built at the mesh's first update, in tree_mem; node
+    // and record indices relative to the mesh's own arrays), and the device variant's check flag (one word, in tree_mem)
+    struct MeshRefit { uint64_t n_nodes = 0; uint2* link = nullptr; uint32_t* leaves = nullptr; uint32_t* arrivals = nullptr; uint32_t n_leaves = 0; };
+    std::vector<MeshRefit> mesh_refit;
+    uint32_t* mesh_bad = nullptr;
 
     // adaptive sampling (rt_set_adaptive_sampling): the requested setting, which rt_reset makes the active one; max_error > 0 = on.
     // The per-pixel state exists only while the active setting is on.
@@ -1633,6 +1651,7 @@ DevInstScene inst_scene(const rt_ctx* c)
     DevInstScene s;
     static_cast<DevScene&>(s) = c->scene;
     s.inst_hdr = c->inst_hdr; s.top = c->inst_top; s.irec = c->inst_rec; s.ibase = c->inst_base;
+    s.prev_tri = c->prev_pos;
     return s;
 }
 
@@ -2086,9 +2105,11 @@ static int upload_scene(rt_ctx* c, const RtSceneDesc* s, const RtMeshDesc* meshe
     c->analytic_lit = rtenv::analytic_lit(s->lights, s->scene_info.analytic_light_count);
     c->instanced = meshes != nullptr;
     c->inst_mem.clear(); c->inst_hdr = c->inst_top = c->inst_rec = c->inst_prev = nullptr; c->inst_base = nullptr;
-    c->inst_cap = c->n_inst = 0; c->inst_last.clear();
+    c->inst_cap = c->n_inst = 0; c->inst_last.clear(); c->inst_list.clear();
+    c->mesh_refit.clear(); c->mesh_bad = nullptr;
+    for (uint32_t k = 0; k < (meshes ? n_meshes : 0u); ++k) { rt_ctx::MeshRefit r; r.n_nodes = meshes[k].n_nodes; c->mesh_refit.push_back(r); }
     if (c->instanced && (rc = alloc_instances(c, 1))) return rc;          // no instances yet: every ray misses
-    if (!c->instanced && c->object_motion && (rc = set_prev_positions(c))) return rc;
+    if (c->object_motion && (rc = set_prev_positions(c))) return rc;
     c->scene_ready = true;
     ++c->config_gen;
     return refresh_lights(c);
@@ -2121,6 +2142,18 @@ int rt_upload_instanced_scene(rt_ctx* c, const RtSceneDesc* s, const RtMeshDesc*
     return upload_scene(c, s, meshes, n_meshes);
 }
 
+// The head of the instance buffer's image: the header (top-level root box, root reference, instance count) and the top-level
+// records, 2 + 4 (n - 1) float4 (2 for n <= 1).  rt_set_instances writes them with the rest of the image,
+// rt_update_mesh_triangles alone.
+static size_t top_level_image(const rtinst::Prepared& pr, uint32_t n, float4* h)
+{
+    const rtinst::Box& rb = pr.tree.root;
+    h[0] = make_float4(rb.lo[0], rb.lo[1], rb.lo[2], rtinst::int_bits(pr.tree.root_ref));
+    h[1] = make_float4(rb.hi[0], rb.hi[1], rb.hi[2], rtinst::int_bits((int)n));
+    memcpy(&h[2], pr.tree.records.data(), pr.tree.records.size() * 4);
+    return 2 + pr.tree.records.size() / 4;
+}
+
 int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
 {
     RT_CHECK_CTX(c); RT_FANOUT(c, rt_set_instances(k, instances, n));
@@ -2144,10 +2177,7 @@ int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
     const size_t f4 = 2 + top * 4 + (size_t)c->inst_cap * 11 + ((size_t)c->inst_cap + 3) / 4;
     std::vector<float4>& h = c->inst_host;
     h.assign(f4, make_float4(0.0f, 0.0f, 0.0f, 0.0f));
-    const rtinst::Box& rb = pr.tree.root;
-    h[0] = make_float4(rb.lo[0], rb.lo[1], rb.lo[2], rtinst::int_bits(pr.tree.root_ref));
-    h[1] = make_float4(rb.hi[0], rb.hi[1], rb.hi[2], rtinst::int_bits((int)n));
-    memcpy(&h[2], pr.tree.records.data(), pr.tree.records.size() * 4);
+    top_level_image(pr, n, h.data());
     float4* rec = &h[2 + top * 4];
     memcpy(rec, pr.rec.data(), pr.rec.size() * 4);
     float4* prev = rec + (size_t)c->inst_cap * 8;
@@ -2160,14 +2190,36 @@ int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
     RT_CUDA(c, cudaMemcpyAsync(c->inst_hdr, h.data(), f4 * 16, cudaMemcpyHostToDevice, c->stream));
     if (n > known) c->inst_last.resize((size_t)n * 12);
     for (uint32_t i = 0; i < n; ++i) memcpy(&c->inst_last[(size_t)i * 12], instances[i].object_to_world, 48);
+    c->inst_list.assign(instances, instances + n);
     c->n_inst = n;
     return RT_OK;
 }
 
 // ---- geometry updates: rt_update_triangles[_device], rt_read_bvh (include/rt_b200.h)
 
-// The checks both variants share, then the refit map (built from the device copy of the upload's nodes at the first update:
-// a refit rewrites only their boxes) and the ordering after earlier work.
+// The refit map of the n_nodes nodes at `nodes` (device memory; references relative to them), built from their device copy (a
+// refit rewrites only their boxes; blocking) into tree_mem: link and arrivals per node, the leaf list.
+static int build_refit_map(rt_ctx* c, const float4* nodes_dev, uint64_t n_nodes, const char* what, uint2*& link, uint32_t*& leaves,
+                           uint32_t*& arrivals, uint32_t& n_leaves)
+{
+    std::vector<RtLinearBVHNode> nodes(n_nodes);
+    RT_CUDA(c, cudaMemcpyAsync(nodes.data(), nodes_dev, n_nodes * sizeof(RtLinearBVHNode), cudaMemcpyDeviceToHost, c->stream));
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    rtbvh::RefitMap m;
+    rtbvh::build_refit_map(nodes.data(), n_nodes, m);
+    DevAllocs g;
+    uint2* l = nullptr; uint32_t *lv = nullptr, *ar = nullptr;
+    cudaError_t e;
+    if ((e = g.alloc(l, m.link.size() / 2)) || (e = g.alloc(lv, m.leaves.size())) || (e = g.alloc(ar, n_nodes)) ||
+        (e = cudaMemcpy(l, m.link.data(), m.link.size() * 4, cudaMemcpyHostToDevice)) ||
+        (e = cudaMemcpy(lv, m.leaves.data(), m.leaves.size() * 4, cudaMemcpyHostToDevice)))
+        RT_FAIL(c, RT_ERR_CUDA, "%s: refit map: %s", what, cudaGetErrorString(e));
+    c->tree_mem.adopt(std::move(g)); link = l; leaves = lv; arrivals = ar;
+    n_leaves = (uint32_t)m.leaves.size();
+    return RT_OK;
+}
+
+// The checks both variants share, then the refit map of the upload's tree (at the first update) and the ordering after earlier work.
 static int begin_update(rt_ctx* c, const void* triangles, uint64_t n, const char* what)
 {
     if (!c->scene_ready) RT_FAIL(c, RT_ERR_NOT_READY, "%s: rt_upload_scene has not been called", what);
@@ -2177,21 +2229,7 @@ static int begin_update(rt_ctx* c, const void* triangles, uint64_t n, const char
     RT_CUDA(c, cudaSetDevice(c->device));
     { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the geometry this call rewrites
     if (c->refit_link) return RT_OK;
-    std::vector<RtLinearBVHNode> nodes(c->n_nodes);
-    RT_CUDA(c, cudaMemcpyAsync(nodes.data(), c->scene.nodes_ref, c->n_nodes * sizeof(RtLinearBVHNode), cudaMemcpyDeviceToHost, c->stream));
-    RT_CUDA(c, cudaStreamSynchronize(c->stream));
-    rtbvh::RefitMap m;
-    rtbvh::build_refit_map(nodes.data(), c->n_nodes, m);
-    DevAllocs g;
-    uint2* link = nullptr; uint32_t *leaves = nullptr, *arrivals = nullptr;
-    cudaError_t e;
-    if ((e = g.alloc(link, m.link.size() / 2)) || (e = g.alloc(leaves, m.leaves.size())) || (e = g.alloc(arrivals, c->n_nodes)) ||
-        (e = cudaMemcpy(link, m.link.data(), m.link.size() * 4, cudaMemcpyHostToDevice)) ||
-        (e = cudaMemcpy(leaves, m.leaves.data(), m.leaves.size() * 4, cudaMemcpyHostToDevice)))
-        RT_FAIL(c, RT_ERR_CUDA, "%s: refit map: %s", what, cudaGetErrorString(e));
-    c->tree_mem.adopt(std::move(g)); c->refit_link = link; c->refit_leaves = leaves; c->refit_arrivals = arrivals;
-    c->refit_n_leaves = (uint32_t)m.leaves.size();
-    return RT_OK;
+    return build_refit_map(c, c->scene.nodes_ref, c->n_nodes, what, c->refit_link, c->refit_leaves, c->refit_arrivals, c->refit_n_leaves);
 }
 
 static int launch_refit_records(rt_ctx* c, const void* src, uint32_t first, uint32_t n)
@@ -2210,14 +2248,21 @@ static int launch_refit_records(rt_ctx* c, const void* src, uint32_t first, uint
 // The refit, then the emitter table of the moved geometry.  The two refit kernels are plain launches and never execute
 // griddepcontrol.launch_dependents: a traversal kernel launched with programmatic dependent launch stages the BVH before its
 // pdl_wait() (rt_traverse.cuh), so an early trigger would let the next frame stage stale boxes.
+static int launch_refit(rt_ctx* c, const uint32_t* leaves, uint32_t n_leaves, const uint2* link, uint32_t* arrivals, uint64_t n_nodes,
+                        const float4* nodes_ref, const float4* tris_ref, const float4* wnodes)
+{
+    RT_CUDA(c, cudaMemsetAsync(arrivals, 0, n_nodes * 4, c->stream));
+    TimedLaunch t(c, RT_K_MISC);
+    k_refit<<<grid_for(n_leaves), 256, 0, c->stream>>>(leaves, n_leaves, link, arrivals, (float*)nodes_ref, tris_ref, (float*)wnodes);
+    return post_launch(c, "k_refit");
+}
+
 static int finish_update(rt_ctx* c)
 {
-    RT_CUDA(c, cudaMemsetAsync(c->refit_arrivals, 0, c->n_nodes * 4, c->stream));
     {
-        TimedLaunch t(c, RT_K_MISC);
-        k_refit<<<grid_for(c->refit_n_leaves), 256, 0, c->stream>>>(c->refit_leaves, c->refit_n_leaves, c->refit_link, c->refit_arrivals,
-                                                                     (float*)c->scene.nodes_ref, c->scene.tris_ref, (float*)c->scene.wnodes);
-        int rc = post_launch(c, "k_refit"); if (rc) return rc;
+        int rc = launch_refit(c, c->refit_leaves, c->refit_n_leaves, c->refit_link, c->refit_arrivals, c->n_nodes, c->scene.nodes_ref,
+                              c->scene.tris_ref, c->scene.wnodes);
+        if (rc) return rc;
     }
     // scene_mid, the origin of k_shade_queues' sort key, stays that of the upload: it orders the continuation rays, which
     // changes no result.  The buffers keep their addresses, so a captured frame graph stays valid.
@@ -2225,10 +2270,9 @@ static int finish_update(rt_ctx* c)
     return (c->emitter_sampling && !c->emit_idx.empty()) ? refresh_lights(c) : RT_OK;
 }
 
-int rt_update_triangles(rt_ctx* c, const RtTriangle* triangles, uint64_t n)
+// The record kernel over the caller's triangles[0 .. n), written to triangles first .. first + n - 1, through the staging
+static int stage_records(rt_ctx* c, const RtTriangle* triangles, uint64_t n, uint64_t first_dst, const char* what)
 {
-    RT_CHECK_CTX(c); RT_FANOUT(c, rt_update_triangles(k, triangles, n));
-    { int rc = begin_update(c, triangles, n, "rt_update_triangles"); if (rc) return rc; }
     rt_ctx::Staging& sg = c->stage;
     if (!sg.host)
     {   // two halves of at most 32 MB each: the host copy into one half overlaps the upload and kernel of the other
@@ -2237,7 +2281,7 @@ int rt_update_triangles(rt_ctx* c, const RtTriangle* triangles, uint64_t n)
         cudaError_t e;
         if ((e = s.mem.alloc(s.host, 2 * s.half, true)) || (e = s.mem.alloc(s.dev, 2 * s.half)) || (e = make_event(s.copied[0])) ||
             (e = make_event(s.copied[1])))
-            RT_FAIL(c, RT_ERR_CUDA, "rt_update_triangles: staging buffers: %s", cudaGetErrorString(e));
+            RT_FAIL(c, RT_ERR_CUDA, "%s: staging buffers: %s", what, cudaGetErrorString(e));
         sg = std::move(s);
     }
     const uint64_t per_chunk = sg.half / sizeof(RtTriangle);
@@ -2249,26 +2293,141 @@ int rt_update_triangles(rt_ctx* c, const RtTriangle* triangles, uint64_t n)
         memcpy(h, triangles + first, (size_t)m * sizeof(RtTriangle));
         RT_CUDA(c, cudaMemcpyAsync(d, h, (size_t)m * sizeof(RtTriangle), cudaMemcpyHostToDevice, c->stream));
         RT_CUDA(c, cudaEventRecord(sg.copied[k], c->stream));
-        int rc = launch_refit_records(c, d, (uint32_t)first, m); if (rc) return rc;
+        int rc = launch_refit_records(c, d, (uint32_t)(first_dst + first), m); if (rc) return rc;
     }
+    return RT_OK;
+}
+
+int rt_update_triangles(rt_ctx* c, const RtTriangle* triangles, uint64_t n)
+{
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_update_triangles(k, triangles, n));
+    { int rc = begin_update(c, triangles, n, "rt_update_triangles"); if (rc) return rc; }
+    { int rc = stage_records(c, triangles, n, 0, "rt_update_triangles"); if (rc) return rc; }
     return finish_update(c);
 }
 
-int rt_update_triangles_device(rt_ctx* c, const void* triangles, uint64_t n)
+// The device variants take a single-device context and 16-byte aligned device memory of its device (a null pointer is left to the
+// caller's own check)
+static int check_device_triangles(rt_ctx* c, const void* triangles, const char* what, const char* host_variant)
 {
-    RT_CHECK_CTX(c);
     if (!c->children.empty())
-        RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_update_triangles_device: a multi-device context: use rt_update_triangles (device memory belongs to one device)");
+        RT_FAIL(c, RT_ERR_UNSUPPORTED, "%s: a multi-device context: use %s (device memory belongs to one device)", what, host_variant);
     if (triangles)
     {
         cudaPointerAttributes a = {};
         if (cudaPointerGetAttributes(&a, triangles) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
         if (a.type != cudaMemoryTypeDevice || a.device != c->device || ((uintptr_t)triangles & 15u))
-            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_update_triangles_device: not 16-byte aligned device memory of device %d", c->device);
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: not 16-byte aligned device memory of device %d", what, c->device);
     }
+    return RT_OK;
+}
+
+int rt_update_triangles_device(rt_ctx* c, const void* triangles, uint64_t n)
+{
+    RT_CHECK_CTX(c);
+    { int rc = check_device_triangles(c, triangles, "rt_update_triangles_device", "rt_update_triangles"); if (rc) return rc; }
     { int rc = begin_update(c, triangles, n, "rt_update_triangles_device"); if (rc) return rc; }
     { int rc = launch_refit_records(c, triangles, 0, (uint32_t)n); if (rc) return rc; }
     return finish_update(c);
+}
+
+// ---- mesh updates in instanced scenes: rt_update_mesh_triangles[_device] (include/rt_b200.h)
+
+// The argument checks both variants share (nothing is enqueued)
+static int check_mesh_update(rt_ctx* c, uint32_t mesh, const void* triangles, uint64_t n, const char* what)
+{
+    if (!c->scene_ready || !c->instanced) RT_FAIL(c, RT_ERR_NOT_READY, "%s: no instanced scene (rt_upload_instanced_scene)", what);
+    if (mesh >= c->meshes.size()) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: mesh %u of %zu", what, mesh, c->meshes.size());
+    if (!triangles) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: null triangles", what);
+    if (n != c->meshes[mesh].n_tris)
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: %llu triangles, mesh %u has %u", what, (unsigned long long)n, mesh, c->meshes[mesh].n_tris);
+    return RT_OK;
+}
+
+// The ordering after earlier work, then the mesh's refit map (at its first update)
+static int begin_mesh_update(rt_ctx* c, uint32_t mesh, const char* what)
+{
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the geometry this call rewrites
+    rt_ctx::MeshRefit& r = c->mesh_refit[mesh];
+    if (r.link) return RT_OK;
+    return build_refit_map(c, c->scene.nodes_ref + (size_t)c->meshes[mesh].first_node * 3, r.n_nodes, what, r.link, r.leaves, r.arrivals,
+                           r.n_leaves);
+}
+
+// The refit of the mesh's nodes (the records were written before), then its refit root box, read back (blocking), into the mesh's
+// box; if an instance of the current list uses the mesh, the top-level tree of that list is rebuilt from the new box and only the
+// header and the top-level records are rewritten: the instance records, the previous transforms and scene_mid stay.
+static int finish_mesh_update(rt_ctx* c, uint32_t mesh, const char* what)
+{
+    rtinst::MeshInfo& mi = c->meshes[mesh];
+    const rt_ctx::MeshRefit& r = c->mesh_refit[mesh];
+    const float4* nodes = c->scene.nodes_ref + (size_t)mi.first_node * 3;
+    {
+        int rc = launch_refit(c, r.leaves, r.n_leaves, r.link, r.arrivals, r.n_nodes, nodes, c->scene.tris_ref + (size_t)mi.first_tri * 3,
+                              c->scene.wnodes + mi.rec_f4);
+        if (rc) return rc;
+    }
+    float4 box[2];
+    RT_CUDA(c, cudaMemcpyAsync(box, nodes, sizeof(box), cudaMemcpyDeviceToHost, c->stream));
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    mi.lo[0] = box[0].x; mi.lo[1] = box[0].y; mi.lo[2] = box[0].z; mi.hi[0] = box[1].x; mi.hi[1] = box[1].y; mi.hi[2] = box[1].z;
+    bool used = false;
+    for (const RtInstance& in : c->inst_list) used = used || in.mesh == mesh;
+    if (!used) return RT_OK;
+    rtinst::Prepared pr;
+    std::string err;
+    if (!rtinst::prepare(c->inst_list.data(), (uint32_t)c->inst_list.size(), c->meshes, pr, err))
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: %s", what, err.c_str());     // not reached: the list passed rt_set_instances, the box is finite
+    const size_t f4 = top_level_image(pr, (uint32_t)c->inst_list.size(), c->inst_host.data());
+    RT_CUDA(c, cudaMemcpyAsync(c->inst_hdr, c->inst_host.data(), f4 * 16, cudaMemcpyHostToDevice, c->stream));
+    return RT_OK;
+}
+
+int rt_update_mesh_triangles(rt_ctx* c, uint32_t mesh, const RtTriangle* triangles, uint64_t n)
+{
+    const char* what = "rt_update_mesh_triangles";
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_update_mesh_triangles(k, mesh, triangles, n));
+    { int rc = check_mesh_update(c, mesh, triangles, n, what); if (rc) return rc; }
+    for (uint64_t i = 0; i < n; ++i)
+    {
+        const RtTriangle& t = triangles[i];
+        const float s[9] = { t.v1.position.x, t.v1.position.y, t.v1.position.z, t.v2.position.x, t.v2.position.y, t.v2.position.z,
+                             t.v3.position.x, t.v3.position.y, t.v3.position.z };
+        for (float v : s)
+            if (!std::isfinite(v)) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: triangle %llu has a position that is not finite", what, (unsigned long long)i);
+    }
+    { int rc = begin_mesh_update(c, mesh, what); if (rc) return rc; }
+    { int rc = stage_records(c, triangles, n, c->meshes[mesh].first_tri, what); if (rc) return rc; }
+    return finish_mesh_update(c, mesh, what);
+}
+
+int rt_update_mesh_triangles_device(rt_ctx* c, uint32_t mesh, const void* triangles, uint64_t n)
+{
+    const char* what = "rt_update_mesh_triangles_device";
+    RT_CHECK_CTX(c);
+    { int rc = check_device_triangles(c, triangles, what, "rt_update_mesh_triangles"); if (rc) return rc; }
+    { int rc = check_mesh_update(c, mesh, triangles, n, what); if (rc) return rc; }
+    { int rc = begin_mesh_update(c, mesh, what); if (rc) return rc; }
+    if (!c->mesh_bad)
+    {
+        DevAllocs g;
+        uint32_t* bad = nullptr;
+        RT_CUDA(c, g.alloc(bad, 1));
+        c->tree_mem.adopt(std::move(g)); c->mesh_bad = bad;
+    }
+    uint32_t bad = 0;
+    RT_CUDA(c, cudaMemsetAsync(c->mesh_bad, 0, 4, c->stream));
+    {
+        TimedLaunch t(c, RT_K_MISC);
+        k_check_positions<<<grid_for((uint32_t)n), 256, 0, c->stream>>>((const float4*)triangles, (uint32_t)n, c->mesh_bad);
+        int rc = post_launch(c, "k_check_positions"); if (rc) return rc;
+    }
+    RT_CUDA(c, cudaMemcpyAsync(&bad, c->mesh_bad, 4, cudaMemcpyDeviceToHost, c->stream));
+    RT_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (bad) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: a position is not finite", what);
+    { int rc = launch_refit_records(c, triangles, c->meshes[mesh].first_tri, (uint32_t)n); if (rc) return rc; }
+    return finish_mesh_update(c, mesh, what);
 }
 
 int rt_read_bvh(rt_ctx* c, RtLinearBVHNode* nodes, float* records, uint64_t* n_records)
@@ -2636,7 +2795,7 @@ int rt_set_option(rt_ctx* c, int key, uint32_t value)
             return RT_OK;
         }
         c->object_motion = 1;
-        return (c->scene_ready && !c->instanced) ? set_prev_positions(c) : RT_OK;   // instances keep their previous transforms always
+        return c->scene_ready ? set_prev_positions(c) : RT_OK;
     case RT_OPT_SAMPLER:
         if (value > 1) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "sampler type must be 0 (kRandom) or 1 (kBlueNoise)");
         if (value == 1 && !c->d_bn)

@@ -54,6 +54,20 @@ __global__ void __launch_bounds__(256) k_refit_records(const float4* __restrict_
     r[6] = make_float4(uv2.x, uv2.y, uv3.x, uv3.y);
 }
 
+// *bad = 1 if a position coordinate (xyz of v1, v2, v3) of src[0 .. n) (RtTriangle layout) is not finite; the caller clears it
+// (rt_update_mesh_triangles_device checks before it writes anything)
+__global__ void __launch_bounds__(256) k_check_positions(const float4* __restrict__ src, uint32_t n, uint32_t* bad)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4* t = src + (size_t)i * 10;
+    const float4 p1 = t[0], p2 = t[3], p3 = t[6];
+    const float s[9] = { p1.x, p1.y, p1.z, p2.x, p2.y, p2.z, p3.x, p3.y, p3.z };
+    bool ok = true;
+    for (int k = 0; k < 9; ++k) ok = ok && isfinite(s[k]);
+    if (!ok) *bad = 1u;
+}
+
 // Positions of the listed triangles from tris_ref (the emitter table's areas after an update): 3 float4 per entry.
 __global__ void __launch_bounds__(256) k_gather_positions(const float4* __restrict__ tris_ref, const uint32_t* __restrict__ idx, uint32_t n,
                                                           float4* out)

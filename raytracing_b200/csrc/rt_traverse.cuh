@@ -35,6 +35,7 @@ struct DevInstScene : DevScene
     const float4* irec;            // 8 float4 per instance: W rows, M rows, (mesh root ref, mesh record base in float4, first
                                    // triangle, base) as int bits, (det sign, first node bits, -, -)
     const uint32_t* ibase;         // base (first virtual triangle id) per instance, ascending
+    const float4* prev_tri;        // RT_OPT_OBJECT_MOTION: the previous positions of every mesh triangle (tris_ref layout); else nullptr
 };
 template <bool INST> using SceneOf = typename std::conditional<INST, DevInstScene, DevScene>::type;
 

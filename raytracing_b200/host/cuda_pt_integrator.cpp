@@ -175,6 +175,11 @@ void CUDAPathTraceIntegrator::SetInstances(const RtInstance* instances, std::uin
     Check(rt_set_instances(ctx_, instances, count), "SetInstances");
 }
 
+void CUDAPathTraceIntegrator::UpdateMeshTriangles(std::uint32_t mesh, const RtTriangle* triangles, size_t count)
+{
+    Check(rt_update_mesh_triangles(ctx_, mesh, triangles, count), "UpdateMeshTriangles");
+}
+
 std::uint64_t CUDAPathTraceIntegrator::RebuildBvh(BvhBuild build)
 {
     std::uint64_t n_nodes = 0;

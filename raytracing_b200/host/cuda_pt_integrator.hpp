@@ -113,6 +113,9 @@ public:
     void UploadInstancedScene(Scene const& shared, const RtTriangle* triangles, size_t n_triangles, const RtLinearBVHNode* nodes,
                               size_t n_nodes, const RtMeshDesc* meshes, std::uint32_t n_meshes);
     void SetInstances(const RtInstance* instances, std::uint32_t count);
+    // mesh update in an instanced scene (rt_update_mesh_triangles): new triangles for one mesh (its leaf order, same count); its
+    // tree is refit on the device and the top-level tree rebuilt.  No reset, as for UpdateTriangles.
+    void UpdateMeshTriangles(std::uint32_t mesh, const RtTriangle* triangles, size_t count);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

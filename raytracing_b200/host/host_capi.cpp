@@ -224,6 +224,11 @@ int rth_render_set_instances(void* h, const RtInstance* instances, std::uint32_t
     try { ((RenderHandle*)h)->render->SetInstances(instances, count); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_update_mesh_triangles(void* h, std::uint32_t mesh, const RtTriangle* triangles, size_t count)
+{
+    try { ((RenderHandle*)h)->render->UpdateMeshTriangles(mesh, triangles, count); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_rebuild_bvh(void* h, std::uint64_t* n_nodes)
 {
     try { *n_nodes = ((RenderHandle*)h)->render->RebuildBvh(); return 0; }

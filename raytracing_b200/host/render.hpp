@@ -70,6 +70,8 @@ public:
         Cuda().UploadInstancedScene(scene_, triangles, n_triangles, nodes, n_nodes, meshes, n_meshes);
     }
     void SetInstances(const RtInstance* instances, std::uint32_t count) { Cuda().SetInstances(instances, count); }
+    // mesh update in an instanced scene (CUDAPathTraceIntegrator::UpdateMeshTriangles); keeps the accumulation, as UpdateTriangles
+    void UpdateMeshTriangles(std::uint32_t mesh, const RtTriangle* triangles, size_t count) { Cuda().UpdateMeshTriangles(mesh, triangles, count); }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

@@ -53,6 +53,7 @@ def load_library():
     L.rth_render_rebuild_bvh.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rth_render_upload_instanced_scene.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32]
     L.rth_render_set_instances.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.rth_render_update_mesh_triangles.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
     L.rth_render_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
@@ -280,6 +281,13 @@ class HostRender:
         rec["object_to_world"] = np.ascontiguousarray(transforms, dtype="<f4").reshape(-1, 12)
         rec["mesh"] = ids
         if self.L.rth_render_set_instances(self.h, rec.ctypes.data if len(rec) else None, len(rec)) != 0:
+            raise _err(self.L)
+
+    def update_mesh_triangles(self, mesh, triangles):
+        """Render::UpdateMeshTriangles: mesh `mesh` of the instanced scene in its leaf order with new positions, normals and
+        texcoords; its tree is refit on the device.  Keeps the accumulation (request_reset() starts over)."""
+        t = np.ascontiguousarray(triangles, dtype=TRIANGLE_DT)
+        if self.L.rth_render_update_mesh_triangles(self.h, int(mesh), t.ctypes.data, t.shape[0]) != 0:
             raise _err(self.L)
 
     def rebuild_bvh(self, method="linear"):

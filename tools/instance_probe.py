@@ -10,6 +10,14 @@ scene holds (free memory before the context's upload minus after it, cudaMemGetI
 rt_set_instances with the 184 instances (host clock around 50 calls, each followed by rt_sync, warm buffer).  Prints one JSON line
 per arm, headed by the GPU's name and power limit read in the same run.  Frames of the two arms are not equal: the instanced matrices
 round differently from the flattened vertices (tests/test_instancing_cpu.py bounds the difference).
+
+  python tools/instance_probe.py --mesh-update [--width ... --frames ... --warmup ... --calls 20] [--out FILE]
+
+Mesh updates in the instanced field (rt_update_mesh_triangles*) instead: the time of one update of the ShaderBalls mesh (54 790
+triangles, under 183 instances) by the host variant (a TRIANGLE_DT array) and by the device variant (a CUDA uint8 tensor), host
+clock around --calls calls, each returning after its blocking root-box read-back and followed by rt_sync; the time of a 32-byte
+device-to-host copy with its synchronise, the read-back's floor; and ms per frame after a deforming update (refit tree) against a
+fresh context that uploaded the same triangles and refit nodes (tests/refit_model.py) with the same instance list.
 """
 import argparse
 import json
@@ -54,11 +62,17 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--copies", type=int, default=183)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--mesh-update", action="store_true")
+    ap.add_argument("--calls", type=int, default=20)
     args = ap.parse_args()
     import torch
     torch.cuda.init()
     base = scene_io.load_scene("ShaderBalls")
     lines = [{"gpu": gpu_info()}]
+    if args.mesh_update:
+        lines += mesh_update(args, base)
+        emit(lines, args.out)
+        return
 
     def free():
         torch.cuda.synchronize()
@@ -94,11 +108,68 @@ def main():
     c.destroy()
     lines.append({"arm": "flattened", "triangles": len(flat["triangles"]), "ms_per_frame": ms, "scene_device_bytes": int(mem),
                   "frame": f"{args.width}x{args.height}x{args.bounces}"})
+    emit(lines, args.out)
+
+
+def emit(lines, out):
     text = "\n".join(json.dumps(x) for x in lines)
     print(text)
-    if args.out:
-        with open(args.out, "w") as f:
+    if out:
+        with open(out, "w") as f:
             f.write(text + "\n")
+
+
+def mesh_update(args, base):
+    import torch
+    from tests.refit_model import deform, refit
+    fld = synthetic.instanced_field(base, copies=args.copies, width=args.width, height=args.height)
+    meshes, ids, mats, cam = fld["meshes"], fld["mesh_ids"], fld["transforms"], fld["camera_pose"]
+    t0 = meshes[0]["triangles"]
+    shapes = [deform(t0, "noise", seed=s, amount=0.02) for s in range(2)]
+    c = capi.Context(args.width, args.height)
+    c.set_camera(cam)
+    c.upload_instanced_scene(meshes, fld["shared"])
+    c.set_instances(ids, mats)
+    out = []
+    for variant in ("host", "device"):
+        src = shapes if variant == "host" else [torch.from_numpy(x.view(np.uint8).reshape(len(x), 160).copy()).cuda() for x in shapes]
+        for k in range(3):
+            c.update_mesh_triangles(0, src[k % 2])
+        c.sync()
+        t = time.perf_counter()
+        for k in range(args.calls):
+            c.update_mesh_triangles(0, src[k % 2]); c.sync()
+        out.append({"update": variant, "mesh_triangles": len(t0), "instances": len(ids),
+                    "ms_per_update": (time.perf_counter() - t) * 1e3 / args.calls})
+    x = torch.zeros(8, device="cuda")
+    y = torch.empty(8, pin_memory=False)
+    for _ in range(10):
+        y.copy_(x); torch.cuda.synchronize()
+    t = time.perf_counter()
+    for _ in range(200):
+        y.copy_(x); torch.cuda.synchronize()
+    out.append({"readback_32B_ms": (time.perf_counter() - t) * 1e3 / 200})
+    c.update_mesh_triangles(0, shapes[1])
+    upd = timed_frames(c, args.bounces, args.frames, args.warmup)
+    c.destroy()
+    cur = list(meshes)
+    cur[0] = {"triangles": shapes[1], "nodes": refit(meshes[0]["nodes"], shapes[1])}
+    f = capi.Context(args.width, args.height)
+    f.set_camera(cam)
+    f.upload_instanced_scene(cur, fld["shared"])
+    f.set_instances(ids, mats)
+    fresh = timed_frames(f, args.bounces, args.frames, args.warmup)
+    f.destroy()
+    c = capi.Context(args.width, args.height)                # the updated arm again, after the fresh one: alternation shows drift
+    c.set_camera(cam)
+    c.upload_instanced_scene(meshes, fld["shared"])
+    c.set_instances(ids, mats)
+    c.update_mesh_triangles(0, shapes[1])
+    upd2 = timed_frames(c, args.bounces, args.frames, args.warmup)
+    c.destroy()
+    out.append({"frame": f"{args.width}x{args.height}x{args.bounces}", "ms_per_frame_after_update": [upd, upd2],
+                "ms_per_frame_fresh_upload": fresh})
+    return out
 
 
 if __name__ == "__main__":
