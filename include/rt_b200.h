@@ -83,14 +83,12 @@ typedef enum RtOption {
                                    option, the scene or the partition changes; the camera and sample index are a node-parameter update) */
     RT_OPT_PDL = 25,            /* 1 (default): the traversal and shading kernels of a frame are chained by programmatic dependent launch
                                    (a kernel's CTAs start and stage the BVH while the previous kernel drains) */
-    RT_OPT_FRAME_KERNEL = 26,   /* how rt_integrate runs a frame.  1: ONE persistent kernel in which every CTA is an independent
-                                   wavefront over its own pixels (queue cursors in shared memory, no global atomics, no launch
-                                   boundaries); 0: one kernel per phase (graph replay / PDL chain as configured above);
-                                   2 (default): the one-kernel frame for partitions of up to 7168 pixels per SM (0.95 M pixels,
-                                   under half a 1080p frame, on an H100's 132 SMs), per-phase kernels for larger ones.  Results are bit-identical.
-                                   rt_integrate_samples: 1 also selects the regenerating frame kernel (one launch per call), which is
-                                   bit-identical but measured slower than n one-kernel frames on scenes traversed through L1 (up to
-                                   29 % on ShaderBalls, DESIGN.md section 4); 0 and 2 run n frames of rt_integrate's schedule */
+    RT_OPT_FRAME_KERNEL = 26,   /* how rt_integrate, and every frame of rt_integrate_samples, runs a frame.  1: ONE persistent kernel
+                                   in which every CTA is an independent wavefront over its own pixels (queue cursors in shared
+                                   memory, no global atomics, no launch boundaries); 0: one kernel per phase (graph replay / PDL
+                                   chain as configured above); 2 (default): the one-kernel frame for partitions of up to 7168
+                                   pixels per SM (0.95 M pixels, under half a 1080p frame, on an H100's 132 SMs), per-phase
+                                   kernels for larger ones.  Results are bit-identical */
     RT_OPT_PRESENT = 27,        /* multi-device contexts, rt_resolve: 0 (default) parallel read-back of every device's rows,
                                    1 gather to devices[0] over NVLink, resolve and read back there */
     RT_OPT_FRAME_THREADS = 28,  /* threads per CTA of the one-kernel frame: 0 (default) by partition size, else a multiple of 32 <= 1024 */
@@ -113,7 +111,6 @@ typedef enum RtOption {
 } RtOption;
 
 #define RT_MAX_BOUNCES 255u     /* bounce index range supported per frame (reference GUI: 0..5) */
-#define RT_MAX_REGEN_SAMPLES (1u << 24)   /* n_samples limit of rt_integrate_samples on the regenerating kernel (RT_OPT_FRAME_KERNEL 1) */
 
 /* Per-bounce device counters of the last rt_integrate / rt_integrate_samples call (index = bounce, 0..max_bounces); a
  * multi-sample call returns the element-wise sums over its samples. */
@@ -253,11 +250,7 @@ int rt_integrate(rt_ctx* ctx, uint32_t max_bounces);
  * sample's values), the resolved image of every view and, once the call completes, the fused-gather slab.  rt_read_frame_stats
  * returns the per-bounce counters summed over the call's samples.  With a gather target set, the completion flag is signalled
  * once per call.
- * With RT_OPT_FRAME_KERNEL = 1 (and neither RT_OPT_KERNEL_TIMING nor RT_OPT_COUNT_TRAVERSAL) the call is ONE launch of the
- * regenerating frame kernel: when a pixel's path ends, its CTA starts that pixel's next sample in the next traversal round.  It
- * carries a path's sample offset in 24 bits: n_samples > RT_MAX_REGEN_SAMPLES is RT_ERR_INVALID_ARGUMENT there.
- * Otherwise, the default included, the frame rt_integrate would run is run n_samples times (measured on H100, the regenerating
- * kernel is not faster at any partition size; DESIGN.md section 4); the fused gather is pushed by the last frame only.
+ * The frame rt_integrate would run is run n_samples times; the fused gather is pushed by the last frame only.
  * n_samples == 1 is rt_integrate.  The stepwise taps (rt_read_rays, rt_read_hits) find no rays of a multi-sample call that ran
  * the one-kernel frame, and the last frame's rays after one that ran the per-phase frames.
  * Errors, checked before anything is enqueued: RT_ERR_INVALID_ARGUMENT for n_samples == 0, a sample count that would wrap
@@ -283,9 +276,8 @@ int rt_integrate_samples(rt_ctx* ctx, uint32_t max_bounces, uint32_t n_samples);
  * rt_set_partition, which clears the radiance but not the context's sample count (the sample index continues; call rt_reset to
  * start over, after which every active pixel's count equals the sample count again).  The per-pixel state (about 20 bytes per pixel) exists only while it is on.
  * With it on: rt_resolve / rt_resolve_async divide the shaded colour by each pixel's own sample count (the AOV views are
- * unchanged); n_ext[0] of rt_read_frame_stats counts the pixels active at the start of the frame; rt_integrate_samples always
- * runs n frames of rt_integrate's schedule (never the regenerating kernel).  Multi-device contexts fan out: every device decides
- * for its own rows, with the same result as one device.
+ * unchanged); n_ext[0] of rt_read_frame_stats counts the pixels active at the start of the frame.  Multi-device contexts fan out:
+ * every device decides for its own rows, with the same result as one device.
  * RT_ERR_UNSUPPORTED, whichever of the two calls comes second: the temporal denoiser, a fused-gather target
  * (rt_set_gather_target), RT_OPT_PRESENT 1 on a multi-device context, and rt_resolve_gathered[_async]. */
 int rt_set_adaptive_sampling(rt_ctx* ctx, float max_error, uint32_t min_samples);
@@ -350,8 +342,7 @@ int rt_set_spatial_denoiser(rt_ctx* ctx, uint32_t iterations, float sigma_color,
  * a caller whose last step bounce is below it gets emitter light from its last vertex, which BSDF sampling never adds (its
  * continuation is not traced): its image converges to a brighter value than with the option off.  Call rt_integrate (or
  * rt_integrate_samples) with the same max_bounces once before driving the steps.
- * Device memory: 4 B per triangle and 8 B per emitter while it is on.  rt_integrate_samples runs n frames of
- * rt_integrate's schedule with it on (the regenerating kernel keeps its path state where the carried p_b goes). */
+ * Device memory: 4 B per triangle and 8 B per emitter while it is on. */
 
 /* ---- environment sampling (new capability): rt_set_option(ctx, RT_OPT_ENV_SAMPLING, 1) --------------------------------------
  * Next-event estimation on the environment map, combined with BSDF sampling by MIS (power heuristic, as for emitters); same

@@ -125,7 +125,7 @@ __device__ __forceinline__ uint32_t warp_grab(uint32_t* cursor)
     return __shfl_sync(0xffffffffu, at, 0);
 }
 
-// Shadow-ray records.  sA = (origin.xyz, word), sC = (light sample.xyz, path state or 0), and sB = (dir.xyz, t_max) only where the
+// Shadow-ray records.  sA = (origin.xyz, word), sC = (light sample.xyz, 0), and sB = (dir.xyz, t_max) only where the
 // light does not fix them: for a directional light they are its record light_rec[2 * l] (light_sample), which the shadow pass
 // reads in place of sB.  The word is the local pixel index (low 24 bits) and the light byte l (high 8 bits); RT_SHADOW_3PLANE
 // marks every other ray (point lights, emitter and environment samples, lights from index 255 on), whose sB is stored.  Partitions
@@ -138,11 +138,11 @@ __device__ __forceinline__ uint32_t shadow_word(const FrameParams& p, uint32_t l
 }
 // Writes the shadow ray of local pixel li in slot si; sB only for a three-plane record
 __device__ __forceinline__ void put_shadow(const FrameParams& p, const Queues& q, uint32_t si, uint32_t li, uint32_t light, f3 o, f3 d, float t_max,
-                                           f3 sample, uint32_t c_w)
+                                           f3 sample)
 {
     q.sA[si] = make_float4(o.x, o.y, o.z, __uint_as_float(shadow_word(p, li, light)));
     if (!shadow_two_plane(p) || light == RT_SHADOW_3PLANE) q.sB[si] = make_float4(d.x, d.y, d.z, t_max);
-    q.sC[si] = make_float4(sample.x, sample.y, sample.z, __uint_as_float(c_w));
+    q.sC[si] = make_float4(sample.x, sample.y, sample.z, 0.0f);
 }
 // The (dir.xyz, t_max) plane of the shadow ray in slot si whose sA word is w, and its local pixel li
 __device__ __forceinline__ float4 shadow_dir(const FrameParams& p, const DevScene& sc, const Queues& q, uint32_t si, uint32_t w, uint32_t& li)

@@ -12,7 +12,7 @@
  *                                C = (path throughput.xyz, -)
  *   shadow-ray queue:            A = (origin.xyz, local pixel index | light byte << 24)
  *                                B = (dir.xyz, t_max = distance to light), not stored for a directional light
- *                                C = (light sample.xyz, 0 or path state)          (rt_kernel_types.cuh, put_shadow)
+ *                                C = (light sample.xyz, 0)                        (rt_kernel_types.cuh, put_shadow)
  *   hit queue:                   (bc.x, bc.y, primitive_id bits, ray slot bits)   — rays that hit, compacted
  *   miss queue:                  ray slot (uint32)                                — rays that missed, compacted
  *   hits (stepwise path only):   (bc.x, bc.y, primitive_id bits, t)
@@ -124,7 +124,7 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
     if (p.gather) p.gather[li] = r;        // the path ends here: its pixel is final (its last shadow ray was accumulated a phase ago)
 }
 
-// kernels/cl/hit_surface.cl:30-186, for the path of sample p.dyn->sample_idx + sample_offset (a later sample of a multi-sample call).
+// kernels/cl/hit_surface.cl:30-186, for the path of sample p.dyn->sample_idx.
 // prev_pdf: C.w of the ray (sampled lights: p_b of its direction at the previous vertex, 0 for primary rays and after a delta lobe).
 // EMIT: the scene has an active emitter table (sc.emit_*, RT_OPT_EMITTER_SAMPLING) or environment table (sc.env_*,
 // RT_OPT_ENV_SAMPLING), each read only while it exists; a template flag, so that the kernels without it are the code of both options off.
@@ -134,7 +134,7 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
 template <bool EMIT = false, bool INST = false>
 __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
                                           f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
-                                          uint32_t sample_offset, ShadeOut& out)
+                                          ShadeOut& out)
 {
 #if RT_SHADE_PROBE == 1
     {   // memory floor: the shading record, material and blue-noise reads of the hit, each value used by a few adds, and a shadow
@@ -146,7 +146,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         float s = 0.0f;
         if (p.bn)
             for (uint32_t d = 0; d < 5; ++d)
-                s += sample_blue_noise(p.bn, pxy & 0xFFFFu, pxy >> 16, p.dyn->sample_idx + sample_offset, bounce * 5u + d);
+                s += sample_blue_noise(p.bn, pxy & 0xFFFFu, pxy >> 16, p.dyn->sample_idx, bounce * 5u + d);
         const float w0 = 1.0f - u - v;
         const f3 position = mk3(q0) * w0 + mk3(q1) * u + mk3(q2) * v;
         out.emissive = false;
@@ -252,7 +252,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
             }
         }
     }
-    uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx + sample_offset);
+    uint32_t pixel_seed = sample_seed_pixel(px, py, p.dyn->sample_idx);
     out.spawn_shadow = false;
     out.s_light = RT_SHADOW_3PLANE;
     bool pick_emitter = false, pick_env = false;
@@ -325,7 +325,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
     }
     else
     {   // direct lighting (next-event estimation on analytic lights)
-        float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx + sample_offset, bounce * 5u + SAMPLE_LIGHT)
+        float s_light = p.bn ? sample_blue_noise(p.bn, px, py, p.dyn->sample_idx, bounce * 5u + SAMPLE_LIGHT)
                              : sample_random(pixel_seed, bounce, SAMPLE_LIGHT);
         f3 outgoing; float pdf, distance_to_light;
         int directional;
@@ -353,7 +353,7 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
         f2 s; float s1;
         if (p.bn)
         {
-            const uint32_t sample_idx = p.dyn->sample_idx + sample_offset;
+            const uint32_t sample_idx = p.dyn->sample_idx;
             s.x = sample_blue_noise(p.bn, px, py, sample_idx, bounce * 5u + SAMPLE_U);
             s.y = sample_blue_noise(p.bn, px, py, sample_idx, bounce * 5u + SAMPLE_V);
             s1 = sample_blue_noise(p.bn, px, py, sample_idx, bounce * 5u + SAMPLE_LAYER);
@@ -408,13 +408,11 @@ __device__ __forceinline__ void make_primary_ray(const FrameParams& p, const Aov
     }
 }
 
-// make_primary_ray, stored in slot `slot` of ray queue `in` with throughput 1 and `state` in C.w (the path state of the
-// regenerating frame kernel; 0 everywhere else)
-__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, int in, uint32_t slot, uint32_t li,
-                                            uint32_t sample_idx, uint32_t state, float4& a, float4& b)
+// make_primary_ray of sample p.dyn->sample_idx, stored in slot `slot` of ray queue 0 with throughput 1 and C.w = 0
+__device__ __forceinline__ void primary_ray(const FrameParams& p, const Queues& q, const AovParams& aov, uint32_t slot, uint32_t li, float4& a, float4& b)
 {
-    make_primary_ray(p, aov, li, sample_idx, a, b);
-    q.A[in][slot] = a; q.B[in][slot] = b; q.C[in][slot] = make_float4(1.0f, 1.0f, 1.0f, __uint_as_float(state));
+    make_primary_ray(p, aov, li, p.dyn->sample_idx, a, b);
+    q.A[0][slot] = a; q.B[0][slot] = b; q.C[0][slot] = make_float4(1.0f, 1.0f, 1.0f, 0.0f);
 }
 
 // Closest hit of the ray (a, b) of entry i (live lanes) and hit/miss stream compaction: __ballot + __popc give every lane its
@@ -506,7 +504,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
         const float4 c = bounce == 0 && !ALL_PLANES ? make_float4(1.0f, 1.0f, 1.0f, 0.0f) : q.C[in][base + i];
         const float4 a = origin ? q.A[in][base + i] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         pixel = __float_as_uint(b.w);
-        shade_hit<EMIT, INST>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, 0u, so);
+        shade_hit<EMIT, INST>(sc, p, aov, bounce, pixel, mk3(a), mk3(b), mk3(c), c.w, __float_as_uint(h.z), h.x, h.y, so);
         li = local_index(p, pixel);
         if (so.emissive) add_radiance(radiance, li, so.emission_add);
     }
@@ -529,7 +527,7 @@ __device__ __forceinline__ bool shade_hit_group(const FrameParams& p, const Scen
     if (ss)
     {
         const uint32_t si = base + (uint32_t)slot + __popc(smask & lt_mask);
-        put_shadow(p, q, si, li, so.s_light, so.s_origin, so.s_dir, so.s_tmax, so.s_sample, 0u);
+        put_shadow(p, q, si, li, so.s_light, so.s_origin, so.s_dir, so.s_tmax, so.s_sample);
     }
     if (STAGE)
     {
@@ -575,7 +573,7 @@ __global__ void __launch_bounds__(256) k_raygen(FrameParams p, Queues q, DevCoun
     if (i == 0) ctr->n_primary = n;
     if (i >= n) return;
     float4 a, b;
-    primary_ray(p, q, aov, 0, i, p.active ? p.active[i] : i, p.dyn->sample_idx, 0u, a, b);
+    primary_ray(p, q, aov, i, p.active ? p.active[i] : i, a, b);
 }
 
 // IntersectRays (stepwise): closest hit of every live ray of bounce b -> hits[]
@@ -1630,7 +1628,7 @@ cudaError_t launch_chain(rt_ctx* c, void (*kernel)(KArgs...), int grid, size_t s
 //           default 0 = off, DESIGN.md section 4 says why) — when the structure does not fit;
 //   mode 0  nothing staged: literal traversal (RT_OPT_TRAVERSAL 0), RT_OPT_SMEM_BVH off.
 struct Stage { int mode; size_t bytes; uint32_t top_k; };
-// octant = false: the one-kernel frame (k_frame, k_frame_regen) stays on mode 1 — at its 64 registers the second traversal loop
+// octant = false: the one-kernel frame (k_frame) stays on mode 1 — at its 64 registers the second traversal loop
 // that mode 3 needs for the guarded rays spills inside the frame loop (measured: CornellBox on rank 0 of 4, 0.761 -> 0.811 ms).
 Stage bvh_stage(const rt_ctx* c, bool octant = true)
 {
@@ -1668,7 +1666,7 @@ auto with_scene(const rt_ctx* c, F&& f)
 //   PER_PHASE  k_trace_closest, k_trace_primary, k_shadow_accumulate: staging modes 0-3 and RT_SMEM_INST, COUNT on 0 and INST;
 //   MERGED     k_trace_both: modes 0-3 and RT_SMEM_INST, no COUNT (merged_trace_available);
 //   STEPWISE   k_intersect, k_intersect_shadow: 0 and RT_SMEM_INST, COUNT on both;
-//   FRAME      k_frame, k_frame_regen: modes 0-2 (bvh_stage without the octant tables) on flat scenes, no COUNT.
+//   FRAME      k_frame: modes 0-2 (bvh_stage without the octant tables) on flat scenes, no COUNT.
 enum Family { PER_PHASE, MERGED, STEPWISE, FRAME };
 
 // Launches a traversal kernel of family F: calls launch(COUNT, SMEM, scene, dynamic shared-memory bytes) once with this launch's
@@ -3305,8 +3303,8 @@ static int gather_signal(rt_ctx* c, bool copy_slab)
     return post_launch(c, "k_gather_signal");
 }
 
-// Launch shape of the one-kernel frames (k_frame, k_frame_regen): the CTAs that are resident at once, at most one per group of 32
-// pixels, and the slots of each CTA's region of every queue.
+// Launch shape of the one-kernel frame (k_frame): the CTAs that are resident at once, at most one per group of 32 pixels, and the
+// slots of each CTA's region of every queue.
 static int frame_kernel_grid(rt_ctx* c, const void* k, int threads, size_t sm, uint32_t& grid, uint32_t& slots_per_cta)
 {
     const int per_sm = std::min(resident_per_sm(c, k, threads, sm), 32);
@@ -3353,30 +3351,6 @@ static int integrate_frame_kernel(rt_ctx* c, uint32_t max_bounces, bool accumula
     return RT_OK;
 }
 
-// n_samples (<= RT_MAX_REGEN_SAMPLES) frames as ONE launch of the regenerating frame kernel (k_frame_regen), with k_frame's CTA
-// shape and queue regions.  The statistics go to counters_sum; it pushes the fused gather's pixels itself.
-static int integrate_regen_kernel(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
-{
-    const int threads = frame_kernel_threads(c);
-    const FrameDyn dyn = frame_dyn(c);
-    FrameParams fp = frame_params(c);
-    fp.gather = c->gather_slab;
-    int rc = launch_traversal<FRAME>(c, [&](auto, auto smem, const DevScene& sc, size_t sm) -> int {
-        auto* k = k_frame_regen<smem.value>;
-        uint32_t grid, slots_per_cta;
-        int rc2 = frame_kernel_grid(c, (const void*)k, threads, sm, grid, slots_per_cta); if (rc2) return rc2;
-        TimedLaunch t(c, RT_K_MISC);
-        k<<<grid, threads, sm, c->stream>>>(fp, sc, c->traversal, c->q, c->counters_sum, c->radiance, aov_params(c), max_bounces, n_samples,
-                                            slots_per_cta, dyn);
-        return RT_OK;
-    });
-    if (rc || (rc = post_launch(c, "k_frame_regen"))) return rc;
-    note_frame_aovs(c);
-    c->frame_started = true; c->cur_bounce = max_bounces;
-    c->sample_count += n_samples;
-    return RT_OK;
-}
-
 // One frame on the schedule rt_integrate selects, without the fused gather's completion signal.  *pushed: the frame kernel has
 // pushed every pixel to the gather target already (otherwise the radiance slab has to be copied).
 static int integrate_frame(rt_ctx* c, uint32_t max_bounces, bool* pushed)
@@ -3416,12 +3390,6 @@ int rt_integrate(rt_ctx* c, uint32_t max_bounces)
     return gather_signal(c, !pushed);
 }
 
-// Which schedule rt_integrate_samples runs: the regenerating kernel only where RT_OPT_FRAME_KERNEL = 1 forces the one-kernel frame.
-// Measured on one H100 80GB HBM3 at 700 W (tools/spp_probe.py, 1080p x 8, rank 0 of 1/2/4/8-way partitions, N = 8 and 64, DESIGN.md
-// section 4) it never clearly beats N one-kernel frames: it ties on CornellBox (-3 % to +4 %) and is 5-29 % slower on ShaderBalls,
-// so every partition size takes the N-frame path.  Adaptive sampling decides between samples, so it always takes the N-frame path.
-static bool regen_selected(const rt_ctx* c) { return c->frame_kernel == 1 && one_kernel_frame(c) && !adaptive_on(c) && !c->emitter_sampling && !c->env_sampling; }
-
 // A multi-sample call leaves its summed statistics in counters_sum, which only rt_read_frame_stats reads: the counters that the
 // taps (rt_read_rays, rt_read_hits) take their entry counts from never exceed one frame's rays.
 int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
@@ -3433,9 +3401,6 @@ int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
         RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_integrate_samples: the sample count %u + %u would wrap", c->sample_count, n_samples);
     if (n_samples > 1 && c->denoiser)
         RT_FAIL(c, RT_ERR_UNSUPPORTED, "rt_integrate_samples: the temporal denoiser runs once per sample; render one sample per call with it");
-    if (n_samples > RT_MAX_REGEN_SAMPLES && regen_selected(c))
-        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "rt_integrate_samples: the regenerating frame kernel (RT_OPT_FRAME_KERNEL 1) renders at most %u samples per call",
-                RT_MAX_REGEN_SAMPLES);
     if (n_samples == 1) return rt_integrate(c, max_bounces);
     c->emit_max_bounces = max_bounces;
     int rc = require_ready(c); if (rc) return rc;
@@ -3445,12 +3410,7 @@ int rt_integrate_samples(rt_ctx* c, uint32_t max_bounces, uint32_t n_samples)
     RT_CUDA(c, cudaMemsetAsync(c->counters_sum, 0, sizeof(DevCounters), c->stream));
     c->stats_summed = false;
     bool pushed = true;
-    if (regen_selected(c))
-    {   // the taps find no rays of this call
-        RT_CUDA(c, cudaMemsetAsync(c->counters, 0, sizeof(DevCounters), c->stream));
-        if ((rc = integrate_regen_kernel(c, max_bounces, n_samples))) return rc;
-    }
-    else if (one_kernel_frame(c))
+    if (one_kernel_frame(c))
     {   // n k_frame launches that add up their statistics in c->counters, folded into counters_sum once per batch (a batch stays
         // small enough that no 32-bit half of the packed 64-bit counters can carry into the other); only the last frame pushes
         // to the gather target

@@ -20,8 +20,8 @@
  *                     the stepwise schedule, bit for bit.
  *   kStepwise         one kernel per virtual, like the OpenCL backend.
  * SetSamplesPerFrame(n): Integrate() renders n progressive samples, the same bits as n calls with one sample each.  kFrame only:
- * AdvanceSampleCount() submits them with ONE rt_integrate_samples call (n frames on the device without a host round trip, or
- * one launch of the regenerating frame kernel with RT_OPT_FRAME_KERNEL 1).  With n > 1 the kFused / kStepwise schedules, a call order other than
+ * AdvanceSampleCount() submits them with ONE rt_integrate_samples call (n frames on the device without a host round trip).
+ * With n > 1 the kFused / kStepwise schedules, a call order other than
  * Integrate()'s and the denoiser (it runs once per sample) throw std::runtime_error.
  * SetAdaptiveSampling(max_error, min_samples): pixels stop tracing once they have settled (include/rt_b200.h); ActivePixels() tells
  * a progressive loop when every pixel has.

@@ -146,7 +146,7 @@ def test_every_pixel_matches_the_oracle_at_its_count(name, w, h, mb, n, sampler)
 @pytest.mark.parametrize("fk", [0, 1, 2], ids=["phase", "frame_kernel_forced", "default"])
 def test_integrate_samples_equals_frames(fk):
     """rt_integrate_samples(N) with the feature on equals N x rt_integrate: the per-phase frames, k_frame (the default at this size)
-    and RT_OPT_FRAME_KERNEL 1, which must not take the regenerating kernel.  Radiance, counts and summed statistics, over two calls."""
+    and RT_OPT_FRAME_KERNEL 1.  Radiance, counts and summed statistics, over two calls."""
     name, w, h, mb = "CornellBox", 128, 128, 3
     sc, cam = scene(name), default_camera(w, h)
     opts = ((capi.OPT_FRAME_KERNEL, fk),)

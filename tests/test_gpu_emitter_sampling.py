@@ -62,8 +62,8 @@ def test_schedules_match_model(name, schedule, sampler):
 
 
 @pytest.mark.parametrize("name", ["CornellBox", "ShaderBalls"])
-def test_multi_sample_regen_setting_and_partitions_match_model(name):
-    """rt_integrate_samples with RT_OPT_FRAME_KERNEL 1 (runs N frames with the option on), a 3-way partition, and a multi-device
+def test_multi_sample_frame_kernel_setting_and_partitions_match_model(name):
+    """rt_integrate_samples with RT_OPT_FRAME_KERNEL 1 (N one-kernel frames with the option on), a 3-way partition, and a multi-device
     context that lists device 0 three times."""
     sc = scene(name)
     w, h, mb, n = 80, 48, 3, 3

@@ -94,8 +94,8 @@ def test_sun_sky_matches_model(schedule):
     c.destroy()
 
 
-def test_multi_sample_regen_setting_and_partitions_match_model():
-    """rt_integrate_samples with RT_OPT_FRAME_KERNEL 1 (runs N frames with the option on), a 3-way partition, and a multi-device
+def test_multi_sample_frame_kernel_setting_and_partitions_match_model():
+    """rt_integrate_samples with RT_OPT_FRAME_KERNEL 1 (N one-kernel frames with the option on), a 3-way partition, and a multi-device
     context that lists device 0 three times."""
     sc = scene("ShaderBalls")
     w, h, mb, n = 80, 48, 3, 3

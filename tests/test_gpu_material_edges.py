@@ -3,7 +3,7 @@ GPU tests (-m gpu) of the shading pass across the packed material space (tests/m
 value of every byte field, channel edges, a cross grid, black and white corners) at the default and a grazing pose, its per-hit
 twin, the normal panel, the light placements and the mirror case.
 
-- Every rt_integrate schedule, the stepwise steps, rt_integrate_samples (per-phase and regenerating) and rank 2 of a 3-way
+- Every rt_integrate schedule, the stepwise steps, rt_integrate_samples (per-phase and one-kernel frames) and rank 2 of a 3-way
   partition, 2 progressive samples of 6 bounces with kRandom and with blue noise, bit for bit against the oracle: radiance,
   per-bounce counters, the AOVs and the stepwise arm's primary hits.
 - The untextured chart (mat_rec) and its per-hit twin (unpack_material) give byte-identical radiance, counters and AOVs.
@@ -82,7 +82,7 @@ def test_every_schedule_matches_oracle(case, sampler):
             rows = np.arange(2, h, 3)
             rad = np.zeros((h, w, 4), "<f4"); part.read_radiance(rad)
             assert np.array_equal(bits(rad[rows][..., :3]), bits(pacc[rows][..., :3])), (case, sampler, "rank 2 of 3", s)
-        for fk in (0, 1):                 # rt_integrate_samples: the per-phase frames, the regenerating one-kernel frame
+        for fk in (0, 1):                 # rt_integrate_samples: the per-phase frames, the one-kernel frames
             c = samples_ctx(sc, cam, w, h, ((capi.OPT_FRAME_KERNEL, fk),), tables=tables)
             try:
                 c.integrate_samples(MB, SAMPLES)

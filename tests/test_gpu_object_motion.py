@@ -99,8 +99,8 @@ def test_every_run_matches_model(run):
     run_sequence(schedule, options)
 
 
-def test_regenerating_frame_kernel_matches_model():
-    """rt_integrate_samples with RT_OPT_FRAME_KERNEL 1 (the regenerating kernel): the AOVs are those of the call's last sample."""
+def test_forced_frame_kernel_samples_match_model():
+    """rt_integrate_samples with RT_OPT_FRAME_KERNEL 1 (N one-kernel frames): the AOVs are those of the call's last sample."""
     run_sequence("frame", (), samples=3)
 
 

@@ -10,7 +10,7 @@ GPU tests (-m gpu) of the packed queue words at their limits, each on every sche
   could carry into the high one.
 
 "Every schedule" is the per-phase graph and direct launches, the one-kernel frame, the unmerged per-phase kernels under kernel
-timing, the stepwise calls and the regenerating frame (rt_integrate_samples with RT_OPT_FRAME_KERNEL 1).  A context of 2^24 local
+timing, the stepwise calls and the N-frame one-kernel loop (rt_integrate_samples with RT_OPT_FRAME_KERNEL 1).  A context of 2^24 local
 pixels takes about 4 GB of device memory (3.98 GB at 4096 x 4096 after a frame, measured on an H100 80GB HBM3); one such context
 exists at a time.  The file runs in about a minute there.
 """
@@ -27,11 +27,11 @@ from tests.test_packed_limits_cpu import LIGHT_COUNTS, edge_origin_scene, light_
 pytestmark = pytest.mark.gpu
 
 STAT_KEYS = ("n_ext", "n_miss", "n_shadow", "n_cont", "n_unoccluded", "n_emissive_hits")
-RUNS = ("frame", "phase_graph", "phase_direct", "timed", "stepwise", "regen")      # "regen": integrate_samples(mb, n), forced k_frame
+RUNS = ("frame", "phase_graph", "phase_direct", "timed", "stepwise", "samples_fk1")      # "samples_fk1": integrate_samples(mb, n), forced k_frame
 
 
 def make(run, sc, cam, w, h, options=(), rank=0, world=1, tables=None):
-    c = schedule_ctx("frame" if run == "regen" else run, sc, cam, w, h, options, rank, world)
+    c = schedule_ctx("frame" if run == "samples_fk1" else run, sc, cam, w, h, options, rank, world)
     if tables is not None:
         c.upload_sampler_tables(*tables); c.set_option(capi.OPT_SAMPLER, 1)
     c.reset()
@@ -39,8 +39,8 @@ def make(run, sc, cam, w, h, options=(), rank=0, world=1, tables=None):
 
 
 def render(c, run, mb, samples):
-    """`samples` frames of `run` on c; -> the per-bounce statistics of each frame (one summed entry for "regen")."""
-    if run == "regen":
+    """`samples` frames of `run` on c; -> the per-bounce statistics of each frame (one summed entry for "samples_fk1")."""
+    if run == "samples_fk1":
         c.integrate_samples(mb, samples)
         return [c.frame_stats()]
     out = []
@@ -55,8 +55,8 @@ def summed(stats):
 
 
 def check_run_stats(run, got, want, mb, where):
-    """got: render()'s statistics; want: the reference's per-frame statistics (the regenerating frame sums them)."""
-    if run == "regen":
+    """got: render()'s statistics; want: the reference's per-frame statistics ("samples_fk1" sums them)."""
+    if run == "samples_fk1":
         got, want = [summed(got)], [summed(want)]
     check_stats(got[-1], want[-1], mb, where)
 

@@ -1,10 +1,10 @@
 """
 GPU tests (-m gpu) of rt_integrate_samples: n_samples frames in one call.  Every check is bit-exact against n calls of
 rt_integrate on a fresh context with the same options: the radiance bits, the sample count and the per-bounce statistics summed
-over the frames, plus (where stated) the AOV buffers, the resolved views and the fused-gather slab.  Where the one-kernel frame
-is forced (RT_OPT_FRAME_KERNEL 1), the call is one launch of the regenerating frame kernel (k_frame_regen), whose rounds mix the
-paths of different bounces and samples; otherwise the frames of rt_integrate's schedule run n times with the statistics summed
-on the device.  A band of rows is also compared with the CPU oracle rendering the samples in sequence.
+over the frames, plus (where stated) the AOV buffers, the resolved views and the fused-gather slab.  The frames of rt_integrate's
+schedule run n times with the statistics summed on the device: n one-kernel frames where RT_OPT_FRAME_KERNEL 1 forces it (or
+the default selects it), n per-phase frames otherwise.  A band of rows is also compared with the CPU oracle rendering the
+samples in sequence.
 """
 import numpy as np
 import pytest
@@ -82,8 +82,8 @@ def oracle_rows(sc, cam, w, h, mb, n, row_first, row_step, tables=None, wf=False
 @pytest.mark.parametrize("staging", list(STAGING))
 def test_samples_match_frames_and_oracle(staging, n):
     """CornellBox (BVH staged whole), ShaderBalls through L1 and with the top of its tree staged, for every RT_OPT_FRAME_KERNEL
-    mode: mode 1 runs the regenerating kernel, mode 2 (default) k_frame n times at this size, mode 0 the per-phase graph n
-    times.  A band of rows equals the oracle's n samples in sequence."""
+    mode: modes 1 and 2 (default) run k_frame n times at this size, mode 0 the per-phase graph n times.  A band of rows equals
+    the oracle's n samples in sequence."""
     name, options = STAGING[staging]
     sc = scene(name)
     w, h, mb = 120, 68, 6
@@ -142,8 +142,8 @@ def test_late_sample_indices(sampler, start, n):
 
 @pytest.mark.parametrize("mb,sampler", [(60, "blue_noise"), (255, "random")])
 def test_long_paths(mb, sampler):
-    """The closed Cornell box, whose paths last up to RT_MAX_BOUNCES bounces: the regenerating kernel's rounds hold live paths of
-    many different bounces and samples at once, and the per-bounce statistics are counted by each path's own bounce."""
+    """The closed Cornell box, whose paths last up to RT_MAX_BOUNCES bounces, on the forced one-kernel frame: the per-bounce
+    statistics of the long paths add up over the call's frames."""
     w, h, n = 64, 48, 4
     sc = closed_cornell(); cam = default_camera(w, h)
     tables = synthetic_sampler_tables() if sampler == "blue_noise" else None
@@ -187,9 +187,9 @@ def test_after_earlier_frames_and_reset():
         got.destroy(); want.destroy()
 
 
-def test_regenerating_call_is_one_launch():
-    """With RT_OPT_FRAME_KERNEL 1 and no gather target a call is exactly one kernel launch for any n; the default selector runs
-    n one-kernel frames at this size, which add up their statistics, and one statistics sum at the end."""
+def test_forced_frame_kernel_call_launches():
+    """With RT_OPT_FRAME_KERNEL 1, and with the default selector at this size, a call of n samples is n one-kernel frames, which
+    add up their statistics, and one statistics sum at the end, whatever the BVH staging."""
     name, w, h, mb = "ShaderBalls", 96, 54, 4
     sc = scene(name); cam = default_camera(w, h)
     for staging in ((), ((capi.OPT_TOP_SMEM, 100),), ((capi.OPT_SMEM_BVH, 0),)):
@@ -197,7 +197,7 @@ def test_regenerating_call_is_one_launch():
         for n in (2, 5, 17, 64):
             before = c.launch_count()
             c.integrate_samples(mb, n)
-            assert c.launch_count() - before == 1, (staging, n)
+            assert c.launch_count() - before == n + 1, (staging, n)
         c.destroy()
     c = make(scene("CornellBox"), default_camera(w, h), w, h)
     before = c.launch_count()
@@ -234,19 +234,6 @@ def test_taps_after_a_call_see_one_frame_at_most(fk):
         got.destroy(); want.destroy()
 
 
-def test_regenerating_kernel_sample_limit():
-    """The regenerating kernel carries a path's sample offset in 24 bits: more than RT_MAX_REGEN_SAMPLES samples in one call are
-    refused before anything is enqueued."""
-    name, w, h, mb = "CornellBox", 64, 32, 2
-    sc = scene(name); cam = default_camera(w, h)
-    c = make(sc, cam, w, h, ((capi.OPT_FRAME_KERNEL, 1),))
-    before = c.launch_count()
-    with pytest.raises(capi.RtError) as e:
-        c.integrate_samples(mb, (1 << 24) + 1)
-    assert e.value.code == -1 and c.launch_count() == before and c.sample_count() == 0
-    c.destroy()
-
-
 @pytest.mark.parametrize("fk", [1, 2])
 @pytest.mark.parametrize("present", [0, 1])
 def test_multi_device_context(present, fk):
@@ -269,7 +256,7 @@ def test_multi_device_context(present, fk):
 
 def test_fused_gather_slab_equals_radiance():
     """rt_set_gather_target on three partition contexts: after a multi-sample call and rt_gather_wait the gather buffer, resolved
-    with rt_resolve_gathered, equals the single-context image; on the regenerating kernel and on the per-phase schedule."""
+    with rt_resolve_gathered, equals the single-context image; on the one-kernel frame and on the per-phase schedule."""
     name, w, h, mb, n = "ShaderBalls", 150, 83, 5, 3
     sc = scene(name); cam = default_camera(w, h)
     for fk in (1, 2, 0):

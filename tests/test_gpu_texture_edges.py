@@ -3,7 +3,7 @@ GPU tests (-m gpu) of the textured-material path at its edges (tests/texture_cas
 and sample textures per hit (rt_device.cuh: unpack_material, sample_texture):
 
 - the texture chart and a textured OBJ loaded by the host loader, under every rt_integrate schedule, the stepwise steps,
-  rt_integrate_samples (per-phase and regenerating) and rank 2 of a 3-way partition, 3 progressive samples of 6 bounces, bit for
+  rt_integrate_samples (per-phase and one-kernel frames) and rank 2 of a 3-way partition, 3 progressive samples of 6 bounces, bit for
   bit against the oracle: radiance, per-bounce counters, the AOVs and the stepwise arm's primary hits;
 - known answers at max_bounces = 0 without the oracle: the chart's albedo AOV is the numpy restatement of
   tests/test_texture_edges_cpu.py, and the emission ladder's radiance is ldexp(mantissa, e - 136) in float64 at every covered
@@ -86,7 +86,7 @@ def test_every_schedule_matches_oracle(case, tmp_path_factory):
             rows = np.arange(2, h, 3)
             rad = np.zeros((h, w, 4), "<f4"); part.read_radiance(rad)
             assert np.array_equal(bits(rad[rows][..., :3]), bits(pacc[rows][..., :3])), (case, "rank 2 of 3", s)
-        for fk in (0, 1):                 # rt_integrate_samples: the per-phase frames, the regenerating one-kernel frame
+        for fk in (0, 1):                 # rt_integrate_samples: the per-phase frames, the one-kernel frames
             c = samples_ctx(sc, cam, w, h, ((capi.OPT_FRAME_KERNEL, fk),))
             c.integrate_samples(MB, SAMPLES)
             assert c.sample_count() == SAMPLES

@@ -7,7 +7,7 @@ sample_bxdf and bxdf_eval_sampled take their per-material constants from one der
 sample_bxdf skips the Fresnel term of materials without specular.
 
 - Radiance bits and per-bounce counters equal the oracle's on every schedule (per-phase, one-kernel frame, stepwise),
-  the regenerating frame (rt_integrate_samples) and both ranks of a 2-way partition, for one directional light, several
+  rt_integrate_samples on the one-kernel frame and both ranks of a 2-way partition, for one directional light, several
   directional lights, a point light among directional lights, and materials with and without specular, metals and textures.
   With emitter and environment sampling on, every schedule agrees with the one-kernel frame.
 """
@@ -105,7 +105,7 @@ def test_every_schedule_matches_oracle(name):
             check_stats(c.frame_stats(), ost[-1], (name, schedule))
         finally:
             c.destroy()
-    # the regenerating one-kernel frame: two samples in one call
+    # rt_integrate_samples on the one-kernel frame: two samples in one call
     c = ctx(sc, cam, "frame")
     try:
         c.integrate_samples(MB, 2)

@@ -28,8 +28,7 @@ from raytracing_b200.camera import default_camera  # noqa: E402
 
 W, H, MB = 1920, 1080, 8
 STAT_KEYS = ("n_ext", "n_miss", "n_shadow", "n_cont", "n_unoccluded", "n_emissive_hits")
-# name: (world, RT_OPT_FRAME_KERNEL).  Rank 0 of 4 takes the default selection, which is k_frame there (518 400 pixels <= 132 SMs x 7168):
-# RT_OPT_FRAME_KERNEL 1 would make rt_integrate_samples run the regenerating kernel with the feature off and N x k_frame with it on.
+# name: (world, RT_OPT_FRAME_KERNEL).  Rank 0 of 4 takes the default selection, which is k_frame there (518 400 pixels <= 132 SMs x 7168).
 CONFIGS = {"whole": (1, 0), "rank0of4": (4, 2)}
 CHUNK, CAP, REF_SPP = 16, 256, 2048
 

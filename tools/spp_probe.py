@@ -4,7 +4,7 @@ partitions at 1920x1080 x 8 bounces (one GPU renders rank 0's rows, as tools/par
 For every scene, partition and N the two arms are first checked to give byte-identical radiance and summed per-bounce statistics,
 then timed with CUDA events around the whole call (ms per sample), the arms alternating, the set repeated.  "frames" and
 "samples" run the default schedule selection (the per-phase graph on the whole frame and on a 2-way partition, k_frame below);
-"frames_fk1" (N x k_frame) and "samples_fk1" (the regenerating kernel) force the one-kernel frame.
+"frames_fk1" (N x k_frame) forces the one-kernel frame and must give the same radiance.
 
     python tools/spp_probe.py [--out DIR] [--reps 3] [--rounds 2]
 """
@@ -83,21 +83,18 @@ def main():
     for name in a.scenes.split(","):
         sc = scene_io.load_scene(name)
         for world in map(int, a.worlds.split(",")):
-            arms = {"frames": None, "samples": None, "frames_fk1": 1, "samples_fk1": 1}
+            arms = {"frames": None, "samples": None, "frames_fk1": 1}
             ctxs = {arm: context(sc, world, fk) for arm, fk in arms.items()}
             for n in map(int, a.ns.split(",")):
-                # correctness first: both arms of each schedule give the same bytes
+                # correctness first: the arms give the same bytes
                 outs = {}
                 for arm, c in ctxs.items():
                     st = run(c, arm, n)
                     outs[arm] = (c.read_radiance().tobytes(), st)
-                for f, s in (("frames", "samples"), ("frames_fk1", "samples_fk1")):
-                    if f not in outs:
-                        continue
-                    same = outs[f][0] == outs[s][0] and all(np.array_equal(outs[f][1][k], outs[s][1][k]) for k in STAT_KEYS)
-                    if not same:
-                        raise SystemExit(f"{name} world {world} N {n}: {s} differs from {f}")
-                if "frames_fk1" in outs and outs["frames"][0] != outs["frames_fk1"][0]:
+                f, s = outs["frames"], outs["samples"]
+                if f[0] != s[0] or not all(np.array_equal(f[1][k], s[1][k]) for k in STAT_KEYS):
+                    raise SystemExit(f"{name} world {world} N {n}: samples differs from frames")
+                if outs["frames"][0] != outs["frames_fk1"][0]:
                     raise SystemExit(f"{name} world {world} N {n}: the schedules differ")
                 for arm, c in ctxs.items():            # warm-up
                     timed(c, arm, n)
