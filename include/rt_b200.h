@@ -540,7 +540,11 @@ int rt_rebuild_bvh_ploc(rt_ctx* ctx, uint64_t* n_nodes);
  * The top-level tree and the world boxes follow the rule of raytracing_b200/csrc/rt_instances.h.
  * Virtual triangle ids: instance i covers [base_i, base_i + n_triangles(mesh_i)), base = the prefix sum in instance order, so
  * RtHit.primitive_id, rt_read_hits and the statistics read as for the flattened scene.
- * Traversal: the top-level tree with the slab test, near/far order and deferred-child stack of the flat traversal; at an instance
+ * Traversal: the top-level tree with the slab test, near/far order and deferred-child stack of the flat traversal, every top-level
+ * box widened on each side by the ray's slack e = max(|o.x|, |o.y|, |o.z|) * a + b, with (a, b) computed by rt_set_instances from
+ * the largest condition number ||A||_inf ||A^-1||_inf of the list, the world boxes and the translations (rt_instances.h states
+ * the rule and its bound): a top-level box never culls a hit that the mesh's own tree finds for the object-space ray, for any |o|,
+ * any condition number and t <= RT_MAX_RENDER_DIST (where e overflows every box passes); at an instance
  * the ray goes to object space, all float without contraction: o' = ((W0*o.x + W1*o.y) + W2*o.z) + W3 per row, d' = (W0*d.x + W1*d.y)
  * + W2*d.z; d' is not renormalised, so t is the same parameter in both spaces, and the mesh's tree is traced with the shared
  * t_max as a flat scene's (a later equal-t hit replaces the earlier, across instances too), except that the back-face test reads

@@ -10,8 +10,21 @@
  *   base   the prefix sum of n_triangles(mesh) in instance order; the sum must stay below RT_INVALID_ID (0xFFFFFFFF).
  *   box    the 8 corners of the mesh's root box (node first_node of the mesh) transformed by M in double
  *          (x = ((m00*cx + m01*cy) + m02*cz) + m03), min / max per component, widened by pad = RT_INST_BOX_PAD * s on each side,
- *          s = the largest |value| of the six, and rounded outward to float.  The box only culls; the pad covers the rounding of
- *          the ray transform.
+ *          s = the largest |value| of the six, and rounded outward to float.  The box only culls.
+ *   kappa  ||A||_inf * ||A^-1||_inf (row-sum norms, A the 3x3 part, A^-1 = adj(A) / det, in double): the condition number of M.
+ * Slack (two floats in the header, per list): a = RT_INST_RAY_SLACK * max_i kappa_i and b = RT_INST_RAY_SLACK * max_i kappa_i *
+ *   (s_i + |t_i|_inf) (s_i = the largest |coordinate| of instance i's float world box, t_i = M's translation column), both in
+ *   double and rounded up to float.  The traversal tests every top-level
+ *   box (the root box and both children of each record) widened by e = max(|o.x|, |o.y|, |o.z|) * a + b (float, in that order) on
+ *   each side: lo - e, hi + e.  Why that is enough: a hit that the mesh's tree yields for the object-space ray (o', d') has a t at
+ *   which o' + t d' meets the mesh's root box up to the rounding of its slab test.  Mapped by M, that point is within
+ *   c * u * kappa * (|o|_inf + s + |t|_inf) of the unpadded world box, u = 2^-24: W's rounding to float, the rounding of o' and d'
+ *   (dot products of 3 terms, so |W| |o| + |w| <= kappa-scaled terms, t |d| <= |o| + s + e for a point in the box), the object-space
+ *   slab rounding and the world slab rounding together give c < 64.  RT_INST_RAY_SLACK = 2^-16 = 256 u covers that with a factor
+ *   4 to spare, and covers the rounding of e and of lo - e, hi + e.  The widening also keeps a ray with a zero direction component
+ *   that starts on a box plane away from the plane (no 0 * inf).  Domain: finite rays (d != 0) and finite matrices, any |o|, any
+ *   kappa and any t <= RT_MAX_RENDER_DIST; where e overflows to inf every box passes (no culling, hits unchanged).  The flat
+ *   traversal is unchanged: a flat scene has no header.
  * Top-level tree (one instance per leaf), built recursively over a list of instances, starting with all of them in index order:
  *   one instance: a leaf.  Otherwise centroid c = (lo + hi) * 0.5f (float) per instance; the centroid bounds' extent per axis
  *   (float max - min); axis = 0, then 1 if ext1 > ext_axis, then 2 if ext2 > ext_axis; the list is sorted stably by (c[axis],
@@ -33,15 +46,16 @@
 #include "rt_b200.h"
 
 #define RT_INST_BOX_PAD 0x1p-20
+#define RT_INST_RAY_SLACK 0x1p-16
 
 namespace rtinst
 {
 
 struct Box { float lo[3], hi[3]; };
 
-// The instance's world-to-object matrix (12 floats, row-major 3x4) and the sign of det (+1 / -1); false for a matrix that is not
-// finite or is singular.
-inline bool invert(const float* m, float* w, float* det_sign)
+// The instance's world-to-object matrix (12 floats, row-major 3x4), the sign of det (+1 / -1) and the condition number kappa;
+// false for a matrix that is not finite or is singular.
+inline bool invert(const float* m, float* w, float* det_sign, double* kappa)
 {
     for (int k = 0; k < 12; ++k) if (!std::isfinite(m[k])) return false;
     const double a = m[0], b = m[1], c = m[2], d = m[4], e = m[5], f = m[6], g = m[8], h = m[9], k = m[10];
@@ -57,6 +71,13 @@ inline bool invert(const float* m, float* w, float* det_sign)
         w[4 * r + 3] = (float)(-(inv[3 * r] * t[0] + inv[3 * r + 1] * t[1] + inv[3 * r + 2] * t[2]));
     }
     *det_sign = det < 0.0 ? -1.0f : 1.0f;
+    double na = 0.0, ni = 0.0;
+    for (int r = 0; r < 3; ++r)
+    {
+        na = std::max(na, (std::fabs((double)m[4 * r]) + std::fabs((double)m[4 * r + 1])) + std::fabs((double)m[4 * r + 2]));
+        ni = std::max(ni, (std::fabs(inv[3 * r]) + std::fabs(inv[3 * r + 1])) + std::fabs(inv[3 * r + 2]));
+    }
+    *kappa = na * ni;
     return true;
 }
 
@@ -98,6 +119,7 @@ struct Tree
     std::vector<float> records;   // 16 floats per interior node (rt_bvh_layout.h's layout)
     Box root = {};                // union of every instance box
     int root_ref = 0;             // 0, or ~0 for a single instance
+    float slack[2] = {};          // (a, b) of the top-level box widening
 };
 
 inline float int_bits(int v) { float f; memcpy(&f, &v, 4); return f; }
@@ -165,13 +187,15 @@ inline bool prepare(const RtInstance* inst, uint32_t n, const std::vector<MeshIn
 {
     out.rec.assign((size_t)n * 32, 0.0f); out.base.assign(n, 0u); out.boxes.resize(n);
     uint64_t next = 0;
+    double kappa_max = 0.0, reach_max = 0.0;
     for (uint32_t i = 0; i < n; ++i)
     {
         const RtInstance& in = inst[i];
         if (in.mesh >= meshes.size()) { err = "instance " + std::to_string(i) + " names mesh " + std::to_string(in.mesh) + " of " + std::to_string(meshes.size()); return false; }
         float* r = out.rec.data() + (size_t)i * 32;
         float sign = 1.0f;
-        if (!invert(in.object_to_world, r, &sign)) { err = "instance " + std::to_string(i) + " has a matrix that is not finite or is singular"; return false; }
+        double kappa = 0.0;
+        if (!invert(in.object_to_world, r, &sign, &kappa)) { err = "instance " + std::to_string(i) + " has a matrix that is not finite or is singular"; return false; }
         const MeshInfo& m = meshes[in.mesh];
         memcpy(r + 12, in.object_to_world, 48);
         out.base[i] = (uint32_t)next;
@@ -180,10 +204,20 @@ inline bool prepare(const RtInstance* inst, uint32_t n, const std::vector<MeshIn
         r[28] = sign; r[29] = int_bits((int)m.first_node);
         next += m.n_tris;
         if (next >= 0xFFFFFFFFull) { err = "the instances cover 2^32 - 1 or more triangle ids"; return false; }
-        out.boxes[i] = world_box(in.object_to_world, m.lo, m.hi);
+        const Box& b = out.boxes[i] = world_box(in.object_to_world, m.lo, m.hi);
+        double s = 0.0, t = 0.0;
+        for (int k = 0; k < 3; ++k)
+        {
+            s = std::max(s, std::max(std::fabs((double)b.lo[k]), std::fabs((double)b.hi[k])));
+            t = std::max(t, std::fabs((double)in.object_to_world[4 * k + 3]));
+        }
+        kappa_max = std::max(kappa_max, kappa);
+        reach_max = std::max(reach_max, kappa * (s + t));
     }
     if (n) build_tree(out.boxes, out.tree);
     else out.tree = Tree();
+    out.tree.slack[0] = round_up(RT_INST_RAY_SLACK * kappa_max);
+    out.tree.slack[1] = round_up(RT_INST_RAY_SLACK * reach_max);
     return true;
 }
 

@@ -1957,11 +1957,11 @@ static int alloc_instances(rt_ctx* c, uint32_t cap)
     DevAllocs g;
     char* base = nullptr;
     const size_t top = (size_t)std::max(cap, 2u) - 1u;
-    const size_t f4 = 2 + top * 4 + (size_t)cap * 8 + (size_t)cap * 3 + ((size_t)cap + 3) / 4;
+    const size_t f4 = 3 + top * 4 + (size_t)cap * 8 + (size_t)cap * 3 + ((size_t)cap + 3) / 4;
     RT_CUDA(c, g.alloc(base, f4 * 16));
     RT_CUDA(c, cudaMemset(base, 0, f4 * 16));
     float4* p = (float4*)base;
-    c->inst_hdr = p; c->inst_top = p + 2; c->inst_rec = c->inst_top + top * 4; c->inst_prev = c->inst_rec + (size_t)cap * 8;
+    c->inst_hdr = p; c->inst_top = p + 3; c->inst_rec = c->inst_top + top * 4; c->inst_prev = c->inst_rec + (size_t)cap * 8;
     c->inst_base = (uint32_t*)(c->inst_prev + (size_t)cap * 3);
     c->inst_mem = std::move(g); c->inst_cap = cap;
     ++c->config_gen;
@@ -2140,16 +2140,17 @@ int rt_upload_instanced_scene(rt_ctx* c, const RtSceneDesc* s, const RtMeshDesc*
     return upload_scene(c, s, meshes, n_meshes);
 }
 
-// The head of the instance buffer's image: the header (top-level root box, root reference, instance count) and the top-level
-// records, 2 + 4 (n - 1) float4 (2 for n <= 1).  rt_set_instances writes them with the rest of the image,
+// The head of the instance buffer's image: the header (top-level root box, root reference, instance count, the slack (a, b) of
+// rt_instances.h) and the top-level records, 3 + 4 (n - 1) float4 (3 for n <= 1).  rt_set_instances writes them with the rest of the image,
 // rt_update_mesh_triangles alone.
 static size_t top_level_image(const rtinst::Prepared& pr, uint32_t n, float4* h)
 {
     const rtinst::Box& rb = pr.tree.root;
     h[0] = make_float4(rb.lo[0], rb.lo[1], rb.lo[2], rtinst::int_bits(pr.tree.root_ref));
     h[1] = make_float4(rb.hi[0], rb.hi[1], rb.hi[2], rtinst::int_bits((int)n));
-    memcpy(&h[2], pr.tree.records.data(), pr.tree.records.size() * 4);
-    return 2 + pr.tree.records.size() / 4;
+    h[2] = make_float4(pr.tree.slack[0], pr.tree.slack[1], 0.0f, 0.0f);
+    memcpy(&h[3], pr.tree.records.data(), pr.tree.records.size() * 4);
+    return 3 + pr.tree.records.size() / 4;
 }
 
 int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
@@ -2172,11 +2173,11 @@ int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
         c->scene_mid = make_float4((b.lo[0] + b.hi[0]) * 0.5f, (b.lo[1] + b.hi[1]) * 0.5f, (b.lo[2] + b.hi[2]) * 0.5f, 0.0f);
     }
     const size_t top = (size_t)std::max(c->inst_cap, 2u) - 1u;
-    const size_t f4 = 2 + top * 4 + (size_t)c->inst_cap * 11 + ((size_t)c->inst_cap + 3) / 4;
+    const size_t f4 = 3 + top * 4 + (size_t)c->inst_cap * 11 + ((size_t)c->inst_cap + 3) / 4;
     std::vector<float4>& h = c->inst_host;
     h.assign(f4, make_float4(0.0f, 0.0f, 0.0f, 0.0f));
     top_level_image(pr, n, h.data());
-    float4* rec = &h[2 + top * 4];
+    float4* rec = &h[3 + top * 4];
     memcpy(rec, pr.rec.data(), pr.rec.size() * 4);
     float4* prev = rec + (size_t)c->inst_cap * 8;
     // previous transforms: index i's transform in the last earlier list that had index i, else its new one

@@ -30,7 +30,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 #define RT_SMEM_INST 4
 struct DevInstScene : DevScene
 {
-    const float4* inst_hdr;        // 2 float4: (top root box min xyz, root ref), (root box max xyz, instance count) as int bits
+    const float4* inst_hdr;        // 3 float4: (top root box min xyz, root ref), (root box max xyz, instance count) as int bits,
+                                   // (slack a, slack b, -, -) of rt_instances.h
     const float4* top;             // top-level records (rt_bvh_layout.h layout, leaf ref = ~instance), rt_instances.h
     const float4* irec;            // 8 float4 per instance: W rows, M rows, (mesh root ref, mesh record base in float4, first
                                    // triangle, base) as int bits, (det sign, first node bits, -, -)
@@ -437,7 +438,8 @@ __device__ __forceinline__ uint32_t trace_fast(const DevScene& sc, const float4*
 }
 
 // Two-level traversal of an instanced scene (rt_b200.h, instanced scenes).  The top-level tree is walked as trace_fast walks a
-// flat one from L1 (same slab test, near/far order, pop rule and 64-entry stack); at an instance leaf the ray is moved into
+// flat one from L1 (same slab test, near/far order, pop rule and 64-entry stack), on every box widened by the ray's slack
+// e = max|o| * a + b (rt_instances.h: no box culls a hit the mesh's tree finds); at an instance leaf the ray is moved into
 // object space by W and the mesh's tree is traced by trace_fast itself, on a view of DevScene whose arrays start at the mesh's,
 // with the shared t_max and a stack of its own.  A hit stores the instance's virtual id, base + the mesh's triangle index.
 // COUNT counts every node whose box is tested once: the top-level root (the header box) and the two children of each top-level
@@ -447,11 +449,12 @@ __device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o
                                                     float& bu, float& bv, float& bt, uint32_t& nv, uint32_t& nt)
 {
     uint32_t prim = RT_INVALID_ID;
-    const float4 h0 = __ldg(sc.inst_hdr), h1 = __ldg(sc.inst_hdr + 1);
+    const float4 h0 = __ldg(sc.inst_hdr), h1 = __ldg(sc.inst_hdr + 1), h2 = __ldg(sc.inst_hdr + 2);
     if (__float_as_uint(h1.w) == 0u) return prim;                  // no instances: every ray misses
     const f3 inv = splat(1.0f) / d;
+    const float e = fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fabsf(o.z)) * h2.x + h2.y;
     if (COUNT) ++nv;
-    if (!box_hit(mk3(h0), mk3(h1), o, inv, t_min, t_max)) return prim;       // root box
+    if (!box_hit(mk3(h0.x - e, h0.y - e, h0.z - e), mk3(h1.x + e, h1.y + e, h1.z + e), o, inv, t_min, t_max)) return prim;   // root box
     int cur = __float_as_int(h0.w);
     int sp = 0;
     int stack_ref[64];
@@ -462,7 +465,10 @@ __device__ __forceinline__ uint32_t trace_instanced(const DevInstScene& sc, f3 o
         {
             const float4* np = sc.top + (size_t)cur * 4;
             if (COUNT) nv += 2;
-            const ChildPair s = child_pair<false>(__ldg(np), __ldg(np + 1), __ldg(np + 2), __ldg(np + 3), o, inv, 0u, t_min, t_max);
+            const float4 a = __ldg(np), b = __ldg(np + 1), c = __ldg(np + 2);
+            // child 0: min (a.x, a.y, a.z) max (a.w, b.x, b.y); child 1: min (b.z, b.w, c.x) max (c.y, c.z, c.w)
+            const ChildPair s = child_pair<false>(make_float4(a.x - e, a.y - e, a.z - e, a.w + e), make_float4(b.x + e, b.y + e, b.z - e, b.w - e),
+                                                  make_float4(c.x - e, c.y + e, c.z + e, c.w + e), __ldg(np + 3), o, inv, 0u, t_min, t_max);
             if (s.near_hit)
             {
                 if (s.far_hit) { stack_ref[sp] = s.far_ref; stack_t[sp] = s.far_lo; ++sp; }

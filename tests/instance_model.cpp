@@ -3,8 +3,8 @@
  * include/rt_b200.h): one sample of the oracle's frame (oracle/oracle.cpp orc_render) with the two-level traversal and instanced
  * shading.  It compiles oracle.cpp into the same translation unit for its building blocks (ray generation, sky, lights, materials,
  * BSDF sampling) and uses the library's own top-level builder (raytracing_b200/csrc/rt_instances.h), so the model and the device
- * trace the same tree.  The traversal restates trace_instanced: the top-level walk with trace_fast's slab test, near/far order and
- * pop rule, the ray moved into object space by W, and the mesh traced by the reference-order traversal (which trace_fast equals
+ * trace the same tree.  The traversal restates trace_instanced: the top-level walk with trace_fast's slab test on boxes widened
+ * by the ray's slack (rt_instances.h), near/far order and pop rule, the ray moved into object space by W, and the mesh traced by the reference-order traversal (which trace_fast equals
  * bit for bit) with the back-face test on det * sign(det M).  Built by tests/instance_model.py with -ffp-contract=off.
  */
 #include "oracle.cpp"
@@ -34,9 +34,10 @@ inline V3 XNormalT(const float* w, V3 n)     // W^T * n
     return v3((w[0] * n.x + w[4] * n.y) + w[8] * n.z, (w[1] * n.x + w[5] * n.y) + w[9] * n.z, (w[2] * n.x + w[6] * n.y) + w[10] * n.z);
 }
 
-inline bool SlabHit(const float* lo3, const float* hi3, V3 o, V3 inv, float t_min, float t_max, float* entry)
+// the slab test of the box (lo3, hi3) widened by e on each side
+inline bool SlabHit(const float* lo3, const float* hi3, float e, V3 o, V3 inv, float t_min, float t_max, float* entry)
 {
-    V3 t0 = (v3(lo3[0], lo3[1], lo3[2]) - o) * inv, t1 = (v3(hi3[0], hi3[1], hi3[2]) - o) * inv;
+    V3 t0 = (v3(lo3[0] - e, lo3[1] - e, lo3[2] - e) - o) * inv, t1 = (v3(hi3[0] + e, hi3[1] + e, hi3[2] + e) - o) * inv;
     float lo = rt_fmaxf(rt_fmaxf(rt_fmaxf(rt_fminf(t0.x, t1.x), rt_fminf(t0.y, t1.y)), rt_fminf(t0.z, t1.z)), t_min);
     float hi = rt_fminf(rt_fminf(rt_fmaxf(t0.x, t1.x), rt_fmaxf(t0.y, t1.y)), rt_fmaxf(t0.z, t1.z));
     *entry = lo;
@@ -107,8 +108,10 @@ inline uint32_t InstTrace(const Scene& sc, const Inst& I, Ray ray, bool any_hit,
     const bool sx = inv.x < 0, sy = inv.y < 0, sz = inv.z < 0;
     float t_max = ray.tmax;
     const rtinst::Tree& tr = I.pr.tree;
+    const float e = rt_fmaxf(rt_fmaxf(std::fabs(o.x), std::fabs(o.y)), std::fabs(o.z)) * tr.slack[0] + tr.slack[1];
     {
-        V3 t0 = (v3(tr.root.lo[0], tr.root.lo[1], tr.root.lo[2]) - o) * inv, t1 = (v3(tr.root.hi[0], tr.root.hi[1], tr.root.hi[2]) - o) * inv;
+        V3 t0 = (v3(tr.root.lo[0] - e, tr.root.lo[1] - e, tr.root.lo[2] - e) - o) * inv,
+           t1 = (v3(tr.root.hi[0] + e, tr.root.hi[1] + e, tr.root.hi[2] + e) - o) * inv;
         float lo = rt_fmaxf(rt_fmaxf(rt_fminf(t0.x, t1.x), rt_fminf(t0.y, t1.y)), rt_fminf(t0.z, t1.z));
         float hi = rt_fminf(rt_fminf(rt_fmaxf(t0.x, t1.x), rt_fmaxf(t0.y, t1.y)), rt_fmaxf(t0.z, t1.z));
         if (!(rt_fminf(hi, t_max) >= rt_fmaxf(lo, ray.tmin))) return prim;
@@ -122,7 +125,7 @@ inline uint32_t InstTrace(const Scene& sc, const Inst& I, Ray ray, bool any_hit,
         {
             const float* r = tr.records.data() + 16 * (size_t)cur;
             float lo0, lo1;
-            bool h0 = SlabHit(r, r + 3, o, inv, ray.tmin, t_max, &lo0), h1 = SlabHit(r + 6, r + 9, o, inv, ray.tmin, t_max, &lo1);
+            bool h0 = SlabHit(r, r + 3, e, o, inv, ray.tmin, t_max, &lo0), h1 = SlabHit(r + 6, r + 9, e, o, inv, ray.tmin, t_max, &lo1);
             int r0, r1; uint32_t axis;
             memcpy(&r0, r + 12, 4); memcpy(&r1, r + 13, 4); memcpy(&axis, r + 14, 4);
             bool swap = axis == 0 ? sx : (axis == 1 ? sy : sz);
@@ -184,12 +187,8 @@ extern "C" {
 /* One sample of the instanced frame, as orc_render: scene = the concatenated meshes and the shared arrays; meshes, instances as
  * rt_upload_instanced_scene / rt_set_instances take them; prev (12 floats per instance, may be NULL) the previous transforms for
  * velocity (float2 per pixel, bounce-0 hits, camera == previous camera; may be NULL).  Returns 0, or -1 for a rejected list. */
-int im_render(const OrcScene* scene, const RtMeshDesc* meshes, uint32_t n_meshes, const RtInstance* instances, uint32_t n_inst,
-              const float* prev, const RtCamera* cam, uint32_t width, uint32_t height, uint32_t max_bounces, uint32_t sample_idx,
-              float* radiance, RtHit* primary_hits, OrcStats* stats, float* velocity)
+static bool make_inst(const Scene& sc, const RtMeshDesc* meshes, uint32_t n_meshes, const RtInstance* instances, uint32_t n_inst, Inst& I)
 {
-    Scene sc = to_scene(scene);
-    Inst I;
     for (uint32_t k = 0; k < n_meshes; ++k)
     {
         const RtMeshDesc& m = meshes[k];
@@ -199,8 +198,55 @@ int im_render(const OrcScene* scene, const RtMeshDesc* meshes, uint32_t n_meshes
         I.meshes.push_back(mi);
     }
     std::string err;
-    if (!rtinst::prepare(instances, n_inst, I.meshes, I.pr, err)) return -1;
+    if (!rtinst::prepare(instances, n_inst, I.meshes, I.pr, err)) return false;
     I.n = n_inst;
+    return true;
+}
+
+/* The two-level traversal of n rays (origin.w = t_min, direction.w = t_max, as orc_trace takes them): closest hits (virtual ids)
+ * into hits, or for any_hit 0 (occluded) / RT_INVALID_ID per ray into flags.  Returns 0, or -1 for a rejected list. */
+int im_trace(const OrcScene* scene, const RtMeshDesc* meshes, uint32_t n_meshes, const RtInstance* instances, uint32_t n_inst,
+             const RtRay* rays, uint32_t n, int any_hit, RtHit* hits, uint32_t* flags)
+{
+    Scene sc = to_scene(scene);
+    Inst I;
+    if (!make_inst(sc, meshes, n_meshes, instances, n_inst, I)) return -1;
+#pragma omp parallel for schedule(dynamic, 256)
+    for (long long i = 0; i < (long long)n; ++i)
+    {
+        Ray r; r.o = v3(rays[i].origin); r.tmin = rays[i].origin.w; r.d = v3(rays[i].direction); r.tmax = rays[i].direction.w;
+        RtHit h;
+        const uint32_t p = InstTrace(sc, I, r, any_hit != 0, any_hit ? nullptr : &h);
+        if (any_hit) flags[i] = p;
+        else hits[i] = h;
+    }
+    return 0;
+}
+
+/* Mesh `mesh`'s own tree alone (no top level) on n object-space rays, culling on det * cull: closest hits (mesh triangle ids). */
+void im_trace_mesh(const OrcScene* scene, const RtMeshDesc* meshes, uint32_t mesh, const RtRay* rays, uint32_t n, float cull, RtHit* hits)
+{
+    Scene sc = to_scene(scene);
+    Scene view = sc;
+    view.triangles = sc.triangles + meshes[mesh].first_triangle;
+    view.nodes = sc.nodes + meshes[mesh].first_node;
+#pragma omp parallel for schedule(dynamic, 256)
+    for (long long i = 0; i < (long long)n; ++i)
+    {
+        Ray r; r.o = v3(rays[i].origin); r.tmin = rays[i].origin.w; r.d = v3(rays[i].direction); r.tmax = rays[i].direction.w;
+        float u = 0.0f, v = 0.0f, t = 0.0f;
+        const uint32_t p = MeshTrace(view, r, cull, false, &u, &v, &t);
+        hits[i].bc.x = u; hits[i].bc.y = v; hits[i].t = t; hits[i].primitive_id = p;
+    }
+}
+
+int im_render(const OrcScene* scene, const RtMeshDesc* meshes, uint32_t n_meshes, const RtInstance* instances, uint32_t n_inst,
+              const float* prev, const RtCamera* cam, uint32_t width, uint32_t height, uint32_t max_bounces, uint32_t sample_idx,
+              float* radiance, RtHit* primary_hits, OrcStats* stats, float* velocity)
+{
+    Scene sc = to_scene(scene);
+    Inst I;
+    if (!make_inst(sc, meshes, n_meshes, instances, n_inst, I)) return -1;
 
     std::vector<uint32_t> pix;
     for (uint32_t y = 0; y < height; ++y)

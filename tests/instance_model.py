@@ -12,7 +12,7 @@ import numpy as np
 from oracle.orcbind import STATS_DT, Oracle
 from oracle.refbind import CAMERA_DT
 from raytracing_b200.capi import INSTANCE_DT
-from raytracing_b200.layouts import HIT_DT, NODE_DT, TRIANGLE_DT
+from raytracing_b200.layouts import HIT_DT, NODE_DT, RAY_DT, TRIANGLE_DT
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
@@ -32,6 +32,11 @@ def lib():
         L.im_render.restype = C.c_int
         L.im_render.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
                                 C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.im_trace.restype = C.c_int
+        L.im_trace.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p,
+                               C.c_void_p]
+        L.im_trace_mesh.restype = None
+        L.im_trace_mesh.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_float, C.c_void_p]
         _lib = L
     return _lib
 
@@ -74,3 +79,23 @@ class InstanceModel(Oracle):
         if rc != 0:
             raise ValueError("instance list rejected")
         return radiance, hits, stats, vel
+
+    def trace_instanced(self, mesh_ids, transforms, rays, any_hit=False):
+        """The two-level traversal of a batch of rays (RAY_DT; origin.w = t_min, direction.w = t_max) -> closest hits (HIT_DT, virtual
+        ids), or for any_hit a uint32 per ray: 0 if occluded, 0xFFFFFFFF if not."""
+        inst = instances(mesh_ids, transforms)
+        rays = np.ascontiguousarray(rays, dtype=RAY_DT)
+        hits = np.zeros(len(rays), dtype=HIT_DT)
+        flags = np.zeros(len(rays), dtype="<u4")
+        rc = lib().im_trace(C.addressof(self.scene), self.desc.ctypes.data, len(self.desc), inst.ctypes.data if len(inst) else None,
+                            len(inst), rays.ctypes.data, len(rays), int(any_hit), hits.ctypes.data, flags.ctypes.data)
+        if rc != 0:
+            raise ValueError("instance list rejected")
+        return flags if any_hit else hits
+
+    def trace_mesh(self, mesh, rays, cull=1.0):
+        """Mesh `mesh`'s own tree alone on object-space rays, culling on det * cull -> closest hits (HIT_DT, mesh triangle ids)."""
+        rays = np.ascontiguousarray(rays, dtype=RAY_DT)
+        hits = np.zeros(len(rays), dtype=HIT_DT)
+        lib().im_trace_mesh(C.addressof(self.scene), self.desc.ctypes.data, mesh, rays.ctypes.data, len(rays), cull, hits.ctypes.data)
+        return hits

@@ -7,11 +7,11 @@
 
 /* n instances (matrices m: 12 floats each, mesh ids) over meshes given by their root boxes (6 floats each: lo xyz, hi xyz) and
  * triangle counts.  Outputs: the instance records (32 floats each), the world boxes (6 floats each), the top-level records
- * (16 floats each, room for max(n - 1, 1)), their count, the root box (6 floats) and the root reference.  Returns 1, or 0 for a
- * rejected list (err gets the message). */
+ * (16 floats each, room for max(n - 1, 1)), their count, the root box (6 floats), the root reference and the slack (a, b).
+ * Returns 1, or 0 for a rejected list (err gets the message). */
 extern "C" int inst_prepare(const float* m, const uint32_t* mesh, uint32_t n, const float* mesh_boxes, const uint32_t* mesh_tris,
                             uint32_t n_meshes, float* rec, float* boxes, float* records, uint32_t* n_records, float* root, int* root_ref,
-                            char* err, int err_len)
+                            float* slack, char* err, int err_len)
 {
     std::vector<RtInstance> in(n);
     for (uint32_t i = 0; i < n; ++i) { memset(&in[i], 0, sizeof(RtInstance)); memcpy(in[i].object_to_world, m + 12 * i, 48); in[i].mesh = mesh[i]; }
@@ -33,5 +33,6 @@ extern "C" int inst_prepare(const float* m, const uint32_t* mesh, uint32_t n, co
     *n_records = (uint32_t)(pr.tree.records.size() / 16);
     memcpy(root, pr.tree.root.lo, 12); memcpy(root + 3, pr.tree.root.hi, 12);
     *root_ref = pr.tree.root_ref;
+    slack[0] = pr.tree.slack[0]; slack[1] = pr.tree.slack[1];
     return 1;
 }

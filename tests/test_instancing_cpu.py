@@ -23,7 +23,7 @@ def lib():
                     "-I" + os.path.join(REPO, "raytracing_b200", "csrc"), "-o", so, os.path.join(HERE, "instance_tree_host.cpp")], check=True)
     L = C.CDLL(so)
     L.inst_prepare.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
-                               C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.POINTER(C.c_int), C.c_char_p, C.c_int]
+                               C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_char_p, C.c_int]
     yield L
     os.remove(so)
 
@@ -37,12 +37,13 @@ def prepare(L, mats, mesh_ids, mesh_boxes, mesh_tris):
     rec = np.zeros((max(n, 1), 32), np.float32); boxes = np.zeros((max(n, 1), 6), np.float32)
     records = np.zeros((max(n - 1, 1), 16), np.float32); root = np.zeros(6, np.float32)
     nrec, ref = C.c_uint32(), C.c_int()
+    slack = np.zeros(2, np.float32)
     err = C.create_string_buffer(256)
     ok = L.inst_prepare(mats.ctypes.data, ids.ctypes.data, n, mb.ctypes.data, mt.ctypes.data, len(mt), rec.ctypes.data, boxes.ctypes.data,
-                        records.ctypes.data, C.byref(nrec), root.ctypes.data, C.byref(ref), err, 256)
+                        records.ctypes.data, C.byref(nrec), root.ctypes.data, C.byref(ref), slack.ctypes.data, err, 256)
     if not ok:
         return None, err.value.decode()
-    return {"rec": rec[:n], "boxes": boxes[:n], "records": records[:nrec.value], "root": root, "root_ref": ref.value}, ""
+    return {"rec": rec[:n], "boxes": boxes[:n], "records": records[:nrec.value], "root": root, "root_ref": ref.value, "slack": slack}, ""
 
 
 def rot(axis, ang):
@@ -76,9 +77,10 @@ def check(L, mats, ids, mesh_boxes, mesh_tris):
     assert np.array_equal(got["rec"][:, 27].view(np.uint32), base)
     for k, m in enumerate(mats):
         w, sign = model.inverse(m)
-        np.testing.assert_allclose(got["rec"][k, :12].reshape(3, 4), w, rtol=2e-7, atol=1e-30)
+        assert np.array_equal(got["rec"][k, :12].reshape(3, 4).view(np.uint32), w.view(np.uint32)), k
         np.testing.assert_array_equal(got["rec"][k, 12:24], np.asarray(m, np.float32).reshape(12))
         assert got["rec"][k, 28] == sign
+    assert np.array_equal(got["slack"].view(np.uint32), model.slack(mats, boxes).view(np.uint32)), (got["slack"], model.slack(mats, boxes))
     recs, root, ref = model.tree(boxes)
     assert got["root_ref"] == ref
     assert np.array_equal(got["root"].view(np.uint32), root.view(np.uint32))

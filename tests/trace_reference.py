@@ -52,13 +52,14 @@ def ray_arrays(rays, t_min=None, t_max=None):
     return o, d, np.asarray(lo, F), np.asarray(hi, F)
 
 
-def triangle_test(o, d, p1, p2, p3, t_min, t_max):
-    """The float32 test on matching rows (broadcast) -> accepted, u, v, t (u, v, t as computed; meaningful where accepted)."""
+def triangle_test(o, d, p1, p2, p3, t_min, t_max, sign=None):
+    """The float32 test on matching rows (broadcast) -> accepted, u, v, t (u, v, t as computed; meaningful where accepted).
+    sign (an instance's sign(det M), broadcast): the back-face test reads det * sign; u, v and t still divide by det."""
     with np.errstate(all="ignore"):
         e1, e2 = p2 - p1, p3 - p1
         pvec = _cross(d, e2)
         det = _dot(e1, pvec)
-        ok = ~(det < F(1e-8))
+        ok = ~((det if sign is None else det * F(sign)) < F(1e-8))
         inv_det = F(1.0) / det
         tvec = o - p1
         u = _dot(tvec, pvec) * inv_det
@@ -132,15 +133,24 @@ def closest(tris, rays, t_min=None, t_max=None, prefilter=None):
     p = tri_points(tris)
     if prefilter is None:
         prefilter = len(tris) > 256
-    out = Closest(len(o))
     acc, pairs = [], []
     for r, ti in candidate_pairs(p, o, d, hi, prefilter):
         ok, u, v, t = triangle_test(o[r], d[r], p[0][ti], p[1][ti], p[2][ti], lo[r], hi[r])
         acc.append((r[ok], ti[ok], t[ok], u[ok], v[ok]))
         if prefilter:
             pairs.append((r, ti))
+    out = reduce_accepted(len(o), acc)
     out.pairs = pairs or None                   # the prefilter's pairs, which classify() tests again in float64
-    r, ti, t, u, v = (np.concatenate(x) for x in zip(*acc))
+    return out
+
+
+def reduce_accepted(n, acc):
+    """The Closest of n rays from the accepted (ray, prim, t, u, v) arrays of acc."""
+    out = Closest(n)
+    if acc:
+        r, ti, t, u, v = (np.concatenate(x) for x in zip(*acc))
+    else:
+        r, ti, t, u, v = np.zeros(0, np.int64), np.zeros(0, np.uint32), np.zeros(0, F), np.zeros(0, F), np.zeros(0, F)
     ti = ti.astype(np.uint32)
     np.minimum.at(out.t, r, t)
     np.add.at(out.n_accepted, r, 1)
@@ -212,37 +222,38 @@ def near_box_face(nodes, o, d, t, prim):
     return near & ~outside
 
 
-def classify(tris, rays, nodes, ref, t_min=None, t_max=None, prefilter=None):
-    """-> (class index per ray into CLASSES, f64 nearest prim per ray (INVALID_ID if none)).  ref: closest() of the same rays."""
-    o, d, lo, hi = ray_arrays(rays, t_min, t_max)
-    p = tri_points(tris)
-    if prefilter is None:
-        prefilter = len(tris) > 256
-    n = len(o)
-    marginal_t = np.full(n, np.inf)               # the smallest t of a test that float32 might decide either way
-    hits = []
-    for r, ti in ref.pairs if getattr(ref, "pairs", None) is not None else candidate_pairs(p, o, d, hi, prefilter):
-        q1, q2, q3 = (x[ti].astype(np.float64) for x in p)
-        oo, dd = o[r].astype(np.float64), d[r].astype(np.float64)
-        with np.errstate(all="ignore"):
-            e1, e2 = q2 - q1, q3 - q1
-            pvec = _cross(dd, e2); det = _dot(e1, pvec)
-            tvec = oo - q1; qvec = _cross(tvec, e1)
-            u = _dot(tvec, pvec) / det; v = _dot(dd, qvec) / det; t = _dot(e2, qvec) / det
-            nrm = lambda a: np.sqrt((a * a).sum(-1))
-            size = nrm(tvec) + nrm(e1) + nrm(e2)
-            err = np.maximum(1.0, size * size * nrm(dd) / np.abs(det))        # conditioning of u and v
-            m = np.minimum(np.minimum(u, v), 1.0 - u - v)
-            t_tol = EPS * np.maximum(np.abs(t), err * nrm(e2) / np.maximum(nrm(dd), 1e-300))
-            det_tol = EPS * nrm(e1) * nrm(pvec) + EPS * 1e-8
-            hit = (det >= 1e-8) & (m >= 0) & (t >= lo[r]) & (t <= hi[r])
-            shaky = (np.abs(det - 1e-8) <= det_tol) | (np.abs(m) <= EPS * err) | (np.abs(t - lo[r]) <= t_tol) | \
-                    (np.abs(t - hi[r]) <= t_tol) | ~np.isfinite(t)
-        cand = shaky & (det > -det_tol)
-        np.minimum.at(marginal_t, r[cand], np.where(np.isfinite(t[cand]), t[cand], -np.inf))
-        h = hit & ~shaky
-        hits.append((r[h], t[h], ti[h]))
-    rr, tt, pp = (np.concatenate(x) for x in zip(*hits))
+def pair_classes(p, o, d, lo, hi, r, ti, marginal_t, sign=None):
+    """The float64 evaluation of the (ray r, triangle ti) pairs (sign as triangle_test's): lowers marginal_t (the smallest t of a
+    test that float32 might decide either way) per ray and -> the pairs that hit without doubt as (r, t, ti)."""
+    q1, q2, q3 = (x[ti].astype(np.float64) for x in p)
+    oo, dd = o[r].astype(np.float64), d[r].astype(np.float64)
+    with np.errstate(all="ignore"):
+        e1, e2 = q2 - q1, q3 - q1
+        pvec = _cross(dd, e2); det = _dot(e1, pvec)
+        tvec = oo - q1; qvec = _cross(tvec, e1)
+        u = _dot(tvec, pvec) / det; v = _dot(dd, qvec) / det; t = _dot(e2, qvec) / det
+        nrm = lambda a: np.sqrt((a * a).sum(-1))
+        size = nrm(tvec) + nrm(e1) + nrm(e2)
+        err = np.maximum(1.0, size * size * nrm(dd) / np.abs(det))        # conditioning of u and v
+        m = np.minimum(np.minimum(u, v), 1.0 - u - v)
+        t_tol = EPS * np.maximum(np.abs(t), err * nrm(e2) / np.maximum(nrm(dd), 1e-300))
+        det_tol = EPS * nrm(e1) * nrm(pvec) + EPS * 1e-8
+        cdet = det if sign is None else det * float(sign)
+        hit = (cdet >= 1e-8) & (m >= 0) & (t >= lo[r]) & (t <= hi[r])
+        shaky = (np.abs(cdet - 1e-8) <= det_tol) | (np.abs(m) <= EPS * err) | (np.abs(t - lo[r]) <= t_tol) | \
+                (np.abs(t - hi[r]) <= t_tol) | ~np.isfinite(t)
+    cand = shaky & (cdet > -det_tol)
+    np.minimum.at(marginal_t, r[cand], np.where(np.isfinite(t[cand]), t[cand], -np.inf))
+    h = hit & ~shaky
+    return r[h], t[h], ti[h]
+
+
+def ray_classes(n, hits, marginal_t, box):
+    """-> (class per ray, f64 nearest prim per ray) from pair_classes' hits and marginal_t, and the near_box_face rays."""
+    if hits:
+        rr, tt, pp = (np.concatenate(x) for x in zip(*hits))
+    else:
+        rr, tt, pp = np.zeros(0, np.int64), np.zeros(0), np.zeros(0, np.uint32)
     order = np.lexsort((pp, tt, rr))
     rr, tt, pp = rr[order], tt[order], pp[order]
     first = np.ones(len(rr), bool); first[1:] = rr[1:] != rr[:-1]
@@ -255,14 +266,27 @@ def classify(tris, rays, nodes, ref, t_min=None, t_max=None, prefilter=None):
     with np.errstate(invalid="ignore"):
         near_tie = np.isfinite(second) & (second - best <= EPS * np.maximum(np.abs(best), 1e-30))
     near_edge = marginal_t <= np.where(np.isfinite(best), best * (1 + EPS) + EPS, np.inf)
-    hit32 = ref.prim != INVALID_ID
-    box = np.zeros(n, bool)
-    box[hit32] = near_box_face(nodes, o[hit32], d[hit32], ref.t[hit32], ref.prim[hit32])
     cls = np.zeros(n, np.int64)
     cls[near_tie] = 1
     cls[near_edge] = 2
     cls[box] = 3
     return cls, best_p
+
+
+def classify(tris, rays, nodes, ref, t_min=None, t_max=None, prefilter=None):
+    """-> (class index per ray into CLASSES, f64 nearest prim per ray (INVALID_ID if none)).  ref: closest() of the same rays."""
+    o, d, lo, hi = ray_arrays(rays, t_min, t_max)
+    p = tri_points(tris)
+    if prefilter is None:
+        prefilter = len(tris) > 256
+    n = len(o)
+    marginal_t = np.full(n, np.inf)
+    hits = [pair_classes(p, o, d, lo, hi, r, ti, marginal_t)
+            for r, ti in (ref.pairs if getattr(ref, "pairs", None) is not None else candidate_pairs(p, o, d, hi, prefilter))]
+    hit32 = ref.prim != INVALID_ID
+    box = np.zeros(n, bool)
+    box[hit32] = near_box_face(nodes, o[hit32], d[hit32], ref.t[hit32], ref.prim[hit32])
+    return ray_classes(n, hits, marginal_t, box)
 
 
 def verdict(tris, rays, nodes, prim, bc, t, where, t_min=None, t_max=None, ref=None, cls=None, allow_box=0.01):
@@ -274,7 +298,14 @@ def verdict(tris, rays, nodes, prim, bc, t, where, t_min=None, t_max=None, ref=N
         cls = classify(tris, rays, nodes, ref, t_min, t_max)[0]
     prim = np.asarray(prim, np.uint32)
     hit = prim != INVALID_ID
-    ok, u, v, tt = restate(tris, rays[hit], prim[hit], t_min, t_max)
+    return judge(restate(tris, rays[hit], prim[hit], t_min, t_max), prim, bc, t, where, ref, cls, allow_box)
+
+
+def judge(restated, prim, bc, t, where, ref, cls, allow_box):
+    """verdict() on the hits' restated tests (accepted, u, v, t of every reported hit, in order)."""
+    prim = np.asarray(prim, np.uint32)
+    hit = prim != INVALID_ID
+    ok, u, v, tt = restated
     bad = np.flatnonzero(hit)[~ok]
     assert bad.size == 0, (where, "hit not accepted by the restated test", bad[:8].tolist(), prim[bad[:8]].tolist())
     got = np.ascontiguousarray(np.stack([bc[hit, 0], bc[hit, 1], t[hit]], 1), F).view(np.uint32)
@@ -286,7 +317,7 @@ def verdict(tris, rays, nodes, prim, bc, t, where, t_min=None, t_max=None, ref=N
     not_box = wrong[cls[wrong] != 3]
     assert not_box.size == 0, (where, "not the closest hit", [(int(i), int(prim[i]), float(t[i]), int(ref.prim[i]), float(ref.t[i]),
                                                             CLASSES[cls[i]]) for i in not_box[:8]])
-    assert wrong.size <= allow_box * len(rays), (where, "box-face misses", wrong.size, len(rays))
+    assert wrong.size <= allow_box * len(prim), (where, "box-face misses", wrong.size, len(prim))
     rep = {c: int((cls == i).sum()) for i, c in enumerate(CLASSES)}
     rep["ties"] = int((ref.n_ties > 1).sum())
     rep["box_misses"] = int(wrong.size)
