@@ -551,7 +551,8 @@ int rt_rebuild_bvh_ploc(rt_ctx* ctx, uint64_t* n_nodes);
  * det * sign(det M): a mirrored instance culls the faces its flattened triangles would.  Any-hit rays stop at the first hit.
  * Shading: the object-space position p as for flat scenes, then position = M * p (same row order as o'); the shading normal is
  * normalize(W^T * n) with n the interpolated vertex normal, the geometric normal normalize(W^T * n_g) * sign(det M); texture
- * coordinates, materials and emission are those of the mesh triangle.  With W = M = identity a frame equals that of the meshes
+ * coordinates, materials and emission are those of the mesh triangle (materials through the instance's row, if
+ * rt_set_instance_materials gave it one).  With W = M = identity a frame equals that of the meshes
  * uploaded flat, except where a signed zero or a NaN coordinate meets the matrix arithmetic (0 * x, -0 + 0).
  * Object motion (RT_OPT_OBJECT_MOTION): the previous transform M_prev of instance index i is its transform in the last earlier
  * rt_set_instances (since the upload) whose list had index i, or its current one if none had; the velocity AOV of a bounce-0 hit is
@@ -610,6 +611,35 @@ int rt_set_instances(rt_ctx* ctx, const RtInstance* instances, uint32_t n_instan
  * rt_launch_count.  rt_update_triangles*, the rebuilds and rt_read_bvh stay RT_ERR_UNSUPPORTED on instanced scenes. */
 int rt_update_mesh_triangles(rt_ctx* ctx, uint32_t mesh, const RtTriangle* triangles, uint64_t n_triangles);
 int rt_update_mesh_triangles_device(rt_ctx* ctx, uint32_t mesh, const void* device_triangles, uint64_t n_triangles);
+
+/* ---- per-instance materials in instanced scenes (new capability): each instance of a shared mesh shades with its own materials --
+ * Rows: `remaps` holds n_remaps rows of n_materials entries (n_materials = the upload's material count); row r maps scene
+ * material m to remaps[r * n_materials + m].  remap_of_instance[i] is the row of instance index i; RT_INVALID_ID, and every index
+ * >= n_instances, keeps the mesh's own materials.
+ * Rule: a hit on mesh triangle t of instance i with row r is shaded with material remaps[r * n_materials + t.mtlIndex] wherever
+ * the frame reads t.mtlIndex: the BSDF, the textured flag (whether texture coordinates are interpolated), the texture lookups
+ * (with the triangle's own texture coordinates), the emission and the n_emissive_hits count, and the albedo AOV.  Traversal,
+ * virtual ids, geometry, normals, depth, motion vectors, the light tables and the sort-key origin are unchanged.  So every output
+ * of a frame (radiance, statistics, the hits of every bounce, every AOV) equals, bit for bit, the frame of the same instanced scene
+ * uploaded with a private copy of its mesh for each instance that has a row, whose triangles carry the remapped mtlIndex, under
+ * the same transforms in the same order.
+ * Lifetime: the assignment is indexed by instance index and replaced whole by each call.  rt_set_instances keeps it (instance i
+ * of a later list uses the row given for index i, as the previous transforms of object motion are kept per index), and so do
+ * rt_update_mesh_triangles* and rt_reset; rt_upload_scene and rt_upload_instanced_scene clear it, and so does a call with
+ * n_remaps = n_instances = 0.
+ * Device side: the row offset r * n_materials (or RT_INVALID_ID) is a word of each instance record; the rows live in a table of
+ * their own (4 B per entry, allocated at the first call that needs it and freed by the next upload).  The shading pass of an
+ * instanced scene makes one dependent 4-byte load per hit of an instance with a row; flat scenes run the code they ran before.
+ * Ordering and buffers as for rt_set_instances: a deferred shadow pass is launched first and the copies are enqueued on the
+ * render stream; the call returns once both host arrays have been read.  The table grows to at least twice its size when a
+ * call needs more entries than it holds, the only case that re-captures a frame graph; otherwise no buffer moves.
+ * Errors, each leaving the next frame as it was: RT_ERR_NOT_READY without an instanced scene (none, or a flat one);
+ * RT_ERR_INVALID_ARGUMENT for a null pointer with a non-zero count, a row entry >= n_materials, a remap_of_instance entry that is
+ * neither < n_remaps nor RT_INVALID_ID, or n_remaps * n_materials >= 2^32 - 1 (row offsets fit 32 bits and stay distinct from
+ * RT_INVALID_ID).  Multi-device contexts fan out.  RtInstance, flat scenes and RT_OPT_EMITTER_SAMPLING (still RT_ERR_UNSUPPORTED
+ * on instanced scenes) are unchanged; RtInstance.padding stays without meaning. */
+int rt_set_instance_materials(rt_ctx* ctx, const uint32_t* remaps, uint32_t n_remaps, const uint32_t* remap_of_instance,
+                              uint32_t n_instances);
 
 /* ---- parity / measurement taps ---------------------------------------------------- */
 int rt_sync(rt_ctx* ctx);

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .layouts import (CAMERA_DT, HIT_DT, LIGHT_DT, MATERIAL_DT, NODE_DT, RAY_DT, SCENE_INFO_DT, TEXTURE_DT, TRIANGLE_DT)
+from .layouts import (CAMERA_DT, HIT_DT, INVALID_ID, LIGHT_DT, MATERIAL_DT, NODE_DT, RAY_DT, SCENE_INFO_DT, TEXTURE_DT, TRIANGLE_DT)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RT_B200_LIB", os.path.join(HERE, "librt_b200.so"))   # override: tuning variants
@@ -40,7 +40,7 @@ SYMBOLS = ["rt_create", "rt_destroy", "rt_last_error", "rt_set_partition", "rt_u
            "rt_set_adaptive_sampling", "rt_read_pixel_samples", "rt_read_active_pixels", "rt_set_spatial_denoiser",
            "rt_set_light_selection", "rt_update_triangles", "rt_update_triangles_device", "rt_read_bvh",
            "rt_rebuild_bvh", "rt_bvh_staging", "rt_rebuild_bvh_ploc", "rt_upload_instanced_scene", "rt_set_instances",
-           "rt_update_mesh_triangles", "rt_update_mesh_triangles_device"]
+           "rt_update_mesh_triangles", "rt_update_mesh_triangles_device", "rt_set_instance_materials"]
 
 
 class RtSceneDesc(C.Structure):
@@ -135,12 +135,27 @@ def load_library():
     L.rt_set_instances.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.rt_update_mesh_triangles.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64]
     L.rt_update_mesh_triangles_device.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64]
+    if hasattr(L, "rt_set_instance_materials"):   # absent from a variant library built from an earlier commit (RT_B200_LIB)
+        L.rt_set_instance_materials.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
     _lib = L
     return L
 
 
 # RtInstance (include/rt_b200.h): row-major 3x4 object-to-world matrix, mesh index, padding
 INSTANCE_DT = np.dtype([("object_to_world", "<f4", (12,)), ("mesh", "<u4"), ("padding", "<u4", (3,))])
+
+
+def instance_material_arrays(remaps, remap_of_instance):
+    """-> (rows, of) for rt_set_instance_materials: remaps as a C-contiguous uint32 (n_remaps, n_materials) array (an empty
+    sequence gives (0, 0)), remap_of_instance as uint32 with -1 / None as RT_INVALID_ID."""
+    rows = np.asarray(remaps if remaps is not None else [])
+    rows = np.ascontiguousarray(rows.reshape(0, 0) if rows.size == 0 else rows, dtype="<u4")
+    if rows.ndim != 2:
+        raise ValueError("set_instance_materials: remaps must be an (n_remaps, n_materials) array")
+    ids = [INVALID_ID if r is None or int(r) == -1 else int(r) for r in (remap_of_instance if remap_of_instance is not None else [])]
+    if any(r < 0 or r > INVALID_ID for r in ids):
+        raise ValueError("set_instance_materials: a row must be >= 0, or -1 / None")
+    return rows, np.ascontiguousarray(ids, dtype="<u4")
 
 
 def _scene_desc(scene: dict):
@@ -266,6 +281,14 @@ class Context:
         rec["object_to_world"] = m
         rec["mesh"] = ids
         self._ck(self.lib.rt_set_instances(self.h, rec.ctypes.data if len(rec) else None, len(rec)))
+
+    def set_instance_materials(self, remaps, remap_of_instance):
+        """Per-instance materials (rt_set_instance_materials): remaps = (n_remaps, n_materials) rows, row r mapping scene material m
+        to remaps[r, m]; remap_of_instance[i] = the row of instance index i, -1 / None for its mesh's own materials (indices beyond
+        the list keep theirs too).  Replaces the assignment; set_instances, mesh updates and reset() keep it, an upload clears it."""
+        rows, of = instance_material_arrays(remaps, remap_of_instance)
+        self._ck(self.lib.rt_set_instance_materials(self.h, rows.ctypes.data if rows.size else None, rows.shape[0],
+                                                    of.ctypes.data if of.size else None, len(of)))
 
     def set_camera(self, cam):
         c = np.ascontiguousarray(cam, dtype=CAMERA_DT)

@@ -130,7 +130,8 @@ __device__ __forceinline__ void shade_miss(const DevScene& sc, const FrameParams
 // RT_OPT_ENV_SAMPLING), each read only while it exists; a template flag, so that the kernels without it are the code of both options off.
 // INST: an instanced scene (rt_b200.h): prim is a virtual id; the hit is shaded on its mesh triangle and moved to world space by the
 // instance's M (position) and W^T (normals); the AOV's previous position places the mesh triangle's previous positions
-// (sc.prev_tri) by the instance's previous M (aov.prev_pos, 3 float4 per instance) when object motion is on.
+// (sc.prev_tri) by the instance's previous M (aov.prev_pos, 3 float4 per instance) when object motion is on; an instance with a
+// material row (rt_set_instance_materials) shades with sc.mtl_map[row offset + the triangle's material].
 template <bool EMIT = false, bool INST = false>
 __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FrameParams& p, const AovParams& aov, uint32_t bounce, uint32_t pxy,
                                           f3 ray_origin, f3 ray_dir, f3 hit_throughput, float prev_pdf, uint32_t prim, float u, float v,
@@ -179,6 +180,11 @@ __device__ __forceinline__ void shade_hit(const SceneOf<INST>& sc, const FramePa
     float4 r0 = __ldg(tp), r1 = __ldg(tp + 1), r2 = __ldg(tp + 2), r3 = __ldg(tp + 3), r4 = __ldg(tp + 4), r5 = __ldg(tp + 5);
     f3 p1 = mk3(r0), p2 = mk3(r1), p3 = mk3(r2), n1 = mk3(r3), n2 = mk3(r4), n3 = mk3(r5);
     uint32_t mtl = __float_as_uint(r0.w);
+    if constexpr (INST)
+    {   // per-instance materials (rt_set_instance_materials): the instance's row, read wherever the mesh triangle's material is
+        const uint32_t row = __float_as_uint(__ldg(sc.irec + (size_t)inst * 8 + 7).z);
+        if (row != RT_INVALID_ID) mtl = __ldg(sc.mtl_map + row + mtl);
+    }
     f3 geometry_normal = mk3(r1.w, r2.w, r3.w);       // normalize(cross(p2-p1, p3-p1)), precomputed at upload
     float w0 = 1.0f - u - v;
     f3 position = p1 * w0 + p2 * u + p3 * v;
@@ -1315,6 +1321,13 @@ struct rt_ctx
     struct MeshRefit { uint64_t n_nodes = 0; uint2* link = nullptr; uint32_t* leaves = nullptr; uint32_t* arrivals = nullptr; uint32_t n_leaves = 0; };
     std::vector<MeshRefit> mesh_refit;
     uint32_t* mesh_bad = nullptr;
+    // rt_set_instance_materials: the upload's material count, the assignment kept per instance index (row offset r * n_materials,
+    // or RT_INVALID_ID), the remap table in mtl_mem (mtl_cap entries; grows to at least twice its size) and its host image
+    uint64_t n_materials = 0;
+    std::vector<uint32_t> inst_mtl_row;
+    uint32_t* mtl_map = nullptr;
+    size_t mtl_cap = 0;
+    std::vector<uint32_t> mtl_host;
 
     // adaptive sampling (rt_set_adaptive_sampling): the requested setting, which rt_reset makes the active one; max_error > 0 = on.
     // The per-pixel state exists only while the active setting is on.
@@ -1372,6 +1385,7 @@ struct rt_ctx
     DevAllocs light_mem;           // the emitter and environment tables
     DevAllocs motion_mem;          // prev_pos: while object motion is on and a scene is uploaded
     DevAllocs inst_mem;            // the instance buffer of an instanced scene
+    DevAllocs mtl_mem;             // mtl_map (rt_set_instance_materials): from the first assignment that needs it to the next upload
     std::vector<std::unique_ptr<void, IpcClose>> ipc_opened;
 };
 
@@ -1650,6 +1664,7 @@ DevInstScene inst_scene(const rt_ctx* c)
     static_cast<DevScene&>(s) = c->scene;
     s.inst_hdr = c->inst_hdr; s.top = c->inst_top; s.irec = c->inst_rec; s.ibase = c->inst_base;
     s.prev_tri = c->prev_pos;
+    s.mtl_map = c->mtl_map;
     return s;
 }
 
@@ -2105,6 +2120,8 @@ static int upload_scene(rt_ctx* c, const RtSceneDesc* s, const RtMeshDesc* meshe
     c->inst_mem.clear(); c->inst_hdr = c->inst_top = c->inst_rec = c->inst_prev = nullptr; c->inst_base = nullptr;
     c->inst_cap = c->n_inst = 0; c->inst_last.clear(); c->inst_list.clear();
     c->mesh_refit.clear(); c->mesh_bad = nullptr;
+    c->mtl_mem.clear(); c->mtl_map = nullptr; c->mtl_cap = 0; c->inst_mtl_row.clear();
+    c->n_materials = s->n_materials;
     for (uint32_t k = 0; k < (meshes ? n_meshes : 0u); ++k) { rt_ctx::MeshRefit r; r.n_nodes = meshes[k].n_nodes; c->mesh_refit.push_back(r); }
     if (c->instanced && (rc = alloc_instances(c, 1))) return rc;          // no instances yet: every ray misses
     if (c->object_motion && (rc = set_prev_positions(c))) return rc;
@@ -2179,6 +2196,8 @@ int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
     top_level_image(pr, n, h.data());
     float4* rec = &h[3 + top * 4];
     memcpy(rec, pr.rec.data(), pr.rec.size() * 4);
+    for (uint32_t i = 0; i < n; ++i)              // the material row of index i in the kept assignment (rt_set_instance_materials)
+        rec[(size_t)i * 8 + 7].z = rtinst::int_bits((int)(i < c->inst_mtl_row.size() ? c->inst_mtl_row[i] : RT_INVALID_ID));
     float4* prev = rec + (size_t)c->inst_cap * 8;
     // previous transforms: index i's transform in the last earlier list that had index i, else its new one
     const size_t known = c->inst_last.size() / 12;
@@ -2191,6 +2210,60 @@ int rt_set_instances(rt_ctx* c, const RtInstance* instances, uint32_t n)
     for (uint32_t i = 0; i < n; ++i) memcpy(&c->inst_last[(size_t)i * 12], instances[i].object_to_world, 48);
     c->inst_list.assign(instances, instances + n);
     c->n_inst = n;
+    return RT_OK;
+}
+
+// ---- per-instance materials: rt_set_instance_materials (include/rt_b200.h)
+
+int rt_set_instance_materials(rt_ctx* c, const uint32_t* remaps, uint32_t n_remaps, const uint32_t* remap_of_instance, uint32_t n_instances)
+{
+    const char* what = "rt_set_instance_materials";
+    RT_CHECK_CTX(c); RT_FANOUT(c, rt_set_instance_materials(k, remaps, n_remaps, remap_of_instance, n_instances));
+    if (!c->scene_ready || !c->instanced) RT_FAIL(c, RT_ERR_NOT_READY, "%s: no instanced scene (rt_upload_instanced_scene)", what);
+    if (n_remaps && !remaps) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: null remaps", what);
+    if (n_instances && !remap_of_instance) RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: null remap_of_instance", what);
+    const uint64_t nm = c->n_materials;
+    if (n_remaps && nm > 0xFFFFFFFEull / n_remaps)          // n_remaps * nm >= 2^32 - 1, without overflow
+        RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: %u rows of %llu materials reach 2^32 - 1 entries", what, n_remaps, (unsigned long long)nm);
+    const size_t entries = (size_t)n_remaps * nm;
+    for (size_t e = 0; e < entries; ++e)
+        if (remaps[e] >= nm)
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: row %llu maps material %llu to %u of %llu", what, (unsigned long long)(e / nm),
+                    (unsigned long long)(e % nm), remaps[e], (unsigned long long)nm);
+    for (uint32_t i = 0; i < n_instances; ++i)
+        if (remap_of_instance[i] >= n_remaps && remap_of_instance[i] != RT_INVALID_ID)
+            RT_FAIL(c, RT_ERR_INVALID_ARGUMENT, "%s: instance %u names row %u of %u", what, i, remap_of_instance[i], n_remaps);
+    RT_CUDA(c, cudaSetDevice(c->device));
+    { int rc = join_shadow(c); if (rc) return rc; }     // a deferred shadow pass reads the instance records this call rewrites
+    if (entries > c->mtl_cap)
+    {   // a larger table (at least twice the old, as the instance buffer grows); frames in flight read the old one.  The launch
+        // arguments change, so a captured frame graph is re-captured.
+        RT_CUDA(c, cudaStreamSynchronize(c->stream));
+        const size_t cap = std::max(entries, 2 * c->mtl_cap);
+        DevAllocs g;
+        uint32_t* p = nullptr;
+        RT_CUDA(c, g.alloc(p, cap));
+        c->mtl_mem = std::move(g); c->mtl_map = p; c->mtl_cap = cap;
+        ++c->config_gen;
+    }
+    // the table and the record words, each one copy in render-stream order from the context's own host images (pageable, so
+    // staged before the call returns; the caller's arrays may be pinned, and are not read after it)
+    if (entries)
+    {
+        c->mtl_host.assign(remaps, remaps + entries);
+        RT_CUDA(c, cudaMemcpyAsync(c->mtl_map, c->mtl_host.data(), entries * 4, cudaMemcpyHostToDevice, c->stream));
+    }
+    c->inst_mtl_row.resize(n_instances);
+    for (uint32_t i = 0; i < n_instances; ++i)
+        c->inst_mtl_row[i] = remap_of_instance[i] == RT_INVALID_ID ? RT_INVALID_ID : (uint32_t)(remap_of_instance[i] * nm);
+    if (c->n_inst)
+    {   // the instance records of the current list, as rt_set_instances wrote them but for the row offsets
+        const size_t top = (size_t)std::max(c->inst_cap, 2u) - 1u;
+        float4* rec = &c->inst_host[3 + top * 4];
+        for (uint32_t i = 0; i < c->n_inst; ++i)
+            rec[(size_t)i * 8 + 7].z = rtinst::int_bits((int)(i < n_instances ? c->inst_mtl_row[i] : RT_INVALID_ID));
+        RT_CUDA(c, cudaMemcpyAsync(c->inst_rec, rec, (size_t)c->n_inst * 8 * 16, cudaMemcpyHostToDevice, c->stream));
+    }
     return RT_OK;
 }
 

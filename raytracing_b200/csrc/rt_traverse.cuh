@@ -34,9 +34,12 @@ struct DevInstScene : DevScene
                                    // (slack a, slack b, -, -) of rt_instances.h
     const float4* top;             // top-level records (rt_bvh_layout.h layout, leaf ref = ~instance), rt_instances.h
     const float4* irec;            // 8 float4 per instance: W rows, M rows, (mesh root ref, mesh record base in float4, first
-                                   // triangle, base) as int bits, (det sign, first node bits, -, -)
+                                   // triangle, base) as int bits, (det sign, first node bits, material row offset, -): the row
+                                   // offset r * n_materials of rt_set_instance_materials as uint bits, RT_INVALID_ID for none
     const uint32_t* ibase;         // base (first virtual triangle id) per instance, ascending
     const float4* prev_tri;        // RT_OPT_OBJECT_MOTION: the previous positions of every mesh triangle (tris_ref layout); else nullptr
+    const uint32_t* mtl_map;       // rt_set_instance_materials: the remap rows, row offset + scene material id -> material id;
+                                   // nullptr before the first assignment (every row offset is then RT_INVALID_ID)
 };
 template <bool INST> using SceneOf = typename std::conditional<INST, DevInstScene, DevScene>::type;
 

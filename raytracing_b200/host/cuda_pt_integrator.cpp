@@ -180,6 +180,12 @@ void CUDAPathTraceIntegrator::UpdateMeshTriangles(std::uint32_t mesh, const RtTr
     Check(rt_update_mesh_triangles(ctx_, mesh, triangles, count), "UpdateMeshTriangles");
 }
 
+void CUDAPathTraceIntegrator::SetInstanceMaterials(const std::uint32_t* remaps, std::uint32_t n_remaps, const std::uint32_t* remap_of_instance,
+                                                   std::uint32_t n_instances)
+{
+    Check(rt_set_instance_materials(ctx_, remaps, n_remaps, remap_of_instance, n_instances), "SetInstanceMaterials");
+}
+
 std::uint64_t CUDAPathTraceIntegrator::RebuildBvh(BvhBuild build)
 {
     std::uint64_t n_nodes = 0;

@@ -116,6 +116,10 @@ public:
     // mesh update in an instanced scene (rt_update_mesh_triangles): new triangles for one mesh (its leaf order, same count); its
     // tree is refit on the device and the top-level tree rebuilt.  No reset, as for UpdateTriangles.
     void UpdateMeshTriangles(std::uint32_t mesh, const RtTriangle* triangles, size_t count);
+    // per-instance materials (rt_set_instance_materials): n_remaps rows of one entry per scene material, and the row of each
+    // instance index (RT_INVALID_ID: the mesh's own materials); replaces the assignment.  No reset, as for SetInstances.
+    void SetInstanceMaterials(const std::uint32_t* remaps, std::uint32_t n_remaps, const std::uint32_t* remap_of_instance,
+                              std::uint32_t n_instances);
     rt_ctx* Context() const { return ctx_; }
 
 protected:

@@ -229,6 +229,12 @@ int rth_render_update_mesh_triangles(void* h, std::uint32_t mesh, const RtTriang
     try { ((RenderHandle*)h)->render->UpdateMeshTriangles(mesh, triangles, count); return 0; }
     catch (std::exception& e) { g_error = e.what(); return -1; }
 }
+int rth_render_set_instance_materials(void* h, const std::uint32_t* remaps, std::uint32_t n_remaps, const std::uint32_t* remap_of_instance,
+                                      std::uint32_t n_instances)
+{
+    try { ((RenderHandle*)h)->render->SetInstanceMaterials(remaps, n_remaps, remap_of_instance, n_instances); return 0; }
+    catch (std::exception& e) { g_error = e.what(); return -1; }
+}
 int rth_render_rebuild_bvh(void* h, std::uint64_t* n_nodes)
 {
     try { *n_nodes = ((RenderHandle*)h)->render->RebuildBvh(); return 0; }

@@ -72,6 +72,11 @@ public:
     void SetInstances(const RtInstance* instances, std::uint32_t count) { Cuda().SetInstances(instances, count); }
     // mesh update in an instanced scene (CUDAPathTraceIntegrator::UpdateMeshTriangles); keeps the accumulation, as UpdateTriangles
     void UpdateMeshTriangles(std::uint32_t mesh, const RtTriangle* triangles, size_t count) { Cuda().UpdateMeshTriangles(mesh, triangles, count); }
+    // per-instance materials (CUDAPathTraceIntegrator::SetInstanceMaterials); keeps the accumulation, as SetInstances
+    void SetInstanceMaterials(const std::uint32_t* remaps, std::uint32_t n_remaps, const std::uint32_t* remap_of_instance, std::uint32_t n_instances)
+    {
+        Cuda().SetInstanceMaterials(remaps, n_remaps, remap_of_instance, n_instances);
+    }
     std::uint32_t ActivePixels() const { return static_cast<CUDAPathTraceIntegrator const&>(*integrator_).ActivePixels(); }
     void NotifyCameraChanged() { camera_changed_ = true; }
 

@@ -54,6 +54,7 @@ def load_library():
     L.rth_render_upload_instanced_scene.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32]
     L.rth_render_set_instances.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.rth_render_update_mesh_triangles.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
+    L.rth_render_set_instance_materials.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
     L.rth_render_rebuild_bvh_ploc.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.rth_render_active_pixels.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
     L.rth_render_enable_white_furnace.argtypes = [C.c_void_p, C.c_int]
@@ -288,6 +289,15 @@ class HostRender:
         texcoords; its tree is refit on the device.  Keeps the accumulation (request_reset() starts over)."""
         t = np.ascontiguousarray(triangles, dtype=TRIANGLE_DT)
         if self.L.rth_render_update_mesh_triangles(self.h, int(mesh), t.ctypes.data, t.shape[0]) != 0:
+            raise _err(self.L)
+
+    def set_instance_materials(self, remaps, remap_of_instance):
+        """Render::SetInstanceMaterials: remaps (n_remaps, n_materials) rows, remap_of_instance the row of each instance index
+        (-1 / None: its mesh's own materials), as capi.Context.set_instance_materials.  Keeps the accumulation."""
+        from .capi import instance_material_arrays
+        rows, of = instance_material_arrays(remaps, remap_of_instance)
+        if self.L.rth_render_set_instance_materials(self.h, rows.ctypes.data if rows.size else None, rows.shape[0],
+                                                    of.ctypes.data if of.size else None, len(of)) != 0:
             raise _err(self.L)
 
     def rebuild_bvh(self, method="linear"):

@@ -18,8 +18,17 @@ triangles, under 183 instances) by the host variant (a TRIANGLE_DT array) and by
 clock around --calls calls, each returning after its blocking root-box read-back and followed by rt_sync; the time of a 32-byte
 device-to-host copy with its synchronise, the read-back's floor; and ms per frame after a deforming update (refit tree) against a
 fresh context that uploaded the same triangles and refit nodes (tests/refit_model.py) with the same instance list.
+
+  python tools/instance_probe.py --materials [--width ... --frames ... --warmup ... --repeats 5] [--out FILE]
+
+Per-instance materials in the instanced field (rt_set_instance_materials) instead, three arms on one context, alternated --repeats
+times: no assignment; every instance with its own row (a seeded permutation of the scene's materials); every instance with the
+identity row.  ms per frame of each repeat from CUDA events; the identity arm's radiance is checked to equal the first arm's bits.
+With RT_B200_LIB naming a library built from a commit before rt_set_instance_materials, only the first arm runs (the parent's
+frame time on the same scene).
 """
 import argparse
+import hashlib
 import json
 import os
 import subprocess
@@ -64,6 +73,8 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--mesh-update", action="store_true")
     ap.add_argument("--calls", type=int, default=20)
+    ap.add_argument("--materials", action="store_true")
+    ap.add_argument("--repeats", type=int, default=5)
     args = ap.parse_args()
     import torch
     torch.cuda.init()
@@ -71,6 +82,10 @@ def main():
     lines = [{"gpu": gpu_info()}]
     if args.mesh_update:
         lines += mesh_update(args, base)
+        emit(lines, args.out)
+        return
+    if args.materials:
+        lines += instance_materials(args, base)
         emit(lines, args.out)
         return
 
@@ -169,6 +184,37 @@ def mesh_update(args, base):
     c.destroy()
     out.append({"frame": f"{args.width}x{args.height}x{args.bounces}", "ms_per_frame_after_update": [upd, upd2],
                 "ms_per_frame_fresh_upload": fresh})
+    return out
+
+
+def instance_materials(args, base):
+    fld = synthetic.instanced_field(base, copies=args.copies, width=args.width, height=args.height)
+    ids, n_mat = fld["mesh_ids"], len(base["materials"])
+    rng = np.random.default_rng(7)
+    own = np.stack([rng.permutation(n_mat) for _ in ids]).astype(np.uint32)
+    arms = {"none": ([], []), "own_rows": (own, list(range(len(ids)))),
+            "identity_rows": (np.arange(n_mat, dtype=np.uint32)[None], [0] * len(ids))}
+    c = capi.Context(args.width, args.height)
+    c.set_camera(fld["camera_pose"])
+    c.upload_instanced_scene(fld["meshes"], fld["shared"])
+    c.set_instances(ids, fld["transforms"])
+    if not hasattr(capi.load_library(), "rt_set_instance_materials"):
+        arms = {"none": arms["none"]}
+    ms = {k: [] for k in arms}
+    image = {}
+    for _ in range(args.repeats):
+        for arm, (rows, of) in arms.items():
+            if len(arms) > 1:
+                c.set_instance_materials(rows, of)
+            ms[arm].append(timed_frames(c, args.bounces, args.frames, args.warmup))
+            image.setdefault(arm, c.read_radiance()[..., :3].view(np.uint32).copy())
+    c.destroy()
+    out = [{"arm": arm, "instances": len(ids), "materials": n_mat, "ms_per_frame": v, "median": float(np.median(v)),
+            "spread": float(max(v) - min(v)), "frame": f"{args.width}x{args.height}x{args.bounces}"} for arm, v in ms.items()]
+    if len(arms) > 1:
+        out.append({"identity_rows_equal_none": bool(np.array_equal(image["identity_rows"], image["none"])),
+                    "own_rows_differ": bool(not np.array_equal(image["own_rows"], image["none"]))})
+    out.append({"library": capi.LIB_PATH, "none_radiance_sha1": hashlib.sha1(image["none"].tobytes()).hexdigest()})
     return out
 
 
